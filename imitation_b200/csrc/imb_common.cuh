@@ -274,3 +274,66 @@ __device__ __forceinline__ float sigmoid_f(float x) {
   float e = expf(x);
   return e / (1.0f + e);
 }
+
+// RunningNorm.update_stats (util/networks.py:121-134): fold the moments of a batch of b_n rows (mean, biased variance)
+// into the running (mean, var) of `cnt` rows
+__device__ __forceinline__ void norm_fold(float& mean, float& var, float cnt, float b_mean, float b_var, float b_n) {
+  const float tot = cnt + b_n;
+  const float delta = b_mean - mean;
+  mean += delta * b_n / tot;
+  var *= cnt;
+  var += b_var * b_n;
+  var += delta * delta * cnt * b_n / tot;
+  var /= tot;
+}
+
+// exact two-pass (mean, M2) of x[0, n), n >= 1, by one warp; every lane receives the result
+__device__ __forceinline__ void warp_moments(const float* x, int n, int lane, float& mean, float& m2) {
+  float s = 0.f;
+  for (int i = lane; i < n; i += 32) s += x[i];
+  mean = warp_sum(s) / (float)n;
+  m2 = 0.f;
+  for (int i = lane; i < n; i += 32) {
+    const float dlt = x[i] - mean;
+    m2 = fmaf(dlt, dlt, m2);
+  }
+  m2 = warp_sum(m2);
+}
+
+// Chan et al. merge of the moments (count, mean, M2) of `nchunks` chunks, chunk c's at cnt[c * stride],
+// mean[c * stride] and m2[c * stride], by one warp: every lane merges its chunks (lane, lane + 32, ...) in index
+// order, then the 32 lane results are merged by a fixed butterfly, so the result is deterministic and every lane
+// receives it (a single thread walking all chunks cost more than the statistics themselves once the chunks became
+// small enough to fill the GPU).  The chunk moments were written by other blocks of the same launch: read past L1.
+__device__ __forceinline__ void warp_chan_merge(const float* cnt, const float* mean, const float* m2, int64_t stride,
+                                                int nchunks, int lane, float& n_out, float& mean_out, float& m2_out) {
+  float na = 0.f, ma = 0.f, m2a = 0.f;
+  for (int c = lane; c < nchunks; c += 32) {
+    const int64_t o = (int64_t)c * stride;
+    const float nb = __ldcg(cnt + o), mb = __ldcg(mean + o), m2b = __ldcg(m2 + o);
+    const float nt = na + nb;
+    const float dlt = mb - ma;
+    ma = ma + dlt * (nb / nt);
+    m2a = m2a + m2b + dlt * dlt * (na * nb / nt);
+    na = nt;
+  }
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const float nb = __shfl_xor_sync(0xffffffffu, na, o), mb = __shfl_xor_sync(0xffffffffu, ma, o),
+                m2b = __shfl_xor_sync(0xffffffffu, m2a, o);
+    // merge (lower lane, higher lane) in that order on both sides so the pair agrees bit for bit
+    const bool lowme = (lane & o) == 0;
+    const float n1 = lowme ? na : nb, m1 = lowme ? ma : mb, q1 = lowme ? m2a : m2b;
+    const float n2 = lowme ? nb : na, m2v = lowme ? mb : ma, q2 = lowme ? m2b : m2a;
+    const float nt = n1 + n2;
+    if (nt > 0.f) {
+      const float dlt = m2v - m1;
+      ma = m1 + dlt * (n2 / nt);
+      m2a = q1 + q2 + dlt * dlt * (n1 * n2 / nt);
+    }
+    na = nt;
+  }
+  n_out = na;
+  mean_out = ma;
+  m2_out = m2a;
+}

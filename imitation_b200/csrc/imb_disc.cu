@@ -7,8 +7,9 @@
 //
 // Kernel plan (no spinning grid barriers -- every dependency is a kernel boundary or the
 // "last block done" ticket, so a bug cannot hang the GPU):
-//   k_norm_stats   per-chunk (n, mean, M2) per input feature; last CTA Chan-merges the chunks in
-//                  fixed order into the running stats (RunningNorm.update_stats).
+//   k_norm_stats   per-chunk (n, mean, M2) per input feature of 1-3 normaliser updates (blockIdx.y = job);
+//                  the last CTA Chan-merges each job's chunks in fixed order and folds the jobs, in order,
+//                  into their running stats (RunningNorm.update_stats).
 //   k_disc_fwdbwd  persistent CTAs over 128-row tiles of the feature-major batch.  The tile is
 //                  staged [feature][row] into shared memory by cp.async.bulk (TMA unit) with a
 //                  2-stage mbarrier pipeline.  Phase A (thread per row): normalise, MLP forward,
@@ -16,8 +17,10 @@
 //                  Phase B (warps split output columns): the three weight-gradient contractions
 //                  dW = D^T . Act over the tile, accumulated in shared memory across tiles.
 //                  Weights (<34 KB) stay in shared memory; activations never touch HBM.
-//   k_disc_reduce  warp-per-parameter deterministic sum of the per-CTA partials.
+//   k_disc_reduce  warp-per-parameter deterministic sum of the per-CTA partials (G = meta[0], written by
+//                  the fwd/bwd kernel).
 //   k_disc_adam    torch.optim.Adam step + the 9 train statistics.
+//   k_disc_reduce_adam  both in one launch: the last block (ticket) runs the Adam step and the statistics.
 #include <stdlib.h>
 
 #include "imb_common.cuh"
@@ -32,6 +35,7 @@ extern "C" const char* imb_last_error(void) { return g_imb_err; }
 namespace {
 
 constexpr int NORM_CHUNK = 512;       // rows per CTA in k_norm_stats
+constexpr int NORM_PS = 2 * IMB_MAX_DIN + 4;  // floats per chunk record of k_norm_stats: mean | M2 | n
 constexpr int MAXG = 296;             // max CTAs of k_disc_fwdbwd (2 per SM)
 
 // ---- workspace layout (floats) -----------------------------------------------------------------
@@ -41,7 +45,7 @@ struct WsLayout {
   int64_t meta;      // [16] ints: grid of the last fwdbwd launch, n rows, n_expert
   int64_t snap;      // [2*IMB_MAX_DIN] potential-norm stats after the first (next_obs) update
   int64_t ticket;    // [16] uint tickets
-  int64_t normpart;  // [MAXCHUNKS][2*IMB_MAX_DIN + 4]
+  int64_t normpart;  // [MAXCHUNKS][NORM_PS]
   int64_t partial;   // [MAXG][P + 16]
   int64_t total;
 };
@@ -61,7 +65,7 @@ inline WsLayout ws_layout(int P) {
   w.ticket = o;
   o += 32;
   w.normpart = o;
-  o += (int64_t)MAXCHUNKS * (2 * IMB_MAX_DIN + 4);
+  o += (int64_t)MAXCHUNKS * NORM_PS;
   w.partial = o;
   o += (int64_t)MAXG * part_stride(P);
   w.total = o;
@@ -69,37 +73,40 @@ inline WsLayout ws_layout(int P) {
 }
 
 // ---- RunningNorm statistics ----------------------------------------------------------------------
-struct NormLaunch {
+// One or more RunningNorm updates over the same batch rows (AIRL: the base net's normaliser and the potential's, the
+// latter updated twice: first with next_obs, then with obs -- reward_nets.py:708-710).
+struct NormJob {
   int din;
   short row[IMB_MAX_DIN];  // batch feature rows
+  float* rmv;              // running [mean | var] of the job's normaliser
+  int32_t* cnt;
+  float* snap;             // optional copy of the statistics after this job's fold
+};
+struct NormJobs {
+  int njobs;  // 1..3
+  NormJob job[3];
 };
 
-// One CTA per NORM_CHUNK rows; warp w handles features w, w+nw, ...: exact two-pass (mean, M2)
-// inside the chunk, then the last CTA to finish merges all chunks in index order (Chan et al.)
-// and folds the batch into the running statistics exactly as util/networks.py:111-134 does.
-__global__ void __launch_bounds__(256) k_norm_stats(NormLaunch L, const float* __restrict__ batch, int64_t ld,
-                                                    int64_t n, int chunk_rows, float* __restrict__ run_mean_var,
-                                                    int32_t* __restrict__ count, float* __restrict__ snap_out,
-                                                    float* __restrict__ part, unsigned int* __restrict__ ticket,
-                                                    float* __restrict__ defer = nullptr, int defer_cap = 0) {
+// blockIdx.y = job, blockIdx.x = chunk of chunk_rows rows; warp w handles features w, w+nw, ...: exact two-pass
+// (mean, M2) inside the chunk.  The last CTA of the whole grid Chan-merges each job's chunks in index order and folds
+// the jobs into their running statistics IN JOB ORDER (two jobs may share a normaliser), exactly as
+// util/networks.py:111-134 does.  Deferred mode (`defer`): the batch moments go to the next free slot of `defer`
+// ([0] = slot counter, slots of 2 * din + 1 floats: mean | biased variance | n) instead of into the running
+// statistics; k_norm_fold applies them later, in order.  Six resident CTAs per SM hold it at 40 registers (left
+// alone, ptxas spends 60 on the unrolled chunk merge).
+__global__ void __launch_bounds__(256, 6) k_norm_stats(NormJobs J, const float* __restrict__ batch, int64_t ld,
+                                                       int64_t n, int chunk_rows, float* __restrict__ part,
+                                                       unsigned int* __restrict__ ticket, float* __restrict__ defer,
+                                                       int defer_cap) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+  const int nchunks = gridDim.x;
+  const NormJob& L = J.job[blockIdx.y];
   const int64_t r0 = (int64_t)blockIdx.x * chunk_rows;
-  const int64_t r1 = min(n, r0 + (int64_t)chunk_rows);
-  const int cn = (int)(r1 - r0);
-  const int PS = 2 * IMB_MAX_DIN + 4;
-  float* my = part + (int64_t)blockIdx.x * PS;
+  const int cn = (int)(min(n, r0 + (int64_t)chunk_rows) - r0);
+  float* my = part + ((int64_t)blockIdx.y * nchunks + blockIdx.x) * NORM_PS;
   for (int k = warp; k < L.din; k += nw) {
-    const float* src = batch + (int64_t)L.row[k] * ld + r0;
-    float s = 0.f;
-    for (int i = lane; i < cn; i += 32) s += src[i];
-    s = warp_sum(s);
-    const float mean = s / (float)cn;
-    float m2 = 0.f;
-    for (int i = lane; i < cn; i += 32) {
-      float dlt = src[i] - mean;
-      m2 = fmaf(dlt, dlt, m2);
-    }
-    m2 = warp_sum(m2);
+    float mean, m2;
+    warp_moments(batch + (int64_t)L.row[k] * ld + r0, cn, lane, mean, m2);
     if (lane == 0) {
       my[k] = mean;
       my[IMB_MAX_DIN + k] = m2;
@@ -109,88 +116,54 @@ __global__ void __launch_bounds__(256) k_norm_stats(NormLaunch L, const float* _
   __threadfence();
   __shared__ bool is_last;
   __syncthreads();
-  if (threadIdx.x == 0) {
-    unsigned int t = atomicAdd(ticket, 1u);
-    is_last = (t == gridDim.x - 1);
-  }
+  if (threadIdx.x == 0) is_last = atomicAdd(ticket, 1u) == gridDim.x * gridDim.y - 1;
   __syncthreads();
   if (!is_last) return;
   __threadfence();
-  // deferred mode: the batch moments go to the next free slot of `defer` ([0] = slot counter, slots of 2 * din + 1
-  // floats: mean | biased variance | n) instead of into the running statistics; k_norm_fold applies them later, in order
-  float* slot = nullptr;
-  if (defer) {
-    int k = (int)defer[0];
-    if (k >= defer_cap) k = defer_cap - 1;  // (host folds long before this; never overrun)
-    slot = defer + 4 + (int64_t)k * (2 * L.din + 1);
-  }
-  const int32_t old_count = defer ? 0 : *count;
-  // warp per feature: every lane Chan-merges its chunks (lane, lane + 32, ...) in index order, then the 32 lane
-  // results are merged by a fixed butterfly (deterministic; a single thread walking all chunks cost more than
-  // the statistics themselves once the chunks became small enough to fill the GPU)
-  for (int k = warp; k < L.din; k += nw) {
-    float na = 0.f, ma = 0.f, m2a = 0.f;
-    for (unsigned int c = lane; c < gridDim.x; c += 32) {
-      const float* p = part + (int64_t)c * PS;
-      const float nb = __ldcg(p + 2 * IMB_MAX_DIN), mb = __ldcg(p + k), m2b = __ldcg(p + IMB_MAX_DIN + k);
-      const float nt = na + nb;
-      const float dlt = mb - ma;
-      ma = ma + dlt * (nb / nt);
-      m2a = m2a + m2b + dlt * dlt * (na * nb / nt);
-      na = nt;
+  for (int jb = 0; jb < J.njobs; ++jb) {
+    const NormJob& Lj = J.job[jb];
+    const float* jpart = part + (int64_t)jb * nchunks * NORM_PS;
+    float* slot = nullptr;
+    if (defer) {
+      int s = (int)defer[0];
+      if (s >= defer_cap) s = defer_cap - 1;  // (host folds long before this; never overrun)
+      slot = defer + 4 + (int64_t)s * (2 * Lj.din + 1);
     }
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const float nb = __shfl_xor_sync(0xffffffffu, na, o), mb = __shfl_xor_sync(0xffffffffu, ma, o),
-                  m2b = __shfl_xor_sync(0xffffffffu, m2a, o);
-      // merge (lower lane, higher lane) in that order on both sides so the pair agrees bit for bit
-      const bool lowme = (lane & o) == 0;
-      const float n1 = lowme ? na : nb, m1 = lowme ? ma : mb, q1 = lowme ? m2a : m2b;
-      const float n2 = lowme ? nb : na, m2v = lowme ? mb : ma, q2 = lowme ? m2b : m2a;
-      const float nt = n1 + n2;
-      if (nt > 0.f) {
-        const float dlt = m2v - m1;
-        ma = m1 + dlt * (n2 / nt);
-        m2a = q1 + q2 + dlt * dlt * (n1 * n2 / nt);
-      }
-      na = nt;
-    }
-    if (lane == 0 && slot) {
-      slot[k] = ma;
-      slot[L.din + k] = m2a / na;
-    } else if (lane == 0) {
-      const float b_mean = ma, b_var = m2a / na, b_n = na;
-      float mean = run_mean_var[k], var = run_mean_var[L.din + k];
-      const float cnt = (float)old_count;
-      const float tot = cnt + b_n;
-      const float delta = b_mean - mean;
-      mean += delta * b_n / tot;
-      var *= cnt;
-      var += b_var * b_n;
-      var += delta * delta * cnt * b_n / tot;
-      var /= tot;
-      run_mean_var[k] = mean;
-      run_mean_var[L.din + k] = var;
-      if (snap_out) {
-        snap_out[k] = mean;
-        snap_out[L.din + k] = var;
+    const int32_t old_count = defer ? 0 : *Lj.cnt;
+    for (int k = warp; k < Lj.din; k += nw) {
+      float b_n, b_mean, b_m2;
+      warp_chan_merge(jpart + 2 * IMB_MAX_DIN, jpart + k, jpart + IMB_MAX_DIN + k, NORM_PS, nchunks, lane, b_n, b_mean,
+                      b_m2);
+      if (lane == 0 && slot) {
+        slot[k] = b_mean;
+        slot[Lj.din + k] = b_m2 / b_n;
+      } else if (lane == 0) {
+        float mean = Lj.rmv[k], var = Lj.rmv[Lj.din + k];
+        norm_fold(mean, var, (float)old_count, b_mean, b_m2 / b_n, b_n);
+        Lj.rmv[k] = mean;
+        Lj.rmv[Lj.din + k] = var;
+        if (Lj.snap) {
+          Lj.snap[k] = mean;
+          Lj.snap[Lj.din + k] = var;
+        }
       }
     }
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    if (slot) {
-      slot[2 * L.din] = (float)n;
-      defer[0] += 1.0f;
-    } else {
-      *count = old_count + (int32_t)n;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      if (slot) {
+        slot[2 * Lj.din] = (float)n;
+        defer[0] += 1.0f;
+      } else {
+        *Lj.cnt = old_count + (int32_t)n;
+      }
     }
-    *ticket = 0u;  // re-arm for the next launch
+    __syncthreads();  // the next job may fold into the same normaliser: count and statistics are in place
   }
+  if (threadIdx.x == 0) *ticket = 0u;  // re-arm for the next launch
 }
 
 // fold the deferred batch moments into the running statistics, slot by slot, with RunningNorm.update_stats'
-// arithmetic (util/networks.py:121-134) -- the same expressions as the in-kernel fold of k_norm_stats
+// arithmetic (util/networks.py:121-134)
 __global__ void k_norm_fold(int din, float* __restrict__ defer, float* __restrict__ run_mean_var,
                             int32_t* __restrict__ count, int k_fixed) {
   const int K = k_fixed > 0 ? k_fixed : (int)defer[0];
@@ -201,15 +174,8 @@ __global__ void k_norm_fold(int din, float* __restrict__ defer, float* __restric
     int32_t c = cnt_i;
     for (int sidx = 0; sidx < K; ++sidx) {
       const float* slot = defer + 4 + (int64_t)sidx * (2 * din + 1);
-      const float b_mean = slot[k], b_var = slot[din + k], b_n = slot[2 * din];
-      const float cnt = (float)c;
-      const float tot = cnt + b_n;
-      const float delta = b_mean - mean;
-      mean += delta * b_n / tot;
-      var *= cnt;
-      var += b_var * b_n;
-      var += delta * delta * cnt * b_n / tot;
-      var /= tot;
+      const float b_n = slot[2 * din];
+      norm_fold(mean, var, (float)c, slot[k], slot[din + k], b_n);
       c += (int32_t)b_n;
     }
     run_mean_var[k] = mean;
@@ -221,112 +187,6 @@ __global__ void k_norm_fold(int din, float* __restrict__ defer, float* __restric
     *count = cnt_i;
     if (k_fixed <= 0) defer[0] = 0.f;
   }
-}
-
-// Several RunningNorm updates in ONE launch (AIRL: the base net's normaliser and the potential's, the latter updated twice:
-// first with next_obs, then with obs -- reward_nets.py:708-710).  blockIdx.y = job; every CTA computes the (mean, M2) of its
-// chunk of its job's rows; the last CTA of the whole grid Chan-merges each job's chunks and folds the jobs into their
-// running statistics IN JOB ORDER (two jobs may share a normaliser; `snap` receives the statistics right after a job's fold).
-struct NormJobs {
-  int njobs;
-  NormLaunch job[3];
-  float* rmv[3];       // running [mean | var] of the job's normaliser
-  int32_t* cnt[3];
-  float* snap[3];      // optional copy of the statistics after this job's fold
-};
-__global__ void __launch_bounds__(256) k_norm_stats_multi(NormJobs J, const float* __restrict__ batch, int64_t ld, int64_t n,
-                                                          int chunk_rows, float* __restrict__ part,
-                                                          unsigned int* __restrict__ ticket) {
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
-  const int jb = blockIdx.y, nchunks = gridDim.x;
-  const NormLaunch& L = J.job[jb];
-  const int64_t r0 = (int64_t)blockIdx.x * chunk_rows;
-  const int64_t r1 = min(n, r0 + (int64_t)chunk_rows);
-  const int cn = (int)(r1 - r0);
-  const int PS = 2 * IMB_MAX_DIN + 4;
-  float* my = part + ((int64_t)jb * nchunks + blockIdx.x) * PS;
-  for (int k = warp; k < L.din; k += nw) {
-    const float* src = batch + (int64_t)L.row[k] * ld + r0;
-    float s = 0.f;
-    for (int i = lane; i < cn; i += 32) s += src[i];
-    s = warp_sum(s);
-    const float mean = s / (float)cn;
-    float m2 = 0.f;
-    for (int i = lane; i < cn; i += 32) {
-      float dlt = src[i] - mean;
-      m2 = fmaf(dlt, dlt, m2);
-    }
-    m2 = warp_sum(m2);
-    if (lane == 0) {
-      my[k] = mean;
-      my[IMB_MAX_DIN + k] = m2;
-    }
-  }
-  if (threadIdx.x == 0) my[2 * IMB_MAX_DIN] = (float)cn;
-  __threadfence();
-  __shared__ bool is_last;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    unsigned int t = atomicAdd(ticket, 1u);
-    is_last = (t == gridDim.x * gridDim.y - 1);
-  }
-  __syncthreads();
-  if (!is_last) return;
-  __threadfence();
-  for (int job = 0; job < J.njobs; ++job) {  // folds in job order (a later job may read what an earlier one wrote)
-    const NormLaunch& Lj = J.job[job];
-    const int32_t old_count = *J.cnt[job];
-    float* run_mean_var = J.rmv[job];
-    for (int k = warp; k < Lj.din; k += nw) {
-      float na = 0.f, ma = 0.f, m2a = 0.f;
-      for (int c = lane; c < nchunks; c += 32) {
-        const float* p = part + ((int64_t)job * nchunks + c) * PS;
-        const float nb = __ldcg(p + 2 * IMB_MAX_DIN), mb = __ldcg(p + k), m2b = __ldcg(p + IMB_MAX_DIN + k);
-        const float nt = na + nb;
-        const float dlt = mb - ma;
-        ma = ma + dlt * (nb / nt);
-        m2a = m2a + m2b + dlt * dlt * (na * nb / nt);
-        na = nt;
-      }
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const float nb = __shfl_xor_sync(0xffffffffu, na, o), mb = __shfl_xor_sync(0xffffffffu, ma, o),
-                    m2b = __shfl_xor_sync(0xffffffffu, m2a, o);
-        const bool lowme = (lane & o) == 0;
-        const float n1 = lowme ? na : nb, m1 = lowme ? ma : mb, q1 = lowme ? m2a : m2b;
-        const float n2 = lowme ? nb : na, m2v = lowme ? mb : ma, q2 = lowme ? m2b : m2a;
-        const float nt = n1 + n2;
-        if (nt > 0.f) {
-          const float dlt = m2v - m1;
-          ma = m1 + dlt * (n2 / nt);
-          m2a = q1 + q2 + dlt * dlt * (n1 * n2 / nt);
-        }
-        na = nt;
-      }
-      if (lane == 0) {
-        const float b_mean = ma, b_var = m2a / na, b_n = na;
-        float mean = run_mean_var[k], var = run_mean_var[Lj.din + k];
-        const float cnt = (float)old_count;
-        const float tot = cnt + b_n;
-        const float delta = b_mean - mean;
-        mean += delta * b_n / tot;
-        var *= cnt;
-        var += b_var * b_n;
-        var += delta * delta * cnt * b_n / tot;
-        var /= tot;
-        run_mean_var[k] = mean;
-        run_mean_var[Lj.din + k] = var;
-        if (J.snap[job]) {
-          J.snap[job][k] = mean;
-          J.snap[job][Lj.din + k] = var;
-        }
-      }
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) *J.cnt[job] = old_count + (int32_t)n;
-    __syncthreads();  // the next job may fold into the same normaliser: count and statistics are in place
-  }
-  if (threadIdx.x == 0) *ticket = 0u;  // re-arm for the next launch
 }
 
 // ---- the fused forward / BCE / backward kernel (tiled-GEMM form, see imb_tile.cuh) ------------------
@@ -704,13 +564,14 @@ __global__ void __launch_bounds__(R, 256 / R) k_disc_fwdbwd(const DiscLaunch L, 
 #include "imb_disc_tc.cuh"
 namespace {
 
-// ---- deterministic reduction of the per-CTA partials -----------------------------------------
-// warp per parameter (and per statistic): lanes stride over the G partial rows, shuffle-reduce.
-__global__ void __launch_bounds__(256) k_disc_reduce(int P, int G, const float* __restrict__ partial,
-                                                    float* __restrict__ gacc, float* __restrict__ stats,
-                                                    float* __restrict__ grad_out_flat) {
-  // (the Adam step number is read by k_disc_adam from the device counter block; the increment is
-  //  committed by a single thread there AFTER every block has read it -- see k_disc_adam)
+// ---- deterministic reduction of the per-CTA partials, Adam step, train statistics -------------
+// The partials are those of the last fwd/bwd launch on this workspace, which records its grid size G in meta[0].
+
+// warp per parameter (and per statistic): lanes stride over the G partial rows, shuffle-reduce.  The gradient sums are
+// added to gacc (and copied to grad_out_flat), the statistic sums replace stats.
+__device__ __forceinline__ void reduce_partials(int P, const int* meta, const float* partial, float* gacc, float* stats,
+                                                float* grad_out_flat) {
+  const int G = meta[0];
   const int gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   const int nwarps = (gridDim.x * blockDim.x) >> 5;
@@ -742,14 +603,18 @@ __device__ __forceinline__ double dpowi(double b, int64_t n) {
   return r;
 }
 
-// single block: every thread reads the step counter before thread 0 commits the increment (no race,
-// no extra launch); P <= ~8.5k parameters = a handful of iterations per thread.
-__global__ void __launch_bounds__(1024) k_disc_adam(int P, imb_adam opt, float* __restrict__ params,
-                                                  float* __restrict__ m, float* __restrict__ v,
-                                                  const float* __restrict__ grad, float grad_div,
-                                                  const float* __restrict__ stats, const int* __restrict__ meta,
-                                                  int64_t* __restrict__ step_io,
-                                                  float* __restrict__ stats_out) {
+// kThisLaunch: the value was written by other blocks of the same launch, so it is read past L1
+template <bool kThisLaunch>
+__device__ __forceinline__ float ld_sum(const float* p) {
+  return kThisLaunch ? __ldcg(p) : *p;
+}
+
+// torch.optim.Adam step (AdamW's decoupled decay when weight_decay > 0) of params[0, P) by the threads of one block,
+// with gradient grad / grad_div.  Thread 0 alone reads and increments the step count; the other threads take the bias
+// corrections from shared memory (no race, no extra launch).
+template <bool kThisLaunch>
+__device__ __forceinline__ void adam_step(int P, const imb_adam& opt, float* params, float* m, float* v,
+                                          const float* grad, float grad_div, int64_t* step_io) {
   // bias corrections in double like torch's Python-scalar arithmetic (torch/optim/adam.py)
   __shared__ float s_bc[2];
   if (threadIdx.x == 0) {
@@ -763,7 +628,7 @@ __global__ void __launch_bounds__(1024) k_disc_adam(int P, imb_adam opt, float* 
   __syncthreads();
   const float step_size = s_bc[0], bc2_sqrt = s_bc[1];
   for (int i = threadIdx.x; i < P; i += blockDim.x) {
-    const float g = grad[i] / grad_div;
+    const float g = ld_sum<kThisLaunch>(grad + i) / grad_div;
     const float mi = m[i] + (g - m[i]) * (1.0f - opt.beta1);        // torch: exp_avg.lerp_(grad, 1-beta1)
     const float vi = v[i] * opt.beta2 + (1.0f - opt.beta2) * g * g;  // exp_avg_sq.mul_(b2).addcmul_(g,g,1-b2)
     m[i] = mi;
@@ -772,91 +637,64 @@ __global__ void __launch_bounds__(1024) k_disc_adam(int P, imb_adam opt, float* 
     const float pw = opt.weight_decay > 0.f ? params[i] * (1.0f - opt.lr * opt.weight_decay) : params[i];  // AdamW
     params[i] = pw - step_size * (mi / denom);
   }
-  if (blockIdx.x == 0 && threadIdx.x == 0 && stats_out) {
-    const float n = (float)meta[1], n_exp = (float)meta[2], n_gen = n - n_exp;
-    const float loss_sum = stats[0], ent_sum = stats[1], c_exp = stats[2], c_gen = stats[3], c_pred = stats[4];
-    const float nanv = __int_as_float(0x7fc00000);
-    stats_out[0] = loss_sum * reinterpret_cast<const float*>(meta)[3];                 // disc_loss (scaled minibatch mean)
-    stats_out[1] = n > 0 ? (c_exp + c_gen) / n : nanv;         // disc_acc
-    stats_out[2] = n_exp >= 1 ? c_exp / n_exp : nanv;          // disc_acc_expert
-    stats_out[3] = c_gen / fmaxf(1.f, n_gen);                  // disc_acc_gen
-    stats_out[4] = n > 0 ? ent_sum / n : nanv;                 // disc_entropy
-    stats_out[5] = n > 0 ? n_exp / n : nanv;                   // disc_proportion_expert_true
-    stats_out[6] = n > 0 ? c_pred / n : nanv;                  // disc_proportion_expert_pred
-    stats_out[7] = n_exp;
-    stats_out[8] = n_gen;
-  }
+}
+
+// the 9 train statistics of the last minibatch (common.py:27-92) from its sums and the row counts in meta; one thread
+template <bool kThisLaunch>
+__device__ __forceinline__ void train_stats(const float* stats, const int* meta, float* stats_out) {
+  const float n = (float)meta[1], n_exp = (float)meta[2], n_gen = n - n_exp;
+  const float loss_sum = ld_sum<kThisLaunch>(stats + 0), ent_sum = ld_sum<kThisLaunch>(stats + 1),
+              c_exp = ld_sum<kThisLaunch>(stats + 2), c_gen = ld_sum<kThisLaunch>(stats + 3),
+              c_pred = ld_sum<kThisLaunch>(stats + 4);
+  const float nanv = __int_as_float(0x7fc00000);
+  stats_out[0] = loss_sum * reinterpret_cast<const float*>(meta)[3];  // disc_loss (scaled minibatch mean)
+  stats_out[1] = n > 0 ? (c_exp + c_gen) / n : nanv;                  // disc_acc
+  stats_out[2] = n_exp >= 1 ? c_exp / n_exp : nanv;                   // disc_acc_expert
+  stats_out[3] = c_gen / fmaxf(1.f, n_gen);                           // disc_acc_gen
+  stats_out[4] = n > 0 ? ent_sum / n : nanv;                          // disc_entropy
+  stats_out[5] = n > 0 ? n_exp / n : nanv;                            // disc_proportion_expert_true
+  stats_out[6] = n > 0 ? c_pred / n : nanv;                           // disc_proportion_expert_pred
+  stats_out[7] = n_exp;
+  stats_out[8] = n_gen;
+}
+
+__global__ void __launch_bounds__(256) k_disc_reduce(int P, const int* __restrict__ meta,
+                                                    const float* __restrict__ partial, float* __restrict__ gacc,
+                                                    float* __restrict__ stats, float* __restrict__ grad_out_flat) {
+  reduce_partials(P, meta, partial, gacc, stats, grad_out_flat);
+}
+
+// single block: P <= ~8.5k parameters = a handful of iterations per thread
+__global__ void __launch_bounds__(1024) k_disc_adam(int P, imb_adam opt, float* __restrict__ params,
+                                                  float* __restrict__ m, float* __restrict__ v,
+                                                  const float* __restrict__ grad, float grad_div,
+                                                  const float* __restrict__ stats, const int* __restrict__ meta,
+                                                  int64_t* __restrict__ step_io,
+                                                  float* __restrict__ stats_out) {
+  adam_step<false>(P, opt, params, m, v, grad, grad_div, step_io);
+  if (threadIdx.x == 0 && stats_out) train_stats<false>(stats, meta, stats_out);
 }
 
 // reduce + Adam in one launch (the last minibatch of an update): every block reduces its share of the partials
 // like k_disc_reduce; the last block to finish (ticket) runs the optimiser step and the statistics.
-__global__ void __launch_bounds__(256) k_disc_reduce_adam(int P, int G, const float* __restrict__ partial,
+__global__ void __launch_bounds__(256) k_disc_reduce_adam(int P, const float* __restrict__ partial,
                                                          float* __restrict__ gacc, float* __restrict__ stats,
                                                          imb_adam opt, float* __restrict__ params,
                                                          float* __restrict__ m, float* __restrict__ v, float grad_div,
                                                          const int* __restrict__ meta, int64_t* __restrict__ step_io,
                                                          float* __restrict__ stats_out,
                                                          unsigned int* __restrict__ ticket) {
-  const int gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  const int nwarps = (gridDim.x * blockDim.x) >> 5;
-  const int64_t ps = part_stride(P);
-  for (int p = gw; p < P + 5; p += nwarps) {
-    float acc = 0.f;
-    for (int c = lane; c < G; c += 32) acc += partial[(int64_t)c * ps + p];
-    acc = warp_sum(acc);
-    if (lane == 0) {
-      if (p < P) gacc[p] += acc;
-      else stats[p - P] = acc;
-    }
-  }
+  reduce_partials(P, meta, partial, gacc, stats, nullptr);
   __threadfence();
   __shared__ bool is_last;
-  __shared__ float s_bc[2];
   __syncthreads();
-  if (threadIdx.x == 0) {
-    const unsigned int t = atomicAdd(ticket, 1u);
-    is_last = (t == gridDim.x - 1);
-  }
+  if (threadIdx.x == 0) is_last = atomicAdd(ticket, 1u) == gridDim.x - 1;
   __syncthreads();
   if (!is_last) return;
   __threadfence();
-  if (threadIdx.x == 0) {
-    const int64_t step = *step_io + 1;
-    const double bc1d = 1.0 - dpowi((double)opt.beta1, step);
-    const double bc2d = 1.0 - dpowi((double)opt.beta2, step);
-    s_bc[0] = (float)((double)opt.lr / bc1d);
-    s_bc[1] = (float)sqrt(bc2d);
-    *step_io = step;
-    *ticket = 0u;  // re-arm for the next launch
-  }
-  __syncthreads();
-  const float step_size = s_bc[0], bc2_sqrt = s_bc[1];
-  for (int i = threadIdx.x; i < P; i += blockDim.x) {
-    const float g = __ldcg(gacc + i) / grad_div;
-    const float mi = m[i] + (g - m[i]) * (1.0f - opt.beta1);
-    const float vi = v[i] * opt.beta2 + (1.0f - opt.beta2) * g * g;
-    m[i] = mi;
-    v[i] = vi;
-    const float denom = sqrtf(vi) / bc2_sqrt + opt.eps;
-    const float pw = opt.weight_decay > 0.f ? params[i] * (1.0f - opt.lr * opt.weight_decay) : params[i];  // AdamW
-    params[i] = pw - step_size * (mi / denom);
-  }
-  if (threadIdx.x == 0 && stats_out) {
-    const float n = (float)meta[1], n_exp = (float)meta[2], n_gen = n - n_exp;
-    const float loss_sum = __ldcg(stats + 0), ent_sum = __ldcg(stats + 1), c_exp = __ldcg(stats + 2),
-                c_gen = __ldcg(stats + 3), c_pred = __ldcg(stats + 4);
-    const float nanv = __int_as_float(0x7fc00000);
-    stats_out[0] = loss_sum * reinterpret_cast<const float*>(meta)[3];
-    stats_out[1] = n > 0 ? (c_exp + c_gen) / n : nanv;
-    stats_out[2] = n_exp >= 1 ? c_exp / n_exp : nanv;
-    stats_out[3] = c_gen / fmaxf(1.f, n_gen);
-    stats_out[4] = n > 0 ? ent_sum / n : nanv;
-    stats_out[5] = n > 0 ? n_exp / n : nanv;
-    stats_out[6] = n > 0 ? c_pred / n : nanv;
-    stats_out[7] = n_exp;
-    stats_out[8] = n_gen;
-  }
+  if (threadIdx.x == 0) *ticket = 0u;  // re-arm for the next launch
+  adam_step<true>(P, opt, params, m, v, gacc, grad_div, step_io);
+  if (threadIdx.x == 0 && stats_out) train_stats<true>(stats, meta, stats_out);
 }
 
 // ---- preference comparisons: fragment returns -> Boltzmann probability -> cross entropy (+ its gradient) -------------
@@ -927,8 +765,6 @@ __global__ void __launch_bounds__(256) k_pref_loss(const float* __restrict__ rew
   }
 }
 
-__global__ void k_state_add(int64_t* state, int idx, int64_t v) { state[idx] += v; }
-
 // statistics -> host-mapped pinned memory, followed by a sequence word (system-scope fence in between): the host polls
 // the word instead of issuing a D2H copy and synchronising on an event (one PCIe posted write burst per update)
 __global__ void k_stats_publish(const float* __restrict__ stats_dev, int n, float* host, const int64_t* __restrict__ state,
@@ -938,12 +774,6 @@ __global__ void k_stats_publish(const float* __restrict__ stats_dev, int n, floa
   __threadfence_system();
   __syncwarp();
   if (lane == 0) reinterpret_cast<volatile int*>(host)[15] = (int)state[state_idx];
-}
-__global__ void k_set_meta(int* meta, int G, int64_t n, int64_t n_expert, float loss_scale) {
-  meta[0] = G;
-  meta[1] = (int)n;
-  meta[2] = (int)n_expert;
-  reinterpret_cast<float*>(meta)[3] = loss_scale;
 }
 
 // ---- forward only (reward relabel / predict) ---------------------------------------------------
@@ -1039,13 +869,7 @@ __global__ void __launch_bounds__(1024) k_reward_norm_scan(float* __restrict__ r
     }
     __syncthreads();
     if (update) {
-      const float bvar = bc[1], bn = (float)E, c = (float)cnt, tot = c + bn;
-      const float delta = bmean - mean;
-      mean += delta * bn / tot;
-      var *= c;
-      var += bvar * bn;
-      var += delta * delta * c * bn / tot;
-      var /= tot;
+      norm_fold(mean, var, (float)cnt, bmean, bc[1], (float)E);
       cnt += (int32_t)E;
     }
     __syncthreads();
@@ -1091,90 +915,62 @@ inline int pick_H(const DiscLaunch& L) {
 
 extern "C" int64_t imb_disc_workspace_floats(const imb_disc_desc* d) { return ws_layout(d->n_params).total; }
 
-static int norm_launch(const imb_mlp& m, const short* rows, const float* batch, int64_t ld, int64_t n,
-                       float* norm_state, int32_t* norm_count, float* snap, float* ws, const WsLayout& w,
-                       cudaStream_t st) {
-  NormLaunch NL;
-  NL.din = m.din;
-  for (int k = 0; k < m.din; ++k) NL.row[k] = rows[k];
+// RunningNorm updates of J's jobs over rows [0, n) of the batch: one k_norm_stats launch, or one per job in job order
+// when the chunk table cannot hold every job's chunks
+static int norm_stats(const NormJobs& J, const float* batch, int64_t ld, int64_t n, float* ws, const WsLayout& w,
+                      cudaStream_t st, float* defer = nullptr, int defer_cap = 0) {
   // chunk size: small enough to fill the GPU at the tuned batch sizes (16 384 rows -> 128 CTAs), larger for the
   // multi-million-row sweeps so the chunk table stays bounded
   const int chunk_rows = n <= (int64_t)128 * 2048 ? 128 : NORM_CHUNK;
-  const int chunks = (int)((n + chunk_rows - 1) / chunk_rows);
+  const int64_t chunks = (n + chunk_rows - 1) / chunk_rows;
   IMB_REQUIRE(chunks >= 1 && chunks <= MAXCHUNKS, "norm update: n=%lld out of range", (long long)n);
-  k_norm_stats<<<chunks, 256, 0, st>>>(NL, batch, ld, n, chunk_rows, norm_state + m.norm_off, norm_count + m.count_idx, snap,
-                                       ws + w.normpart, reinterpret_cast<unsigned int*>(ws + w.ticket));
+  if (chunks * J.njobs > MAXCHUNKS) {
+    for (int j = 0; j < J.njobs; ++j)
+      if (int rc = norm_stats(NormJobs{1, {J.job[j]}}, batch, ld, n, ws, w, st, defer, defer_cap)) return rc;
+    return 0;
+  }
+  k_norm_stats<<<dim3((unsigned)chunks, J.njobs), 256, 0, st>>>(J, batch, ld, n, chunk_rows, ws + w.normpart,
+                                                                 reinterpret_cast<unsigned int*>(ws + w.ticket), defer,
+                                                                 defer_cap);
   IMB_CHECK_LAUNCH("k_norm_stats");
   return 0;
 }
 
 extern "C" int imb_disc_norm_update(const imb_disc_desc* d, const float* batch, int64_t ld, int64_t n,
                                     float* norm_state, int32_t* norm_count, float* ws, void* stream) {
-  cudaStream_t st = (cudaStream_t)stream;
   IMB_REQUIRE(n >= 1, "norm update needs n >= 1");
   const WsLayout w = ws_layout(d->n_params);
   DiscLaunch L;
   if (int rc = build_launch(d, norm_state, nullptr, L)) return rc;
-  short rows[IMB_MAX_DIN];
-  // shaped nets: all updates of one training forward in ONE launch (base normaliser; potential normaliser with next_obs,
-  // then with obs -- reference order, both on the same RunningNorm) when the chunk table has room for the jobs
-  if (d->shaped && d->potential.has_norm) {
-    const int chunk_rows = n <= (int64_t)128 * 2048 ? 128 : NORM_CHUNK;
-    const int chunks = (int)((n + chunk_rows - 1) / chunk_rows);
-    NormJobs J;
-    memset(&J, 0, sizeof(J));
-    int nj = 0;
-    auto add = [&](const imb_mlp& m, int pass, float* snap) {
-      J.job[nj].din = m.din;
-      for (int k = 0; k < m.din; ++k) J.job[nj].row[k] = L.stage_row[L.pass[pass].in_slot[k]];
-      J.rmv[nj] = norm_state + m.norm_off;
-      J.cnt[nj] = norm_count + m.count_idx;
-      J.snap[nj] = snap;
-      ++nj;
-    };
-    if (d->base.has_norm) add(d->base, 0, nullptr);
-    add(d->potential, 1, ws + w.snap);
-    add(d->potential, 2, nullptr);
-    J.njobs = nj;
-    if ((int64_t)chunks * nj <= MAXCHUNKS) {
-      k_norm_stats_multi<<<dim3(chunks, nj), 256, 0, st>>>(J, batch, ld, n, chunk_rows, ws + w.normpart,
-                                                           reinterpret_cast<unsigned int*>(ws + w.ticket));
-      IMB_CHECK_LAUNCH("k_norm_stats_multi");
-      return 0;
-    }
-  }
-  if (d->base.has_norm) {
-    for (int k = 0; k < d->base.din; ++k) rows[k] = L.stage_row[L.pass[0].in_slot[k]];
-    if (int rc = norm_launch(d->base, rows, batch, ld, n, norm_state, norm_count, nullptr, ws, w, st)) return rc;
-  }
+  NormJobs J = {};
+  auto add = [&](const imb_mlp& m, int pass, float* snap) {
+    NormJob& job = J.job[J.njobs++];
+    job.din = m.din;
+    for (int k = 0; k < m.din; ++k) job.row[k] = L.stage_row[L.pass[pass].in_slot[k]];
+    job.rmv = norm_state + m.norm_off;
+    job.cnt = norm_count + m.count_idx;
+    job.snap = snap;
+  };
+  if (d->base.has_norm) add(d->base, 0, nullptr);
   if (d->shaped && d->potential.has_norm) {
     // reference order: Phi(next_state) first, then Phi(state); both update the same RunningNorm
-    for (int k = 0; k < d->potential.din; ++k) rows[k] = L.stage_row[L.pass[1].in_slot[k]];
-    if (int rc = norm_launch(d->potential, rows, batch, ld, n, norm_state, norm_count, ws + w.snap, ws, w, st))
-      return rc;
-    for (int k = 0; k < d->potential.din; ++k) rows[k] = L.stage_row[L.pass[2].in_slot[k]];
-    if (int rc = norm_launch(d->potential, rows, batch, ld, n, norm_state, norm_count, nullptr, ws, w, st)) return rc;
+    add(d->potential, 1, ws + w.snap);
+    add(d->potential, 2, nullptr);
   }
-  return 0;
+  return J.njobs ? norm_stats(J, batch, ld, n, ws, w, (cudaStream_t)stream) : 0;
 }
 
 extern "C" int imb_norm_batch_stats(const imb_disc_desc* d, const float* batch, int64_t ld, int64_t n, int row0, int din,
                                     float* norm_state, int32_t* norm_count, float* defer, int defer_cap, float* ws,
                                     void* stream) {
-  cudaStream_t st = (cudaStream_t)stream;
   IMB_REQUIRE(n >= 1 && din >= 1 && din <= IMB_MAX_DIN, "norm batch stats: bad sizes");
   IMB_REQUIRE(defer == nullptr || defer_cap >= 1, "norm batch stats: defer_cap");
-  const WsLayout w = ws_layout(d->n_params);
-  NormLaunch NL;
-  NL.din = din;
-  for (int k = 0; k < din; ++k) NL.row[k] = (short)(row0 + k);
-  const int chunk_rows = n <= (int64_t)128 * 2048 ? 128 : NORM_CHUNK;
-  const int chunks = (int)((n + chunk_rows - 1) / chunk_rows);
-  IMB_REQUIRE(chunks >= 1 && chunks <= MAXCHUNKS, "norm update: n=%lld out of range", (long long)n);
-  k_norm_stats<<<chunks, 256, 0, st>>>(NL, batch, ld, n, chunk_rows, norm_state, norm_count, nullptr, ws + w.normpart,
-                                       reinterpret_cast<unsigned int*>(ws + w.ticket), defer, defer_cap);
-  IMB_CHECK_LAUNCH("k_norm_stats(batch)");
-  return 0;
+  NormJobs J = {1};
+  J.job[0].din = din;
+  for (int k = 0; k < din; ++k) J.job[0].row[k] = (short)(row0 + k);
+  J.job[0].rmv = norm_state;
+  J.job[0].cnt = norm_count;
+  return norm_stats(J, batch, ld, n, ws, ws_layout(d->n_params), (cudaStream_t)stream, defer, defer_cap);
 }
 
 extern "C" int imb_norm_fold(int din, float* defer, float* norm_state, int32_t* norm_count, int n_slots, void* stream) {
@@ -1256,11 +1052,8 @@ static int launch_fwdbwd(const DiscLaunch& L, const TPlan& t, const float* param
                                                ws + w.partial, reinterpret_cast<int*>(ws + w.meta), t.JP, t.KP, t.img_sz, t.aw_off, t.st_off, t.xn_off,
                                                t.t_off, t.v_off, t.nsl);
   IMB_CHECK_LAUNCH("k_disc_fwdbwd");
-  return (int)G;
+  return 0;
 }
-
-// host mirror of the grid chosen by the last fwd/bwd launch (stream-ordered use only)
-static thread_local int g_last_grid = 0;
 
 extern "C" int imb_disc_fwd_bwd(const imb_disc_desc* d, const float* params, const float* norm_state,
                                 const float* batch, int64_t ld, int64_t n, int64_t n_expert, float loss_scale,
@@ -1297,35 +1090,30 @@ extern "C" int imb_disc_fwd_bwd(const imb_disc_desc* d, const float* params, con
                                                          ws + w.partial, reinterpret_cast<int*>(ws + w.meta),
                                                          part_stride(d->n_params));
     IMB_CHECK_LAUNCH("k_disc_fwdbwd_tc");
-    g_last_grid = (int)Gt;
     return 0;
   }
   // Preferred: 128-row tiles with TWO resident CTAs per SM (independent CTAs overlap each other's
   // barriers and epilogues); else one 256-row CTA; else one 128-row CTA.
   TPlan t256 = plan_tiled(L, 256), t128 = plan_tiled(L, 128);
-  int G;
   if (2 * ((size_t)t128.total * 4 + 1024 + 512) <= 228 * 1024)
-    G = launch_fwdbwd<128>(L, t128, params, batch, ld, n, n_expert, loss_scale, grad_out, logits_out, ws, w, st, 2);
-  else if ((size_t)t256.total * 4 <= IMB_SMEM_MAX && n > 128)
-    G = launch_fwdbwd<256>(L, t256, params, batch, ld, n, n_expert, loss_scale, grad_out, logits_out, ws, w, st, 1);
-  else if ((size_t)t128.total * 4 <= IMB_SMEM_MAX)
-    G = launch_fwdbwd<128>(L, t128, params, batch, ld, n, n_expert, loss_scale, grad_out, logits_out, ws, w, st, 1);
-  else
-    IMB_FAIL(-1, "discriminator too large for the fused kernel (%zu B of shared memory)", (size_t)t128.total * 4);
-  if (G < 0) return G;
-  g_last_grid = G;
-  return 0;
+    return launch_fwdbwd<128>(L, t128, params, batch, ld, n, n_expert, loss_scale, grad_out, logits_out, ws, w, st, 2);
+  if ((size_t)t256.total * 4 <= IMB_SMEM_MAX && n > 128)
+    return launch_fwdbwd<256>(L, t256, params, batch, ld, n, n_expert, loss_scale, grad_out, logits_out, ws, w, st, 1);
+  if ((size_t)t128.total * 4 <= IMB_SMEM_MAX)
+    return launch_fwdbwd<128>(L, t128, params, batch, ld, n, n_expert, loss_scale, grad_out, logits_out, ws, w, st, 1);
+  IMB_FAIL(-1, "discriminator too large for the fused kernel (%zu B of shared memory)", (size_t)t128.total * 4);
+}
+
+// warp per parameter and per statistic, at most two blocks per SM
+static int reduce_blocks(int P) {
+  const int blocks = ((P + 5) * 32 + 255) / 256;
+  return blocks < 2 * imb_num_sms() ? blocks : 2 * imb_num_sms();
 }
 
 extern "C" int imb_disc_reduce(const imb_disc_desc* d, float* ws, float* grad_out_flat, void* stream) {
-  cudaStream_t st = (cudaStream_t)stream;
   const WsLayout w = ws_layout(d->n_params);
-  IMB_REQUIRE(g_last_grid > 0, "imb_disc_reduce called before imb_disc_fwd_bwd");
-  const int P = d->n_params;
-  const int warps = P + 5;
-  int blocks = (warps * 32 + 255) / 256;
-  if (blocks > 2 * imb_num_sms()) blocks = 2 * imb_num_sms();
-  k_disc_reduce<<<blocks, 256, 0, st>>>(P, g_last_grid, ws + w.partial, ws + w.gacc, ws + w.stats, grad_out_flat);
+  k_disc_reduce<<<reduce_blocks(d->n_params), 256, 0, (cudaStream_t)stream>>>(
+      d->n_params, reinterpret_cast<const int*>(ws + w.meta), ws + w.partial, ws + w.gacc, ws + w.stats, grad_out_flat);
   IMB_CHECK_LAUNCH("k_disc_reduce");
   return 0;
 }
@@ -1347,17 +1135,11 @@ extern "C" int imb_disc_adam(const imb_disc_desc* d, const imb_adam* opt, float*
 extern "C" int imb_disc_reduce_adam(const imb_disc_desc* d, const imb_adam* opt, float* params, float* exp_avg,
                                     float* exp_avg_sq, float grad_div, float* ws, int64_t* state, float* stats_out,
                                     void* stream) {
-  cudaStream_t st = (cudaStream_t)stream;
   const WsLayout w = ws_layout(d->n_params);
-  IMB_REQUIRE(g_last_grid > 0, "imb_disc_reduce_adam called before imb_disc_fwd_bwd");
-  const int P = d->n_params;
-  const int warps = P + 5;
-  int blocks = (warps * 32 + 255) / 256;
-  if (blocks > 2 * imb_num_sms()) blocks = 2 * imb_num_sms();
-  k_disc_reduce_adam<<<blocks, 256, 0, st>>>(P, g_last_grid, ws + w.partial, ws + w.gacc, ws + w.stats, *opt, params,
-                                             exp_avg, exp_avg_sq, grad_div, reinterpret_cast<const int*>(ws + w.meta),
-                                             state + IMB_ST_DISC_STEP, stats_out,
-                                             reinterpret_cast<unsigned int*>(ws + w.ticket) + 8);
+  k_disc_reduce_adam<<<reduce_blocks(d->n_params), 256, 0, (cudaStream_t)stream>>>(
+      d->n_params, ws + w.partial, ws + w.gacc, ws + w.stats, *opt, params, exp_avg, exp_avg_sq, grad_div,
+      reinterpret_cast<const int*>(ws + w.meta), state + IMB_ST_DISC_STEP, stats_out,
+      reinterpret_cast<unsigned int*>(ws + w.ticket) + 8);
   IMB_CHECK_LAUNCH("k_disc_reduce_adam");
   return 0;
 }

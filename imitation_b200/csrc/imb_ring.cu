@@ -57,41 +57,51 @@ __global__ void k_ring_advance(int64_t* state, int64_t capacity, int64_t n_store
 }
 
 // ---- index generation (perf mode) -----------------------------------------------------------------
-// kind 0: Philox randint with replacement in [0, ring size)   (twin: oracle/philox.randint)
-// kind 1: endless Feistel permutations with drop_last          (twin: ExpertStreamPort in tests)
+// replay draw i: Philox randint with replacement in [0, ring size)   (twin: oracle/philox.randint)
+__device__ __forceinline__ int64_t replay_row(uint64_t seed, const int64_t* state, int64_t i) {
+  const int64_t size = state[IMB_ST_RING_N];
+  const uint64_t draw = (uint64_t)state[IMB_ST_REPLAY_DRAW];
+  uint32_t k0, k1;
+  philox_key(seed, IMB_STREAM_REPLAY, k0, k1);
+  const Philox4 r = philox4x32((uint32_t)(i >> 2), (uint32_t)draw, (uint32_t)(draw >> 32), 0u, k0, k1);
+  const uint32_t w = ((i & 3) == 0) ? r.x : ((i & 3) == 1) ? r.y : ((i & 3) == 2) ? r.z : r.w;
+  return (int64_t)(((uint64_t)w * (uint64_t)size) >> 32);
+}
+// expert draw i of n_expert rows: endless Feistel permutations with drop_last   (twin: ExpertStreamPort in tests).
+// Position `pos` inside epoch `ep`; a batch never straddles an epoch: expert_advance guarantees
+// pos + batch <= n_expert - (n_expert % batch).
+__device__ __forceinline__ int64_t expert_row(uint64_t seed, const int64_t* state, int64_t n_expert, int64_t i) {
+  const int64_t pos = state[IMB_ST_EXPERT_POS];
+  const uint64_t ep = (uint64_t)state[IMB_ST_EXPERT_EPOCH];
+  const FeistelKey f = feistel_key(seed, IMB_STREAM_EXPERT, ep, (uint64_t)n_expert);
+  return (int64_t)feistel_perm(f, (uint64_t)(pos + i), (uint64_t)n_expert);
+}
+// the expert stream after a batch of n draws
+__device__ __forceinline__ void expert_advance(int64_t* state, int64_t n, int64_t n_expert) {
+  int64_t pos = state[IMB_ST_EXPERT_POS] + n;
+  if (pos + n > n_expert) {  // the next batch would not fit: drop the tail, start a new permutation
+    pos = 0;
+    state[IMB_ST_EXPERT_EPOCH] += 1;
+  }
+  state[IMB_ST_EXPERT_POS] = pos;
+}
+
+// kind 0: replay draws over the ring, kind 1: expert draws over size_arg rows
 __global__ void __launch_bounds__(256) k_sample_indices(int kind, int64_t* __restrict__ out, int64_t n,
                                                        int64_t size_arg, uint64_t seed,
                                                        const int64_t* __restrict__ state) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  if (kind == 0) {
-    const int64_t size = state[IMB_ST_RING_N];
-    const uint64_t draw = (uint64_t)state[IMB_ST_REPLAY_DRAW];
-    uint32_t k0, k1;
-    philox_key(seed, IMB_STREAM_REPLAY, k0, k1);
-    const Philox4 r = philox4x32((uint32_t)(i >> 2), (uint32_t)draw, (uint32_t)(draw >> 32), 0u, k0, k1);
-    const uint32_t w = ((i & 3) == 0) ? r.x : ((i & 3) == 1) ? r.y : ((i & 3) == 2) ? r.z : r.w;
-    out[i] = (int64_t)(((uint64_t)w * (uint64_t)size) >> 32);
-  } else {
-    // position `pos` inside epoch `ep`; a batch never straddles an epoch (drop_last): the host/
-    // advance kernel guarantees pos + n <= size_arg - (size_arg % n).
-    const int64_t pos = state[IMB_ST_EXPERT_POS];
-    const uint64_t ep = (uint64_t)state[IMB_ST_EXPERT_EPOCH];
-    const FeistelKey f = feistel_key(seed, IMB_STREAM_EXPERT, ep, (uint64_t)size_arg);
-    out[i] = (int64_t)feistel_perm(f, (uint64_t)(pos + i), (uint64_t)size_arg);
-  }
+  if (kind == 0)
+    out[i] = replay_row(seed, state, i);
+  else
+    out[i] = expert_row(seed, state, size_arg, i);
 }
 __global__ void k_sample_advance(int kind, int64_t n, int64_t size, int64_t* state) {
-  if (kind == 0) {
+  if (kind == 0)
     state[IMB_ST_REPLAY_DRAW] += 1;
-  } else {
-    int64_t pos = state[IMB_ST_EXPERT_POS] + n;
-    if (pos + n > size) {  // the next batch would not fit: drop the tail, start a new permutation
-      pos = 0;
-      state[IMB_ST_EXPERT_EPOCH] += 1;
-    }
-    state[IMB_ST_EXPERT_POS] = pos;
-  }
+  else
+    expert_advance(state, n, size);
 }
 
 // ---- gather table rows into the feature-major batch --------------------------------------------------
@@ -102,6 +112,18 @@ __global__ void k_sample_advance(int kind, int64_t n, int64_t size, int64_t* sta
 // feature row.  All tw loads of a lane are independent, so the whole tile costs ~one memory latency
 // (the former shuffle-and-transpose form serialised 32 dependent row reads per warp).
 constexpr int G_WARPS = 4;
+// table row src[0, tw) -> batch column dst (feature stride ld), 8 independent loads in flight per step
+__device__ __forceinline__ void row_to_column(const float* src, int tw, float* dst, int64_t ld) {
+  int c = 0;
+  for (; c + 8 <= tw; c += 8) {
+    float v[8];
+#pragma unroll
+    for (int u = 0; u < 8; ++u) v[u] = src[c + u];
+#pragma unroll
+    for (int u = 0; u < 8; ++u) dst[(int64_t)(c + u) * ld] = v[u];
+  }
+  for (; c < tw; ++c) dst[(int64_t)c * ld] = src[c];
+}
 __global__ void __launch_bounds__(G_WARPS * 32) k_gather_rows(const float* __restrict__ table, int64_t capacity,
                                                               int tw, const int64_t* __restrict__ idx, int64_t n,
                                                               float* __restrict__ batch, int64_t ld,
@@ -113,17 +135,7 @@ __global__ void __launch_bounds__(G_WARPS * 32) k_gather_rows(const float* __res
     if (mine >= n) continue;
     int64_t r = idx ? idx[mine] : mine;
     r = r < 0 ? 0 : (r >= capacity ? capacity - 1 : r);
-    const float* src = table + r * tw;
-    float* dst = batch + col0 + mine;
-    int c = 0;
-    for (; c + 8 <= tw; c += 8) {
-      float v[8];
-#pragma unroll
-      for (int u = 0; u < 8; ++u) v[u] = src[c + u];
-#pragma unroll
-      for (int u = 0; u < 8; ++u) dst[(int64_t)(c + u) * ld] = v[u];
-    }
-    for (; c < tw; ++c) dst[(int64_t)c * ld] = src[c];
+    row_to_column(table + r * tw, tw, batch + col0 + mine, ld);
   }
 }
 
@@ -146,42 +158,18 @@ __global__ void __launch_bounds__(G_WARPS * 32) k_sample_gather(const float* __r
     if (mine >= n) continue;
     const float* src;
     if (mine < mb) {
-      const int64_t i = start + mine;
-      const FeistelKey f = feistel_key(seed, IMB_STREAM_EXPERT, (uint64_t)e_state[IMB_ST_EXPERT_EPOCH], (uint64_t)e_n);
-      const int64_t r = (int64_t)feistel_perm(f, (uint64_t)(e_state[IMB_ST_EXPERT_POS] + i), (uint64_t)e_n);
-      src = e_table + r * tw;
+      src = e_table + expert_row(seed, e_state, e_n, start + mine) * tw;
     } else {
-      const int64_t i = start + (mine - mb);
-      const int64_t size = g_state[IMB_ST_RING_N];
-      const uint64_t draw = (uint64_t)g_state[IMB_ST_REPLAY_DRAW];
-      uint32_t k0, k1;
-      philox_key(seed, IMB_STREAM_REPLAY, k0, k1);
-      const Philox4 p = philox4x32((uint32_t)(i >> 2), (uint32_t)draw, (uint32_t)(draw >> 32), 0u, k0, k1);
-      const uint32_t w = ((i & 3) == 0) ? p.x : ((i & 3) == 1) ? p.y : ((i & 3) == 2) ? p.z : p.w;
-      int64_t r = (int64_t)(((uint64_t)w * (uint64_t)size) >> 32);
+      int64_t r = replay_row(seed, g_state, start + (mine - mb));
       r = r < 0 ? 0 : (r >= g_cap ? g_cap - 1 : r);
       src = g_table + r * tw;
     }
-    float* dst = batch + mine;
-    int c = 0;
-    for (; c + 8 <= tw; c += 8) {
-      float v[8];
-#pragma unroll
-      for (int u = 0; u < 8; ++u) v[u] = src[c + u];
-#pragma unroll
-      for (int u = 0; u < 8; ++u) dst[(int64_t)(c + u) * ld] = v[u];
-    }
-    for (; c < tw; ++c) dst[(int64_t)c * ld] = src[c];
+    row_to_column(src, tw, batch + mine, ld);
   }
 }
 __global__ void k_sample_advance2(int64_t n, int64_t e_n, int64_t* e_state, int64_t* g_state) {
   g_state[IMB_ST_REPLAY_DRAW] += 1;
-  int64_t pos = e_state[IMB_ST_EXPERT_POS] + n;
-  if (pos + n > e_n) {  // the next batch would not fit: drop the tail, start a new permutation
-    pos = 0;
-    e_state[IMB_ST_EXPERT_EPOCH] += 1;
-  }
-  e_state[IMB_ST_EXPERT_POS] = pos;
+  expert_advance(e_state, n, e_n);
 }
 
 }  // namespace

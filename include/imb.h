@@ -100,7 +100,8 @@ enum {
 
 int imb_version(void);
 const char* imb_last_error(void);
-/* number of floats of workspace the discriminator kernels need (partials, accumulators) */
+/* number of floats of workspace the discriminator kernels need (partials, accumulators).  The workspace must be
+ * zero-filled when allocated: its launch tickets and launch record start from zero. */
 int64_t imb_disc_workspace_floats(const imb_disc_desc* d);
 
 /* ---- stage 3: discriminator ------------------------------------------------------------ */
@@ -152,7 +153,8 @@ int imb_disc_fwd_bwd(const imb_disc_desc* d, const float* params, const float* n
  * gradient to grad_out_flat (for external optimisers / all-reduce), optional Adam step
  * (common.py:372) and the 9 train stats of the LAST minibatch (common.py:27-92) into
  * stats_out[16] = {loss, acc, acc_expert, acc_gen, entropy, prop_expert_true,
- * prop_expert_pred, n_expert, n_generated}.  state[IMB_ST_DISC_STEP] is incremented. */
+ * prop_expert_pred, n_expert, n_generated}.  state[IMB_ST_DISC_STEP] is incremented.  The partials reduced are
+ * those of the last imb_disc_fwd_bwd on the same workspace (none before the first). */
 int imb_disc_reduce(const imb_disc_desc* d, float* ws, float* grad_out_flat, void* stream);
 int imb_disc_adam(const imb_disc_desc* d, const imb_adam* opt, float* params, float* exp_avg,
                   float* exp_avg_sq, const float* grad_flat_or_null, float grad_div, float* ws,
