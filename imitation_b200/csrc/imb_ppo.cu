@@ -245,10 +245,11 @@ __device__ __forceinline__ void tower_wgrad(const int tnet, const int gj, const 
 //   * weight gradients over the CTA's 8 rows: thread = (unit, input subset) of one tower, staged in local shared
 //     memory in the parameter layout.  The VALUE tower's are computed early by warps 2-7 (its chain ends ~1 k cycles
 //     before the policy tower's: no action head, no loss terms) while warps 0, 1 finish the policy chain; the policy
-//     tower's by all eight warps after the step's second barrier.  The staged vector is pushed to the slice owners
-//     through distributed shared memory with 16-byte stores; owners sum the CL partials in fixed order, exchange the
-//     squared slice norms, run clip_grad_norm_ + Adam on their slice (the moments never leave their owner) and
-//     all-gather the new parameters into every CTA's copy.
+//     tower's by all eight warps after the step's second barrier.  The staged vector is pushed to the peer slice
+//     owners through distributed shared memory with 16-byte stores; owners sum the CL partials in fixed order (their
+//     own straight from the staging vector), exchange the squared slice norms, run clip_grad_norm_ + Adam on their
+//     slice (the moments never leave their owner) and all-gather the new parameters into every CTA's copy (their
+//     own with a local store).
 // No cluster barrier inside the step loop (the exchanged data signals mbarriers at the receivers), three CTA
 // barriers per optimiser step; the only global-memory traffic inside a step is the asynchronous minibatch prefetch.
 template <int HP>
@@ -268,8 +269,17 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
   __shared__ __align__(8) uint64_t mbar[3];  // one per staged-minibatch buffer (step s lives in buffer s % 3)
   __shared__ __align__(8) uint64_t xbar[3];  // [0]: partial gradients of the owned slice arrived; [1]: all new parameter slices; [2]: all slice norms
   __shared__ float SSQ[CL];                  // squared gradient norms of the 8 slices (each written by its owner)
+  __shared__ float nred[PT / 32];            // per-warp partial sums of the owned slice's squared norm
   const imb_policy_desc& pd = A.pol;
   const int Do = pd.d_obs, Da = pd.d_act, h = pd.hidden, NP = pd.n_params, KP = A.KP, S = A.S;
+  // Thread t < S / 4 owns quad t of this CTA's slice, so warps 0 .. n_own_w - 1 hold owned quads.  The warps above them
+  // and above the chain's warps 0-3 run the next minibatch's statistics in the TAIL of the step, beside the slice sum,
+  // norm exchange and Adam, so that nothing shared-memory heavy competes with the chain for issue slots; they issue the
+  // row prefetch beside the chain.  With fewer than two such warps (policies of more than 192 quads per slice) the
+  // statistics stay beside the chain too, on warps 4-7.
+  const int n_own_w = (S / 4 + 31) / 32;
+  const bool tail_stats = n_own_w <= PT / 32 - 2;
+  const int st0 = tail_stats ? 32 * max(n_own_w, 4) : 128, nst = PT - st0;  // first statistics thread, their count
   const PLay PL = make_play(pd);
   const int ldo = PL.ldo, ldh = PL.ldh;
   const int da_store = pd.discrete ? 1 : Da;
@@ -311,9 +321,9 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
     LOSS[tid & 31] = 0.f;
   }
   if (tid == 0) {
-    mbar_init(&mbar[0], 128);
-    mbar_init(&mbar[1], 128);
-    mbar_init(&mbar[2], 128);
+    mbar_init(&mbar[0], nst);
+    mbar_init(&mbar[1], nst);
+    mbar_init(&mbar[2], nst);
     mbar_init(&xbar[0], 1);
     mbar_init(&xbar[1], 1);
     mbar_init(&xbar[2], 1);
@@ -340,17 +350,17 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
   const WgradOff wo_p = {PL.w1[0], PL.b1[0], PL.w2[0], PL.b2[0], PL.wa, PL.ba, PL.wv, PL.bv, PL.ls, ldo, ldh};
   const WgradOff wo_v = {PL.w1[1], PL.b1[1], PL.w2[1], PL.b2[1], PL.wa, PL.ba, PL.wv, PL.bv, PL.ls, ldo, ldh};
 
-  // Asynchronous row gather of one minibatch (epoch ep, first row start) into buffer `buf` by warps 4-7: two
-  // threads per row draw the row index and copy half of the 16-byte aligned rollout row each with 16-byte
-  // cp.async (LDGSTS); completion is tracked by the buffer's mbarrier (one deferred arrival per thread).  (One
+  // Asynchronous row gather of one minibatch (epoch ep, first row start) into buffer `buf` by the nst statistics
+  // threads: two (thread) tasks per row draw the row index and copy half of the 16-byte aligned rollout row each with
+  // 16-byte cp.async (LDGSTS); completion is tracked by the buffer's mbarrier (one deferred arrival per thread).  (One
   // bulk-async copy per row and lane was tried first: the 32 per-lane UBLKCP issues serialise, ~2500 cycles per
-  // warp.)  Rows are fetched TWO optimiser steps ahead (three buffers), so their latency is never waited for.
+  // warp.)  Rows are fetched at least one full optimiser step ahead (three buffers), so their latency is never waited for.
   auto issue_gather = [&](int ep, int start, int buf) {
-    const int t = tid - 128;
-    if (t < 0) return;
-    const int r = t >> 1, half = t & 1;
+    if (tid < st0) return;
     const int nbx = min(mb, Ni - start);
-    if (r < nbx) {
+    for (int t = tid - st0; t < 2 * PR; t += nst) {
+      const int r = t >> 1, half = t & 1;
+      if (r >= nbx) continue;
       int64_t idx;
       if (perm_in) {
         idx = perm_in[(int64_t)ep * N + start + r];
@@ -437,7 +447,9 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
   // landed -- no cluster-wide barrier inside the step loop.  Each barrier is re-armed (one arrival + expected
   // bytes) by its owner right after the previous phase completed, which is always before a peer can send for
   // the next phase (a peer's next-phase data depends on data this CTA sends later).
-  const uint32_t xbytes = (uint32_t)(CL * S * 4);
+  // A CTA never sends to itself: the slice sum reads its own partial from GP, the owner stores its new slice into its
+  // own Pm directly, so both exchanges expect the bytes of the CL - 1 peers.
+  const uint32_t xbytes = (uint32_t)((CL - 1) * S * 4);
   const unsigned qmagic = (unsigned)(0x100000000ull / (unsigned)(S / 4)) + 1u;  // exact quotient for the < 2^16 quads here
   const uint32_t recv_sa = smem_u32(RECV), pm_sa = smem_u32(Pm), ssq_sa = smem_u32(SSQ);
   const uint32_t xbar0_sa = smem_u32(&xbar[0]), xbar1_sa = smem_u32(&xbar[1]), xbar2_sa = smem_u32(&xbar[2]);
@@ -477,20 +489,27 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
     const long long wclk0 = clock64();
 #endif
     float l_pg = 0.f, l_v = 0.f, l_ent = 0.f;
-    if (warp >= 4) {
-      // ---- 1b. warps 4-7, beside the chain: the NEXT step's minibatch statistics and own-row tile (they do not
-      //          depend on the parameters), then the row prefetch for the step after it ------------------------------
-      if (gs + 1 < n_steps) minibatch_stats(gs + 1, min(mb, Ni - start_next), (tid - 128) >> 3, (PT - 128) / 8);
+    // The NEXT step's minibatch statistics and own-row tile, by the statistics threads: they do not depend on the
+    // parameters, and XNo[(gs + 1) & 1] and buffer (gs + 1) % 3 are not read in this step
+    auto next_stats = [&]() {
+      if (gs + 1 < n_steps) minibatch_stats(gs + 1, min(mb, Ni - start_next), (tid - st0) >> 3, nst / 8);
       PPO_WCLK(1);
-      if (gs + 2 < n_steps) {
-        int ep2 = ep_next, start2 = start_next + mb;
-        if (start2 >= Ni) {
-          start2 = 0;
-          ++ep2;
+    };
+    if (warp >= 4) {
+      // ---- 1b. the statistics threads, beside the chain: the statistics when they cannot go in the tail, then the row
+      //          prefetch for the step after next into buffer (gs + 2) % 3 (last read by the previous step) -----------------
+      if (tid >= st0) {
+        if (!tail_stats) next_stats();
+        if (gs + 2 < n_steps) {
+          int ep2 = ep_next, start2 = start_next + mb;
+          if (start2 >= Ni) {
+            start2 = 0;
+            ++ep2;
+          }
+          issue_gather(ep2, start2, (int)((gs + 2) % 3));
         }
-        issue_gather(ep2, start2, (int)((gs + 2) % 3));
+        PPO_WCLK(3);
       }
-      PPO_WCLK(3);
     } else {
       // ---- 1a. warp-autonomous chain on warps 0-3: forward, loss terms, backward to dL/dz for (tower, 4 own rows).
       //          Four rows per warp: every weight fetched from shared memory feeds four FMAs (the chain was bound
@@ -736,7 +755,6 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
           make_float4(jl ? a0 * (1.f - h10 * h10) : 0.f, jl ? a1 * (1.f - h11 * h11) : 0.f,
                       jl ? a2 * (1.f - h12 * h12) : 0.f, jl ? a3 * (1.f - h13 * h13) : 0.f));
     }
-    if (pd.has_norm && gs + 1 < n_steps) run_count += min(mb, Ni - start_next);
     PPO_WCLK(0);
     // ---- 1c. the VALUE tower's weight gradients, early: its chain (warps 2, 3) finishes ~1 k cycles before the policy
     //          tower's (no action head, no loss terms) and the statistics / prefetch warps are done by then as well, so
@@ -765,9 +783,10 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
     tower_wgrad<PT / 32, HP>(0, lane, warp, h, Do, Da, pd.discrete != 0, wo_p, GP, TH1, TLAT, TDZ2, TDZ1, XNc, DM, DLS, DVAL);
     __syncthreads();
     PPO_TICK(7);
-    // ---- 3. push the partials to the slice owners: RECV[this CTA][i], one 16-byte DSMEM store per quad ----------
-    // CTA c starts with the quads owned by CTA c+1, so at any time the 8 senders target 8 different receivers
-    for (int q = tid; q < CL * S / 4; q += PT) {
+    // ---- 3. push the partials to the PEER slice owners: RECV[this CTA][i], one 16-byte DSMEM store per quad ------------
+    // CTA c starts with the quads owned by CTA c+1 and stops before its own slice (which its slice sum reads from GP),
+    // so at any time the 8 senders target 8 different receivers
+    for (int q = tid; q < (CL - 1) * (S / 4); q += PT) {
       int qq = q + ((crank + 1) & (CL - 1)) * (S / 4);
       if (qq >= CL * S / 4) qq -= CL * S / 4;
       const int p0 = 4 * qq, owner = (int)__umulhi((unsigned)qq, qmagic);  // = qq / (S / 4)
@@ -789,68 +808,88 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
       loss_log[gs * 4 + 3] = pg + A.hp.ent_coef * el + A.hp.vf_coef * vl;
     }
     PPO_TICK(8);
-    // wait until the 8 partials of the owned slice have landed
-    mbar_wait(&xbar[0], (uint32_t)(gs & 1));
-    if (tid == 0) mbar_expect_tx(&xbar[0], xbytes);  // re-arm for the next step
-    PPO_TICK(9);
+    if (tail_stats && tid >= st0) {
+      // ---- 4a. the statistics threads own no slice quad: they run the next step's statistics while the owners finish
+      //          the step.  They skip the exchange waits (they read none of RECV, SSQ or the new parameters before the
+      //          next step's top barrier, which the owners reach only after those waits).
+      next_stats();
+    } else {
+      // wait until the 7 peer partials of the owned slice have landed
+      mbar_wait(&xbar[0], (uint32_t)(gs & 1));
+      if (tid == 0) mbar_expect_tx(&xbar[0], xbytes);  // re-arm for the next step
+      PPO_TICK(9);
 
-    // ---- 4. slice owners: sum the CL partials in fixed order (one quad per thread), exchange the squared slice
-    //         norms for clip_grad_norm_ (4 bytes to every CTA, same st.async + mbarrier mechanism) ------------------------
-    const int i0 = 4 * tid;
-    const bool own = i0 < S;  // S / 4 <= PT is checked by the launcher
-    float4 g = make_float4(0.f, 0.f, 0.f, 0.f);
-    float ss = 0.f;
-    if (own) {
-      g = ld4(RECV + i0);
-#pragma unroll
-      for (int c = 1; c < CL; ++c) {  // fixed order: deterministic
-        const float4 t = ld4(RECV + c * S + i0);
-        g.x += t.x, g.y += t.y, g.z += t.z, g.w += t.w;
+      // ---- 4. slice owners: sum the CL partials in fixed order (one quad per thread), exchange the squared slice
+      //         norms for clip_grad_norm_ (4 bytes to every CTA, same st.async + mbarrier mechanism) ------------------------
+      const int i0 = 4 * tid;
+      const bool own = i0 < S;  // S / 4 <= PT is checked by the launcher
+      float4 g = make_float4(0.f, 0.f, 0.f, 0.f);
+      float ss = 0.f;
+      if (own) {
+        // CTA c's partial of the slice: RECV[c], or this CTA's own straight from GP
+        auto part = [&](int c) { return ld4(c == crank ? GP + crank * S + i0 : RECV + c * S + i0); };
+        g = part(0);
+  #pragma unroll
+        for (int c = 1; c < CL; ++c) {  // fixed order: deterministic
+          const float4 t = part(c);
+          g.x += t.x, g.y += t.y, g.z += t.z, g.w += t.w;
+        }
+        ss = (g.x * g.x + g.y * g.y) + (g.z * g.z + g.w * g.w);
       }
-      ss = (g.x * g.x + g.y * g.y) + (g.z * g.z + g.w * g.w);
-    }
-    const float my_ssq = block_sum(ss, red);
-    if (tid < CL) st_async_f32(mapa_u32(ssq_sa + (uint32_t)crank * 4u, tid), my_ssq, mapa_u32(xbar2_sa, tid));
-    PPO_TICK(10);
-    mbar_wait(&xbar[2], (uint32_t)(gs & 1));
-    if (tid == 0) mbar_expect_tx(&xbar[2], (uint32_t)(CL * 4));  // re-arm for the next step
-    PPO_TICK(11);
+      // squared norm of the slice: warp sums, then the warps' in warp order, over the owner warps only (a named barrier;
+      // the other warps' terms are +0.0 and are still added, so the sum is the full-CTA reduction's bit for bit)
+      float my_ssq = 0.f;
+      if (warp < n_own_w) {
+        const float ws = warp_sum(ss);
+        if (lane == 0) nred[warp] = ws;
+        asm volatile("bar.sync 2, %0;" ::"r"(32 * n_own_w) : "memory");
+  #pragma unroll
+        for (int w = 0; w < PT / 32; ++w) my_ssq += w < n_own_w ? nred[w] : 0.f;
+      }
+      if (tid < CL) st_async_f32(mapa_u32(ssq_sa + (uint32_t)crank * 4u, tid), my_ssq, mapa_u32(xbar2_sa, tid));
+      PPO_TICK(10);
+      mbar_wait(&xbar[2], (uint32_t)(gs & 1));
+      if (tid == 0) mbar_expect_tx(&xbar[2], (uint32_t)(CL * 4));  // re-arm for the next step
+      PPO_TICK(11);
 
-    // ---- 5. clip_grad_norm_ + Adam on the OWNED slice (moments never leave their owner); the new parameters are
-    //         all-gathered into every CTA's parameter vector ----------------------------------------------------------
-    float total = 0.f;
-#pragma unroll
-    for (int c = 0; c < CL; ++c) total += SSQ[c];  // same order everywhere: the replicas' clip factors agree bit for bit
-    total = sqrtf(total);
-    float clip = A.hp.max_grad_norm / (total + 1e-6f);
-    clip = clip > 1.0f ? 1.0f : clip;
-    if (own) {
-      const float step_size = bc[2 * cur], inv_bc2s = rcp_fast(bc[2 * cur + 1]);
-      const int q0 = crank * S + i0;
-      const float4 m4 = ld4(Ms + q0), v4 = ld4(Vs + q0), p4 = ld4(Pm + q0);
-      // approximate sqrt / division (~1e-7 relative on an update that is itself ~lr relative to the weights)
-      auto adam1 = [&](float gg, float& m, float& v, float& pw) {
-        gg *= clip;
-        m = m + (gg - m) * (1.0f - 0.9f);
-        v = v * 0.999f + (1.0f - 0.999f) * gg * gg;
-        pw -= step_size * __fdividef(m, fmaf(sqrt_fast(v), inv_bc2s, A.hp.adam_eps));
-      };
-      float4 m = m4, v = v4, pw = p4;
-      adam1(g.x, m.x, v.x, pw.x);
-      adam1(g.y, m.y, v.y, pw.y);
-      adam1(g.z, m.z, v.z, pw.z);
-      adam1(g.w, m.w, v.w, pw.w);
-      st4(Ms + q0, m);
-      st4(Vs + q0, v);
-#pragma unroll
-      for (int c = 0; c < CL; ++c) {  // rotated start: the 8 owners write to 8 different CTAs at a time
-        const int dstc = (crank + c) & (CL - 1);
-        st_async_v4(mapa_u32(pm_sa + (uint32_t)q0 * 4u, dstc), pw, mapa_u32(xbar1_sa, dstc));
+      // ---- 5. clip_grad_norm_ + Adam on the OWNED slice (moments never leave their owner); the new parameters are
+      //         all-gathered into every CTA's parameter vector ----------------------------------------------------------
+      float total = 0.f;
+  #pragma unroll
+      for (int c = 0; c < CL; ++c) total += SSQ[c];  // same order everywhere: the replicas' clip factors agree bit for bit
+      total = sqrtf(total);
+      float clip = A.hp.max_grad_norm / (total + 1e-6f);
+      clip = clip > 1.0f ? 1.0f : clip;
+      if (own) {
+        const float step_size = bc[2 * cur], inv_bc2s = rcp_fast(bc[2 * cur + 1]);
+        const int q0 = crank * S + i0;
+        const float4 m4 = ld4(Ms + q0), v4 = ld4(Vs + q0), p4 = ld4(Pm + q0);
+        // approximate sqrt / division (~1e-7 relative on an update that is itself ~lr relative to the weights)
+        auto adam1 = [&](float gg, float& m, float& v, float& pw) {
+          gg *= clip;
+          m = m + (gg - m) * (1.0f - 0.9f);
+          v = v * 0.999f + (1.0f - 0.999f) * gg * gg;
+          pw -= step_size * __fdividef(m, fmaf(sqrt_fast(v), inv_bc2s, A.hp.adam_eps));
+        };
+        float4 m = m4, v = v4, pw = p4;
+        adam1(g.x, m.x, v.x, pw.x);
+        adam1(g.y, m.y, v.y, pw.y);
+        adam1(g.z, m.z, v.z, pw.z);
+        adam1(g.w, m.w, v.w, pw.w);
+        st4(Ms + q0, m);
+        st4(Vs + q0, v);
+        st4(Pm + q0, pw);
+  #pragma unroll
+        for (int c = 1; c < CL; ++c) {  // rotated start: the 8 owners write to 8 different CTAs at a time
+          const int dstc = (crank + c) & (CL - 1);
+          st_async_v4(mapa_u32(pm_sa + (uint32_t)q0 * 4u, dstc), pw, mapa_u32(xbar1_sa, dstc));
+        }
       }
+      mbar_wait(&xbar[1], (uint32_t)(gs & 1));  // every CTA's new parameter slice has landed in Pm
+      if (tid == 0) mbar_expect_tx(&xbar[1], xbytes);  // re-arm for the next step
+      PPO_TICK(12);
     }
-    mbar_wait(&xbar[1], (uint32_t)(gs & 1));  // every CTA's new parameter slice has landed in Pm
-    if (tid == 0) mbar_expect_tx(&xbar[1], xbytes);  // re-arm for the next step
-    PPO_TICK(12);
+    if (pd.has_norm && gs + 1 < n_steps) run_count += min(mb, Ni - start_next);  // (after the statistics that read it)
     ep_now = ep_next;
     start = start_next;
     // (the barrier at the top of the next step orders these parameter writes before their first use)

@@ -12,7 +12,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from imitation_b200 import _desc, _lib  # noqa: E402
 
 NAMES = ["top barrier", "-", "-", "warp chain fwd/loss/bwd", "-", "-", "-",
-         "weight gradients -> GP", "push partials", "barrier a wait", "slice sum + norm exchange issue", "wait: slice norms landed",
+         "weight gradients -> GP", "push partials (7 peers)", "barrier a wait", "slice sum + norm exchange issue", "wait: slice norms landed",
          "clip + Adam (own slice) + parameter all-gather + wait", "-"]
 pd = _desc.policy_desc(17, 6, False, 32, True)
 N = 4096
@@ -47,7 +47,8 @@ print(f"{'total':<18s} {tot / steps:9.0f} cycles/step")
 
 w = (ctypes.c_longlong * 80)()
 assert _lib.lib().imb_debug_ppo_warp_clocks(w, 0) == 0
-print("per-warp cycles/step since the top barrier (CTA 0; warps 0,1 policy tower, 2,3 value tower; warps 4-7: slot 1 = next-step stats done, slot 3 = prefetch issued):")
+print("per-warp cycles/step since the top barrier (CTA 0; warps 0,1 policy tower, 2,3 value tower; warps 4-7: slot 1 = "
+      "next-step stats done (in the step's tail), slot 3 = prefetch issued (beside the chain)):")
 for slot, name in ((1, "stats done (w4-7)"), (3, "after layer 1 | prefetch"), (4, "after layer 2"), (5, "after means (policy)"), (6, "after logp reduce"), (7, "after dM/dlogstd"),
                    (2, "after heads/loss"), (0, "chain end"), (8, "early value wgrad done (w2-7)")):
     print(f"  {name:<22s}", [round(w[slot * 8 + i] / steps) for i in range(8)])
