@@ -66,6 +66,17 @@ class PpoHparams(C.Structure):
                 ("n_epochs", C.c_int32), ("batch_size", C.c_int32), ("normalize_advantage", C.c_int32)]
 
 
+PU_MAX_MEMBERS = 16
+
+
+class PrefUncDesc(C.Structure):
+    _fields_ = [("n_members", C.c_int32), ("rews", C.c_void_p * PU_MAX_MEMBERS),
+                ("norm_state", C.c_void_p * PU_MAX_MEMBERS), ("norm_count", C.c_void_p * PU_MAX_MEMBERS),
+                ("norm_eps", C.c_float * PU_MAX_MEMBERS)]
+
+
+PU_MODES = {"logit": 0, "probability": 1, "label": 2}
+
 SYNC_MAX_AVG, SYNC_MAX_NORM = 8, 4
 
 
@@ -86,7 +97,7 @@ SYMBOLS = [
     "imb_rollout_advance", "imb_env_reset", "imb_ppo_update", "imb_policy_logp", "imb_state_init",
     "imb_sync_buffer_doubles", "imb_sync_snapshot", "imb_sync_pack", "imb_sync_unpack",
     "imb_disc_sample_gather", "imb_sample_advance2", "imb_disc_reduce_adam", "imb_norm_batch_stats", "imb_norm_fold",
-    "imb_disc_set_rows", "imb_stats_publish", "imb_pref_loss",
+    "imb_disc_set_rows", "imb_stats_publish", "imb_pref_loss", "imb_pref_uncertainty_ws_floats", "imb_pref_uncertainty",
 ]
 
 
@@ -101,6 +112,7 @@ def lib() -> C.CDLL:
         _lib.imb_last_error.restype = C.c_char_p
         _lib.imb_disc_workspace_floats.restype = C.c_int64
         _lib.imb_sync_buffer_doubles.restype = C.c_int64
+        _lib.imb_pref_uncertainty_ws_floats.restype = C.c_int64
         for name in SYMBOLS:
             getattr(_lib, name)  # AttributeError if the .so is stale
     return _lib
@@ -115,6 +127,7 @@ _KERNELS_PER_CALL = {
     "imb_rollout_advance": 1, "imb_env_reset": 1, "imb_ppo_update": 1, "imb_policy_logp": 1,
     "imb_disc_sample_gather": 1, "imb_sample_advance2": 1, "imb_disc_reduce_adam": 1, "imb_norm_batch_stats": 1,
     "imb_norm_fold": 1, "imb_disc_set_rows": 1, "imb_stats_publish": 1, "imb_pref_loss": 1,
+    "imb_pref_uncertainty": None,
 }
 
 
@@ -246,6 +259,35 @@ def pref_loss(rews, n_pairs, frag_len, prefs, noise_prob, discount, threshold, g
                                C.c_float(noise_prob), C.c_float(discount), C.c_float(threshold), C.c_float(grad_scale),
                                _p(grad_rews), _p(probs_out), _p(stats_acc), C.c_int32(stats_slot), _stream()),
            "imb_pref_loss")
+
+
+def pref_uncertainty_desc(rews, norms) -> PrefUncDesc:
+    """rews: one float32 CUDA tensor [2C * L] per member; norms: per member None or (state [mean, var], int32 count, eps)
+    of its output RunningNorm."""
+    if not 2 <= len(rews) <= PU_MAX_MEMBERS or len(norms) != len(rews):
+        raise ImbError(f"imb_pref_uncertainty takes 2 to {PU_MAX_MEMBERS} members, got {len(rews)}")
+    d = PrefUncDesc()
+    d.n_members = len(rews)
+    for m, (r, nm) in enumerate(zip(rews, norms)):
+        d.rews[m] = _p(r, th.float32).value
+        if nm is not None:
+            d.norm_state[m], d.norm_count[m] = _p(nm[0], th.float32).value, _p(nm[1], th.int32).value
+            d.norm_eps[m] = nm[2]
+    return d
+
+
+def pref_uncertainty_ws_floats(n_members: int, n_pairs: int) -> int:
+    return int(lib().imb_pref_uncertainty_ws_floats(C.c_int32(n_members), C.c_int64(n_pairs)))
+
+
+def pref_uncertainty(d: PrefUncDesc, n_pairs, frag_len, mode, noise_prob, discount, threshold, ws, scores,
+                     member_out=None):
+    """Active-selection scores of n_pairs candidate pairs (mode: 0 logit, 1 probability, 2 label; PU_MODES)."""
+    norm = any(d.norm_state[m] for m in range(d.n_members))
+    _check(lib().imb_pref_uncertainty(C.byref(d), C.c_int64(n_pairs), C.c_int32(frag_len), C.c_int32(mode),
+                                      C.c_float(noise_prob), C.c_float(discount), C.c_float(threshold),
+                                      _p(ws, th.float32), _p(scores, th.float32), _p(member_out, th.float32),
+                                      _stream()), "imb_pref_uncertainty", (1 + int(norm)) if n_pairs > 0 else 0)
 
 
 def reward_norm_scan(rews, n_envs, n_steps, step_stride, env_stride, norm_state2, norm_count, eps, update_stats):

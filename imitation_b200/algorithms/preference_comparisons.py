@@ -339,6 +339,8 @@ class FragmentPool:
         self.rews: Optional[th.Tensor] = None
         self._slots: Dict[int, Tuple[object, int]] = {}
         self._state = th.zeros(_lib.ST_WORDS, dtype=th.int64, device=self.device)
+        self._stage_table: Optional[th.Tensor] = None
+        self._stage_rews: Optional[th.Tensor] = None
 
     def _grow(self, n_slots: int) -> None:
         rows = n_slots * self.L
@@ -353,6 +355,25 @@ class FragmentPool:
             r = th.zeros(cap, device=self.device)
             r[:self.rews.shape[0]] = self.rews
             self.table, self.rews = t, r
+
+    def _upload(self, frags: Sequence[TrajectoryWithRew], table: th.Tensor, rews: th.Tensor, row0: int) -> None:
+        """Stack `frags` on the host and store their L-row blocks at rows [row0, row0 + len(frags) * L) of `table`
+        (and their ground-truth rewards, if any, in `rews`)."""
+        tr = _stack_fragments(frags)
+        n = len(tr["obs"])
+        dev = self.device
+        f32 = lambda x: th.as_tensor(np.ascontiguousarray(x, dtype=np.float32)).to(dev).reshape(n, -1)
+        dones = th.as_tensor(np.ascontiguousarray(tr["dones"]).astype(np.uint8)).to(dev)
+        dst = table[row0:]
+        if self.discrete:
+            acts = th.as_tensor(np.ascontiguousarray(tr["acts"]).astype(np.int64)).to(dev).reshape(n)
+            _lib.table_store(dst, n, self.d_obs, self.d_act, f32(tr["obs"]), None, acts, f32(tr["next_obs"]), dones, n,
+                             False, self._state)
+        else:
+            _lib.table_store(dst, n, self.d_obs, self.d_act, f32(tr["obs"]), f32(tr["acts"]), None, f32(tr["next_obs"]),
+                             dones, n, False, self._state)
+        if isinstance(frags[0], TrajectoryWithRew):
+            rews[row0:row0 + n] = th.as_tensor(np.concatenate([f.rews for f in frags]).astype(np.float32)).to(dev)
 
     def slots(self, frags: Sequence[TrajectoryWithRew]) -> th.Tensor:
         """Slot index of every fragment (uploading the ones not seen before), as a device int64 vector."""
@@ -369,23 +390,41 @@ class FragmentPool:
         if new:
             k0 = self._slots[id(new[0])][1]
             self._grow(len(self._slots))
-            tr = _stack_fragments(new)
-            n = len(tr["obs"])
-            dev = self.device
-            f32 = lambda x: th.as_tensor(np.ascontiguousarray(x, dtype=np.float32)).to(dev).reshape(n, -1)
-            dones = th.as_tensor(np.ascontiguousarray(tr["dones"]).astype(np.uint8)).to(dev)
-            dst = self.table[k0 * self.L:]
-            if self.discrete:
-                acts = th.as_tensor(np.ascontiguousarray(tr["acts"]).astype(np.int64)).to(dev).reshape(n)
-                _lib.table_store(dst, n, self.d_obs, self.d_act, f32(tr["obs"]), None, acts, f32(tr["next_obs"]), dones, n,
-                                 False, self._state)
-            else:
-                _lib.table_store(dst, n, self.d_obs, self.d_act, f32(tr["obs"]), f32(tr["acts"]), None, f32(tr["next_obs"]),
-                                 dones, n, False, self._state)
-            if isinstance(new[0], TrajectoryWithRew):
-                self.rews[k0 * self.L:k0 * self.L + n] = th.as_tensor(
-                    np.concatenate([f.rews for f in new]).astype(np.float32)).to(dev)
+            self._upload(new, self.table, self.rews, k0 * self.L)
         return th.as_tensor(np.asarray(out, dtype=np.int64)).to(self.device)
+
+    def stage(self, frags: Sequence[TrajectoryWithRew]) -> th.Tensor:
+        """Upload `frags` to the staging table (fragment j at rows [j * L, (j + 1) * L)) without registering them, and
+        return that table.  Candidates of an active selection go here: only the selected ones are then `adopt`ed, so the
+        rejected ones leave no rows behind.  The table is reused (and grown) across calls."""
+        if self.L is None:
+            self.L = len(frags[0])
+        rows = len(frags) * self.L
+        if self._stage_table is None or self._stage_table.shape[0] < rows:
+            self._stage_table = th.zeros(rows, self.tw, device=self.device)
+            self._stage_rews = th.zeros(rows, device=self.device)
+        self._upload(frags, self._stage_table, self._stage_rews, 0)
+        return self._stage_table
+
+    def adopt(self, frags: Sequence[TrajectoryWithRew], staged: Sequence[int]) -> None:
+        """Register `frags`, whose rows sit at staging slots `staged` since the last `stage`, as pool fragments: a
+        device-to-device copy of their rows, no upload."""
+        src, new = [], []
+        for f, j in zip(frags, staged):
+            ent = self._slots.get(id(f))
+            if ent is None or ent[0] is not f:
+                self._slots[id(f)] = (f, len(self._slots))
+                new.append(f)
+                src.append(j)
+        if not new:
+            return
+        k0 = self._slots[id(new[0])][1]
+        self._grow(len(self._slots))
+        ar = th.arange(self.L, device=self.device)
+        src_rows = (th.as_tensor(np.asarray(src, dtype=np.int64)).to(self.device)[:, None] * self.L + ar).reshape(-1)
+        n = src_rows.numel()
+        self.table[k0 * self.L:k0 * self.L + n] = self._stage_table.index_select(0, src_rows)
+        self.rews[k0 * self.L:k0 * self.L + n] = self._stage_rews.index_select(0, src_rows)
 
     def row_index(self, slots: th.Tensor) -> th.Tensor:
         return (slots[:, None] * self.L + th.arange(self.L, device=self.device)[None, :]).reshape(-1)
@@ -541,6 +580,158 @@ class PreferenceModel(nn.Module):
                 gt_probs = th.stack([self._probability(th.from_numpy(a.rews), th.from_numpy(b.rews), 0)
                                      for a, b in fragment_pairs])
         return probs, gt_probs
+
+    # -- active selection: candidate scores on the device -------------------------------------------------------------
+    def _scoring_members(self) -> Optional[Tuple[list, list]]:
+        """(fused nets, output norms) of the members, when every member is a fused reward net on CUDA, optionally inside
+        a NormalizedRewardNet, all with the same spaces and at most 16 of them; otherwise None."""
+        if self.ensemble_model is None or not self.use_fragment_pool:
+            return None
+        members = list(self.ensemble_model.members)
+        if len(members) > _lib.PU_MAX_MEMBERS:
+            return None
+        nets, outs = [], []
+        for m in members:
+            out = m if type(m) is reward_nets.NormalizedRewardNet else None
+            net = m.base if out is not None else m
+            if not isinstance(net, reward_nets._FusedNetMixin) or net.device.type != "cuda":
+                return None
+            nets.append(net)
+            outs.append(out)
+        d0 = nets[0].engine().desc
+        if any(n.device != nets[0].device or n.engine().desc.d_obs != d0.d_obs or n.engine().desc.d_act != d0.d_act
+               for n in nets):
+            return None
+        return nets, outs
+
+    def uncertainty_scores(self, fragment_pairs: Sequence[TrajectoryWithRewPair], uncertainty_on: str,
+                           member_values: bool = False) -> Optional[Tuple[th.Tensor, Optional[th.Tensor]]]:
+        """Active-selection scores of the candidate pairs (device float32 [C]), and with `member_values` the per-member
+        return differences (logit) or probabilities (probability, label) [C, M]; None when the members or fragments are
+        outside the device path (see `ActiveSelectionFragmenter`).
+
+        The candidates go to the fragment pool's staging table (slot 2 i + s = pair i, fragment s), one gather builds the
+        feature-major batch, one `imb_reward_forward` per member (eval mode, as `predict_processed`) writes its raw
+        rewards, and `imb_pref_uncertainty` applies the NormalizedRewardNet members' output normalisation fragment by
+        fragment -- advancing their statistics as the reference's per-fragment `predict_processed` calls do -- and scores
+        every pair.  `adopt_candidates` then registers the selected fragments in the pool."""
+        frags = [f for pair in fragment_pairs for f in pair]
+        lengths = {len(f) for f in frags}
+        members = self._scoring_members()
+        if len(lengths) != 1 or members is None:
+            return None
+        L = lengths.pop()
+        nets, outs = members
+        pool = self._get_pool(nets[0])
+        if pool.L not in (None, L):
+            return None
+        table = pool.stage(frags)
+        C, M, n = len(fragment_pairs), len(nets), len(frags) * L
+        e0 = nets[0].engine()
+        dev = e0.device()
+        batch, ld = e0.new_batch(n)
+        _lib.gather_rows(table, table.shape[0], pool.tw, None, n, batch, ld, 0)
+        rews = th.empty(M, n, device=dev)
+        for k, net in enumerate(nets):
+            e = net.engine()
+            _lib.reward_forward(e.desc, e.params, e.norm_state, batch, ld, n, 0, rews[k])
+        norms = [None if o is None else (*o.output_norm_vectors(), float(o.normalize_output_layer.eps)) for o in outs]
+        desc = _lib.pref_uncertainty_desc(list(rews), norms)
+        ws_n = _lib.pref_uncertainty_ws_floats(M, C)
+        ws = self.__dict__.get("_pu_ws")
+        if ws is None or ws.numel() < ws_n or ws.device != dev:
+            ws = self._pu_ws = th.zeros(ws_n, device=dev)  # (zero-filled once: the kernel re-arms its ticket)
+        scores = th.empty(C, device=dev)
+        member_out = th.empty(C, M, device=dev) if member_values else None
+        _lib.pref_uncertainty(desc, C, L, _lib.PU_MODES[uncertainty_on], self.noise_prob, self.discount_factor,
+                              self.threshold, ws, scores, member_out)
+        return scores, member_out
+
+    def adopt_candidates(self, fragment_pairs: Sequence[TrajectoryWithRewPair], chosen: Sequence[int]) -> None:
+        """Register pairs `chosen` of the candidates last scored by `uncertainty_scores` in the fragment pool (a device
+        row copy from the staging table), so training on them uploads nothing."""
+        pool = (self._pool_owner or self)._pool
+        frags = [f for i in chosen for f in fragment_pairs[i]]
+        pool.adopt(frags, [2 * i + s for i in chosen for s in (0, 1)])
+
+
+class ActiveSelectionFragmenter(Fragmenter):
+    """Pairs the ensemble members disagree on most (:668-778): draws `fragment_sample_factor * num_pairs` candidates
+    from `base_fragmenter` (the same host random draws as the reference), scores each and returns the `num_pairs` with
+    the highest scores, ordered by descending score.  The score is the variance over the members of
+
+    - `logit`: the undiscounted return difference sum_t r1 - sum_t r2 (torch.var, ddof 1; discount, threshold and noise
+      are not used);
+    - `probability`: `PreferenceModel.probability` (np.var, ddof 0);
+    - `label`: the Bernoulli variance q (1 - q) of the labels probability > 0.5, q their mean;
+
+    where the rewards are each member's `predict_processed` of one fragment at a time, in the order pair 0 first, pair
+    0 second, pair 1 first, ...; a NormalizedRewardNet member normalises each fragment with its output statistics as
+    they stood before that fragment, then merges it into them.
+
+    Ties are ordered by descending candidate index (`np.argsort(scores, kind="stable")[::-1]`).  The reference uses
+    NumPy's default sort, which is not stable and orders equal scores differently on different CPUs; the label mode has
+    ties all the time.
+
+    When every member is a fused reward net on CUDA (optionally inside a NormalizedRewardNet), there are at most 16 and
+    all candidates have the fragment pool's length, the scoring runs on the device (`PreferenceModel.uncertainty_scores`)
+    and the selected fragments enter the fragment pool without another upload; otherwise the reference's per-pair loop
+    over `PreferenceModel.rewards` and `variance_estimate` runs."""
+
+    def __init__(self, preference_model: PreferenceModel, base_fragmenter: Fragmenter, fragment_sample_factor: float,
+                 uncertainty_on: str = "logit", custom_logger: Optional[imit_logger.HierarchicalLogger] = None) -> None:
+        super().__init__(custom_logger=custom_logger)
+        if preference_model.ensemble_model is None:
+            raise ValueError("PreferenceModel not wrapped over an ensemble of networks.")
+        self.preference_model = preference_model
+        self.base_fragmenter = base_fragmenter
+        self.fragment_sample_factor = fragment_sample_factor
+        self._uncertainty_on = uncertainty_on
+        if uncertainty_on not in ("logit", "probability", "label"):
+            self.raise_uncertainty_on_not_supported()
+
+    @property
+    def uncertainty_on(self) -> str:
+        return self._uncertainty_on
+
+    def raise_uncertainty_on_not_supported(self):
+        raise ValueError(f"""{self.uncertainty_on} not supported.
+            `uncertainty_on` should be from `logit`, `probability`, or `label`""")
+
+    def __call__(self, trajectories: Sequence[TrajectoryWithRew], fragment_length: int, num_pairs: int
+                 ) -> Sequence[TrajectoryWithRewPair]:
+        candidates = self.base_fragmenter(trajectories=trajectories, fragment_length=fragment_length,
+                                          num_pairs=int(self.fragment_sample_factor * num_pairs))
+        if len(candidates) == 0:
+            return []
+        with th.no_grad():
+            dev = self.preference_model.uncertainty_scores(candidates, self.uncertainty_on)
+        if dev is not None:
+            # stable ascending sort, reversed: descending score, ties by descending index; one read-back
+            chosen = th.argsort(dev[0], stable=True).flip(0)[:num_pairs].cpu().tolist()
+            self.preference_model.adopt_candidates(candidates, chosen)
+        else:
+            scores = np.zeros(len(candidates))
+            for i, (frag1, frag2) in enumerate(candidates):
+                with th.no_grad():
+                    rews1 = self.preference_model.rewards(rollout.flatten_trajectories([frag1]))
+                    rews2 = self.preference_model.rewards(rollout.flatten_trajectories([frag2]))
+                scores[i] = self.variance_estimate(rews1, rews2)
+            chosen = np.argsort(scores, kind="stable")[::-1][:num_pairs].tolist()
+        return [candidates[i] for i in chosen]
+
+    def variance_estimate(self, rews1: th.Tensor, rews2: th.Tensor) -> float:
+        """Score of one pair from the members' rewards of its fragments, [fragment_length, members] each (:749-778)."""
+        if self.uncertainty_on == "logit":
+            return (rews1.sum(0) - rews2.sum(0)).var().item()
+        probs = self.preference_model.probability(rews1, rews2).cpu().numpy()
+        assert probs.shape == (self.preference_model.model.num_members,)
+        if self.uncertainty_on == "probability":
+            return probs.var()
+        if self.uncertainty_on == "label":
+            q = (probs > 0.5).astype(np.float32).mean()
+            return q * (1 - q)
+        self.raise_uncertainty_on_not_supported()
 
 
 class LossAndMetrics(NamedTuple):

@@ -23,6 +23,8 @@
 //   k_disc_reduce_adam  both in one launch: the last block (ticket) runs the Adam step and the statistics.
 #include <stdlib.h>
 
+#include <algorithm>
+
 #include "imb_common.cuh"
 #include "imb_mlp.cuh"
 #include "imb_tile.cuh"
@@ -698,6 +700,23 @@ __global__ void __launch_bounds__(256) k_disc_reduce_adam(int P, const float* __
 }
 
 // ---- preference comparisons: fragment returns -> Boltzmann probability -> cross entropy (+ its gradient) -------------
+// PreferenceModel.probability (algorithms/preference_comparisons.py:487-530) from the (discounted) return difference
+// s = sum_t g^t (r2 - r1): d = clip(s, -threshold, threshold), m = 1 / (1 + e^d), p = noise / 2 + (1 - noise) m.
+// k_pref_loss also needs e^d, m and whether s was clipped for its gradient.
+struct PrefProb {
+  float ed, m, p;
+  bool clipped;
+};
+__device__ __forceinline__ PrefProb pref_probability(float s, float noise_prob, float threshold) {
+  PrefProb q;
+  q.clipped = s < -threshold || s > threshold;
+  const float d = fminf(fmaxf(s, -threshold), threshold);
+  q.ed = expf(d);
+  q.m = 1.0f / (1.0f + q.ed);
+  q.p = noise_prob * 0.5f + (1.0f - noise_prob) * q.m;
+  return q;
+}
+
 // Warp per fragment pair: lanes stride over the L time steps (coalesced: a fragment's rewards are contiguous), shuffle
 // reduction of the discounted difference, lane-parallel write of the 2 L gradient entries.  The minibatch sums (loss,
 // accuracy) are accumulated per CTA and added to the statistics accumulator with one atomic each; a minibatch is a few
@@ -720,11 +739,9 @@ __global__ void __launch_bounds__(256) k_pref_loss(const float* __restrict__ rew
       for (int t = lane; t < L; t += 32) s = fmaf(powf(discount, (float)t), r2[t] - r1[t], s);
     }
     s = warp_sum(s);
-    const bool clipped = s < -threshold || s > threshold;  // th.clip passes the gradient on [min, max] only
-    const float d = fminf(fmaxf(s, -threshold), threshold);
-    const float ed = expf(d);
-    const float m = 1.0f / (1.0f + ed);
-    const float p = noise_prob * 0.5f + (1.0f - noise_prob) * m;
+    const PrefProb q = pref_probability(s, noise_prob, threshold);
+    const bool clipped = q.clipped;  // th.clip passes the gradient on [min, max] only
+    const float ed = q.ed, m = q.m, p = q.p;
     const float y = prefs[pr];
     // F.binary_cross_entropy: logs clamped at -100; backward (p - y) / max(p (1 - p), 1e-12)
     const float lp = fmaxf(logf(p), -100.0f), l1p = fmaxf(log1pf(-p), -100.0f);
@@ -762,6 +779,133 @@ __global__ void __launch_bounds__(256) k_pref_loss(const float* __restrict__ rew
     atomicAdd(stats_acc + 0, a * inv_P);
     atomicAdd(stats_acc + 1, b * inv_P);
     if (blockIdx.x == 0) atomicAdd(stats_acc + 2, 1.0f);
+  }
+}
+
+// ---- active selection of preference queries (imb_pref_uncertainty) ---------------------------------------------------
+// Workspace: word 0 = the ticket, then mom[M][F][2] = each fragment's batch mean and biased variance, then aff[M][F][2] =
+// the (mean, 1 / sqrt(var + eps)) each fragment is normalised with.  The ticket sits at a fixed word so that a workspace
+// reused by calls with different member or candidate counts always finds it where the last call re-armed it.
+__host__ __device__ __forceinline__ int64_t pu_aff_off(int M, int F) { return 1 + 2 * (int64_t)M * F; }
+
+// NormalizedRewardNet members: a warp per (member, fragment) computes the fragment's moments; the last CTA to finish
+// folds them into each member's output RunningNorm in fragment order, one thread per member.  The fold is a chain of
+// F dependent updates, as in the reference, which updates the statistics once per fragment.
+__global__ void __launch_bounds__(256) k_pref_frag_norm(const imb_pref_unc_desc d, int F, int L, float* __restrict__ ws) {
+  const int M = d.n_members;
+  unsigned int* ticket = reinterpret_cast<unsigned int*>(ws);
+  float* mom = ws + 1;
+  float* aff = ws + pu_aff_off(M, F);
+  const int lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+  const int64_t jobs = (int64_t)M * F;
+  for (int64_t j = (int64_t)blockIdx.x * nw + (threadIdx.x >> 5); j < jobs; j += (int64_t)gridDim.x * nw) {
+    const int m = (int)(j / F);
+    if (d.norm_state[m] == nullptr) continue;
+    float mean, m2;
+    warp_moments(d.rews[m] + (j - (int64_t)m * F) * L, L, lane, mean, m2);
+    if (lane == 0) {
+      mom[2 * j] = mean;
+      mom[2 * j + 1] = m2 / (float)L;
+    }
+  }
+  __threadfence();
+  __shared__ bool is_last;
+  __syncthreads();
+  if (threadIdx.x == 0) is_last = atomicAdd(ticket, 1u) == gridDim.x - 1;
+  __syncthreads();
+  if (!is_last) return;
+  __threadfence();
+  if (threadIdx.x == 0) *ticket = 0u;  // re-arm for the next call
+  const int m = threadIdx.x;
+  if (m >= M || d.norm_state[m] == nullptr) return;
+  float* mv = d.norm_state[m];
+  float mean = mv[0], var = mv[1];
+  int32_t cnt = *d.norm_count[m];
+  const float eps = d.norm_eps[m];
+  const float* bm = mom + 2 * (int64_t)m * F;
+  float* out = aff + 2 * (int64_t)m * F;
+#pragma unroll 4
+  for (int f = 0; f < F; ++f) {
+    out[2 * f] = mean;  // normalise fragment f with the statistics from before its own update
+    out[2 * f + 1] = 1.0f / sqrtf(var + eps);
+    norm_fold(mean, var, (float)cnt, __ldcg(bm + 2 * f), __ldcg(bm + 2 * f + 1), (float)L);
+    cnt += L;
+  }
+  mv[0] = mean;
+  mv[1] = var;
+  *d.norm_count[m] = cnt;
+}
+
+// Warp per candidate pair, lanes over t, one register accumulator per member (two for the logit mode's separate
+// returns); each fragment's normalisation is applied as its rewards are read.  Lane 0 then takes the mode's per-member
+// value and a two-pass mean / variance over the members, in member order.
+__global__ void __launch_bounds__(256) k_pref_score(const imb_pref_unc_desc d, int C, int L, int mode, float noise_prob,
+                                                   float discount, float threshold, const float* __restrict__ aff,
+                                                   float* __restrict__ scores, float* __restrict__ member_out) {
+  const int M = d.n_members, F = 2 * C;
+  const int lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+  for (int i = blockIdx.x * nw + (threadIdx.x >> 5); i < C; i += gridDim.x * nw) {
+    float v[IMB_PU_MAX_MEMBERS];
+#pragma unroll
+    for (int m = 0; m < IMB_PU_MAX_MEMBERS; ++m) {
+      v[m] = 0.f;
+      if (m >= M) continue;
+      float mu1 = 0.f, is1 = 1.f, mu2 = 0.f, is2 = 1.f;
+      if (d.norm_state[m] != nullptr) {
+        const float* a = aff + 2 * ((int64_t)m * F + 2 * i);
+        mu1 = a[0];
+        is1 = a[1];
+        mu2 = a[2];
+        is2 = a[3];
+      }
+      const float* r1 = d.rews[m] + (int64_t)(2 * i) * L;
+      const float* r2 = r1 + L;
+      float s1 = 0.f, s2 = 0.f;
+      for (int t = lane; t < L; t += 32) {
+        const float x1 = (r1[t] - mu1) * is1, x2 = (r2[t] - mu2) * is2;
+        if (mode == 0) {
+          s1 += x1;
+          s2 += x2;
+        } else if (discount == 1.0f) {
+          s1 += x2 - x1;
+        } else {
+          s1 = fmaf(powf(discount, (float)t), x2 - x1, s1);
+        }
+      }
+      s1 = warp_sum(s1);
+      if (mode == 0) {
+        v[m] = s1 - warp_sum(s2);  // sum_t r1 - sum_t r2, undiscounted
+      } else {
+        v[m] = pref_probability(s1, noise_prob, threshold).p;
+      }
+    }
+    if (lane != 0) continue;
+    float score;
+    if (mode == 2) {
+      int k = 0;
+#pragma unroll
+      for (int m = 0; m < IMB_PU_MAX_MEMBERS; ++m) k += (m < M && v[m] > 0.5f) ? 1 : 0;
+      const float q = (float)k / (float)M;
+      score = q * (1.0f - q);
+    } else {
+      float s = 0.f;
+#pragma unroll
+      for (int m = 0; m < IMB_PU_MAX_MEMBERS; ++m) s += (m < M) ? v[m] : 0.f;
+      const float mean = s / (float)M;
+      float q = 0.f;
+#pragma unroll
+      for (int m = 0; m < IMB_PU_MAX_MEMBERS; ++m) {
+        const float dv = v[m] - mean;
+        q += (m < M) ? dv * dv : 0.f;
+      }
+      score = q / (float)(mode == 0 ? M - 1 : M);  // torch.var (ddof 1) for logits, np.var (ddof 0) for probabilities
+    }
+    scores[i] = score;
+    if (member_out) {
+#pragma unroll
+      for (int m = 0; m < IMB_PU_MAX_MEMBERS; ++m)
+        if (m < M) member_out[(int64_t)i * M + m] = v[m];
+    }
   }
 }
 
@@ -1201,6 +1345,40 @@ extern "C" int imb_pref_loss(const float* rews, int64_t n_pairs, int32_t frag_le
                                                              threshold, grad_scale, grad_rews, probs_out,
                                                              stats_acc ? stats_acc + 4 * stats_slot : nullptr);
   IMB_CHECK_LAUNCH("k_pref_loss");
+  return 0;
+}
+
+extern "C" int64_t imb_pref_uncertainty_ws_floats(int32_t n_members, int64_t n_pairs) {
+  return 1 + 4 * (int64_t)n_members * 2 * n_pairs;
+}
+
+extern "C" int imb_pref_uncertainty(const imb_pref_unc_desc* d, int64_t n_pairs, int32_t frag_len, int32_t mode,
+                                    float noise_prob, float discount, float threshold, float* ws, float* scores,
+                                    float* member_out, void* stream) {
+  const int M = d->n_members;
+  IMB_REQUIRE(M >= 2 && M <= IMB_PU_MAX_MEMBERS, "imb_pref_uncertainty: %d members (2 to %d)", M, IMB_PU_MAX_MEMBERS);
+  IMB_REQUIRE(n_pairs >= 0 && n_pairs < (1ll << 28) && frag_len >= 1, "imb_pref_uncertainty: bad sizes");
+  IMB_REQUIRE(mode >= 0 && mode <= 2, "imb_pref_uncertainty: mode %d (0 logit, 1 probability, 2 label)", mode);
+  bool any_norm = false;
+  for (int m = 0; m < M; ++m) {
+    IMB_REQUIRE(d->rews[m] != nullptr, "imb_pref_uncertainty: member %d has no rewards", m);
+    IMB_REQUIRE((d->norm_state[m] == nullptr) == (d->norm_count[m] == nullptr),
+                "imb_pref_uncertainty: member %d: norm state and count go together", m);
+    any_norm = any_norm || d->norm_state[m] != nullptr;
+  }
+  if (n_pairs == 0) return 0;
+  const cudaStream_t st = (cudaStream_t)stream;
+  const int C = (int)n_pairs, F = 2 * C;
+  const int64_t cap = 4 * (int64_t)imb_num_sms();
+  if (any_norm) {
+    const int64_t blocks = std::min(((int64_t)M * F + 7) / 8, cap);
+    k_pref_frag_norm<<<(int)blocks, 256, 0, st>>>(*d, F, frag_len, ws);
+    IMB_CHECK_LAUNCH("k_pref_frag_norm");
+  }
+  const int64_t blocks = std::min(((int64_t)C + 7) / 8, cap);
+  k_pref_score<<<(int)blocks, 256, 0, st>>>(*d, C, frag_len, mode, noise_prob, discount, threshold,
+                                            ws + pu_aff_off(M, F), scores, member_out);
+  IMB_CHECK_LAUNCH("k_pref_score");
   return 0;
 }
 

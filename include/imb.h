@@ -318,6 +318,33 @@ int imb_pref_loss(const float* rews, int64_t n_pairs, int32_t frag_len, const fl
                   float discount, float threshold, float grad_scale, float* grad_rews, float* probs_out,
                   float* stats_acc, int32_t stats_slot, void* stream);
 
+/* Active selection of preference queries: ActiveSelectionFragmenter.__call__ + variance_estimate
+ * (algorithms/preference_comparisons.py:721-778), which loops over the candidate pairs in Python and calls
+ * PreferenceModel.rewards -> RewardEnsemble.predict_processed_all (rewards/reward_nets.py:926-951) -> each member's
+ * predict_processed twice per pair.  Member m's raw rewards are rews[m][2C][L] (fragment f = 2 i + s is pair i's first
+ * (s = 0) or second (s = 1) fragment).  A member with norm_state[m] != NULL is a NormalizedRewardNet
+ * (reward_nets.py:637-671): fragment f is normalised with its output statistics as they stood before f, then f's raw
+ * rewards are merged into them (RunningNorm.update_stats, util/networks.py:121-134), in the order f = 0, 1, ..., 2C - 1;
+ * the final statistics and count are written back.  mode 0 (logit): v_m = sum_t r1 - sum_t r2 (undiscounted), score =
+ * variance with ddof 1; mode 1 (probability): v_m = PreferenceModel.probability (:487-530), score = variance with ddof 0;
+ * mode 2 (label): v_m = (probability > 0.5), score = q (1 - q) with q = mean_m v_m.  Outputs: scores[C] and, optional,
+ * member_out[C][M] = the return difference sum r1 - sum r2 (mode 0) or the probability (modes 1, 2) per member.  No
+ * atomics in the arithmetic: two calls give the same bits.  ws: imb_pref_uncertainty_ws_floats(M, C) floats, zero-filled
+ * when allocated; word 0 is a ticket that every call re-arms, so one workspace serves later calls of any size up to the
+ * one it was sized for.  One launch, two when a member is normalised. */
+#define IMB_PU_MAX_MEMBERS 16
+typedef struct imb_pref_unc_desc {
+  int32_t n_members;
+  const float* rews[IMB_PU_MAX_MEMBERS];
+  float* norm_state[IMB_PU_MAX_MEMBERS];   /* [mean, var] of the output RunningNorm, or NULL */
+  int32_t* norm_count[IMB_PU_MAX_MEMBERS];
+  float norm_eps[IMB_PU_MAX_MEMBERS];
+} imb_pref_unc_desc;
+int64_t imb_pref_uncertainty_ws_floats(int32_t n_members, int64_t n_pairs);
+int imb_pref_uncertainty(const imb_pref_unc_desc* d, int64_t n_pairs, int32_t frag_len, int32_t mode,
+                         float noise_prob, float discount, float threshold, float* ws, float* scores,
+                         float* member_out, void* stream);
+
 /* ---- multi-GPU: replica state around the ONE all-reduce of a round ---------------------------
  * (SURVEY.md section 8e; the reference is single-process, so there is no reference interface to
  * cite: the merge restates RunningNorm's Chan update, util/networks.py:96-134, in its additive
