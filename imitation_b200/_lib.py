@@ -77,6 +77,11 @@ class PrefUncDesc(C.Structure):
 
 PU_MODES = {"logit": 0, "probability": 1, "label": 2}
 
+
+class RolloutMembers(C.Structure):
+    _fields_ = [("n_members", C.c_int32), ("params", C.c_void_p * PU_MAX_MEMBERS),
+                ("norm_state", C.c_void_p * PU_MAX_MEMBERS), ("raw", C.c_void_p)]
+
 SYNC_MAX_AVG, SYNC_MAX_NORM = 8, 4
 
 
@@ -98,6 +103,7 @@ SYMBOLS = [
     "imb_sync_buffer_doubles", "imb_sync_snapshot", "imb_sync_pack", "imb_sync_unpack",
     "imb_disc_sample_gather", "imb_sample_advance2", "imb_disc_reduce_adam", "imb_norm_batch_stats", "imb_norm_fold",
     "imb_disc_set_rows", "imb_stats_publish", "imb_pref_loss", "imb_pref_uncertainty_ws_floats", "imb_pref_uncertainty",
+    "imb_rollout_ensemble", "imb_ensemble_relabel_ws_floats", "imb_ensemble_relabel",
 ]
 
 
@@ -113,6 +119,7 @@ def lib() -> C.CDLL:
         _lib.imb_disc_workspace_floats.restype = C.c_int64
         _lib.imb_sync_buffer_doubles.restype = C.c_int64
         _lib.imb_pref_uncertainty_ws_floats.restype = C.c_int64
+        _lib.imb_ensemble_relabel_ws_floats.restype = C.c_int64
         for name in SYMBOLS:
             getattr(_lib, name)  # AttributeError if the .so is stale
     return _lib
@@ -127,7 +134,7 @@ _KERNELS_PER_CALL = {
     "imb_rollout_advance": 1, "imb_env_reset": 1, "imb_ppo_update": 1, "imb_policy_logp": 1,
     "imb_disc_sample_gather": 1, "imb_sample_advance2": 1, "imb_disc_reduce_adam": 1, "imb_norm_batch_stats": 1,
     "imb_norm_fold": 1, "imb_disc_set_rows": 1, "imb_stats_publish": 1, "imb_pref_loss": 1,
-    "imb_pref_uncertainty": None,
+    "imb_pref_uncertainty": None, "imb_rollout_ensemble": 1, "imb_ensemble_relabel": None,
 }
 
 
@@ -352,6 +359,44 @@ def rollout(env, env_params, env_obs, pol, pol_params, pol_norm, disc, disc_para
                              _p(flat_out), _p(aux, th.float32), _p(noise), C.c_int(flags), _p(state, th.int64),
                              _stream()),
            "imb_rollout")
+
+
+def rollout_members(params, norm_states, raw) -> RolloutMembers:
+    """Member table of an ensemble rollout: per member its flat parameter vector and input-norm state (None when the
+    architecture has no input RunningNorm); raw: float32 [M * T * E] for the members' outputs."""
+    if not 2 <= len(params) <= PU_MAX_MEMBERS or len(norm_states) != len(params):
+        raise ImbError(f"imb_rollout_ensemble takes 2 to {PU_MAX_MEMBERS} members, got {len(params)}")
+    d = RolloutMembers()
+    d.n_members = len(params)
+    for m, (pm, nm) in enumerate(zip(params, norm_states)):
+        d.params[m] = _p(pm, th.float32).value
+        d.norm_state[m] = _p(nm, th.float32).value if nm is not None else None
+    d.raw = _p(raw, th.float32).value
+    return d
+
+
+def rollout_ensemble(env, env_params, env_obs, pol, pol_params, pol_norm, disc, members: RolloutMembers, hp, n_envs,
+                     n_steps, rollout_tbl, ring, ring_capacity, flat_out, aux, noise, state, flags=0):
+    """`rollout` with every member's raw reward written to members.raw ([M][T][E]) instead of the reward column."""
+    _check(lib().imb_rollout_ensemble(C.byref(env), _p(env_params, th.float32), _p(env_obs, th.float32), C.byref(pol),
+                                      _p(pol_params, th.float32), _p(pol_norm), C.byref(disc), C.byref(members),
+                                      C.byref(hp), C.c_int64(n_envs), C.c_int64(n_steps), _p(rollout_tbl, th.float32),
+                                      _p(ring), C.c_int64(ring_capacity), _p(flat_out), _p(aux, th.float32), _p(noise),
+                                      C.c_int(flags), _p(state, th.int64), _stream()),
+           "imb_rollout_ensemble")
+
+
+def ensemble_relabel_ws_floats(n_members: int, n_steps: int) -> int:
+    return int(lib().imb_ensemble_relabel_ws_floats(C.c_int32(n_members), C.c_int64(n_steps)))
+
+
+def ensemble_relabel(d: PrefUncDesc, alpha, rollout_tbl, rw, col_rew, n_envs, n_steps, ws):
+    """Per-step output normalisation of the members (d.rews[m] = member m's raw [T][E]) and mean + alpha * std into the
+    rollout table's reward column."""
+    norm = any(d.norm_state[m] for m in range(d.n_members))
+    _check(lib().imb_ensemble_relabel(C.byref(d), C.c_float(alpha), _p(rollout_tbl, th.float32), C.c_int32(rw),
+                                      C.c_int32(col_rew), C.c_int64(n_envs), C.c_int64(n_steps), _p(ws, th.float32),
+                                      _stream()), "imb_ensemble_relabel", 1 + int(norm))
 
 
 def gae(rollout_tbl, rw, col_value, n_envs, n_steps, aux, gamma, gae_lambda, state, horizon):

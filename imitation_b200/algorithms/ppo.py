@@ -55,6 +55,8 @@ class DevicePPO:
         self.exp_avg_sq = th.zeros(n, device=self.device)
         self._tbl = None
         self._aux = None
+        self._ens_raw = None      # ensemble reward: the members' raw rewards [M][T][E]
+        self._ens_ws = None       # ensemble reward: the relabel's workspace
         self.loss_log = None      # optional [n_minibatch_steps][4] device tensor (parity tests)
         self.noise = None         # optional pinned sampling noise for the next rollout (parity tests)
         self.perm = None          # optional host permutations [n_epochs][N] (parity tests)
@@ -101,22 +103,32 @@ class DevicePPO:
         if self._tbl is None or self._tbl.shape[0] != E * T:
             self._tbl = th.zeros(E * T, rw, device=self.device)
             self._aux = th.zeros(2 * E + 2 * E * T, device=self.device)
-        disc = dparams = dnorm = None
+        disc = dparams = dnorm = ens = None
         mode, out_norm = 0, None
         if self._rw_wrapper is not None:
             net, mode, out_norm = self._rw_wrapper.resolve()
-            eng = net.engine()
-            disc, dparams, dnorm = eng.desc, eng.params, eng.norm_state
+            if isinstance(net, reward_wrapper.EnsembleRelabel):
+                ens = net
+            else:
+                eng = net.engine()
+                disc, dparams, dnorm = eng.desc, eng.params, eng.norm_state
         flat, ring = (None, None)
         if self._buffering is not None:
             flat, ring = self._buffering.rollout_targets(T)
         t0 = env.host_ep_step
-        _lib.rollout(env.desc, env.params, env.obs, pol.desc, pp, pn, disc, dparams, dnorm, mode, self.hp, E, T,
-                     self._tbl, ring.table if ring is not None else None, ring.capacity if ring is not None else 0,
-                     flat, self._aux, self.noise, env.state)
+        ring_args = (ring.table if ring is not None else None, ring.capacity if ring is not None else 0)
+        if ens is None:
+            _lib.rollout(env.desc, env.params, env.obs, pol.desc, pp, pn, disc, dparams, dnorm, mode, self.hp, E, T,
+                         self._tbl, *ring_args, flat, self._aux, self.noise, env.state)
+        else:
+            members, relabel = self._ensemble_tables(ens, E, T)
+            _lib.rollout_ensemble(env.desc, env.params, env.obs, pol.desc, pp, pn, ens.nets[0].engine().desc, members,
+                                  self.hp, E, T, self._tbl, *ring_args, flat, self._aux, self.noise, env.state)
         da = 1 if pol.discrete else pol.d_act
         col_val = pol.d_obs + da + 1
-        if out_norm is not None:
+        if ens is not None:
+            _lib.ensemble_relabel(relabel, ens.alpha, self._tbl, rw, col_val + 1, E, T, self._ens_ws)
+        elif out_norm is not None:
             ns, nc = out_norm.output_norm_vectors()
             _lib.reward_norm_scan(self._tbl.view(-1)[col_val + 1:], E, T, rw, T * rw, ns, nc,
                                   out_norm.normalize_output_layer.eps, True)
@@ -124,6 +136,22 @@ class DevicePPO:
         _lib.rollout_advance(env.state, E, T, env.horizon, ring.capacity if ring is not None else 0)
         if not self._capturing:
             self.after_rollout_host(t0)
+
+    def _ensemble_tables(self, ens, E: int, T: int):
+        """Member table of the ensemble rollout and member descriptor of its relabel, over buffers kept across rounds
+        (a captured graph bakes their addresses in)."""
+        M = len(ens.nets)
+        n_ws = _lib.ensemble_relabel_ws_floats(M, T)
+        if self._ens_raw is None or self._ens_raw.numel() != M * T * E:
+            self._ens_raw = th.empty(M * T * E, device=self.device)
+        if self._ens_ws is None or self._ens_ws.numel() < n_ws:
+            self._ens_ws = th.zeros(n_ws, device=self.device)  # zero-filled: the relabel's ticket starts at 0
+        engines = [n.engine() for n in ens.nets]
+        members = _lib.rollout_members([e.params for e in engines],
+                                       [e.norm_state if e.has_norm else None for e in engines], self._ens_raw)
+        norms = [None if o is None else (*o.output_norm_vectors(), float(o.normalize_output_layer.eps))
+                 for o in ens.out_norms]
+        return members, _lib.pref_uncertainty_desc(list(self._ens_raw.view(M, T * E)), norms)
 
     def after_rollout_host(self, t0: int) -> None:
         """Host-side mirrors of what the rollout kernels just did (also called per graph replay)."""
@@ -148,8 +176,18 @@ class DevicePPO:
                self.n_steps, id(self._rw_wrapper), id(self._buffering)]
         if self._rw_wrapper is not None:
             net, mode, out_norm = self._rw_wrapper.resolve()
-            eng = net.engine()
-            key += [eng.params.data_ptr(), eng.norm_state.data_ptr(), mode, id(out_norm)]
+            if isinstance(net, reward_wrapper.EnsembleRelabel):
+                # alpha is a launch argument of the relabel: a new default_alpha needs a new graph
+                key += [net.alpha, self._ens_raw.data_ptr() if self._ens_raw is not None else 0,
+                        self._ens_ws.data_ptr() if self._ens_ws is not None else 0]
+                for n, o in zip(net.nets, net.out_norms):
+                    eng = n.engine()
+                    key += [eng.params.data_ptr(), eng.norm_state.data_ptr(), id(o)]
+                    if o is not None:
+                        key += [t.data_ptr() for t in o.output_norm_vectors()]
+            else:
+                eng = net.engine()
+                key += [eng.params.data_ptr(), eng.norm_state.data_ptr(), mode, id(out_norm)]
         if self._buffering is not None and self._buffering._ring is not None:
             key.append(self._buffering._ring.table.data_ptr())
         return tuple(key)

@@ -836,6 +836,43 @@ __global__ void __launch_bounds__(256) k_pref_frag_norm(const imb_pref_unc_desc 
   *d.norm_count[m] = cnt;
 }
 
+// Ensemble relabel (imb_ensemble_relabel): thread per (t, e), reading each member's raw reward of that step
+// (coalesced along e) and the affine k_pref_frag_norm left for the step, with fragment = env step; two-pass mean and
+// ddof-1 variance over the members in member order, as AddSTDRewardWrapper.predict_processed computes them.
+__global__ void __launch_bounds__(256) k_ensemble_combine(const imb_pref_unc_desc d, int64_t E, int64_t T, float alpha,
+                                                         const float* __restrict__ aff, float* __restrict__ rollout,
+                                                         int rw, int col_rew) {
+  const int M = d.n_members;
+  const int64_t n = E * T;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t t = i / E, e = i - t * E;
+    float v[IMB_PU_MAX_MEMBERS];
+    float s = 0.f;
+#pragma unroll
+    for (int m = 0; m < IMB_PU_MAX_MEMBERS; ++m) {
+      v[m] = 0.f;
+      if (m >= M) continue;
+      float x = __ldg(d.rews[m] + i);
+      if (d.norm_state[m] != nullptr) {
+        const float* a = aff + 2 * ((int64_t)m * T + t);
+        x = (x - a[0]) * a[1];
+      }
+      v[m] = x;
+      s += x;
+    }
+    const float mean = s / (float)M;
+    // every product is rounded before its sum, as numpy computes var and mean + alpha * sqrt(var): no fused
+    // multiply-adds
+    float q = 0.f;
+#pragma unroll
+    for (int m = 0; m < IMB_PU_MAX_MEMBERS; ++m) {
+      const float dv = v[m] - mean;
+      if (m < M) q = __fadd_rn(q, __fmul_rn(dv, dv));
+    }
+    rollout[(e * T + t) * rw + col_rew] = mean + __fmul_rn(alpha, sqrtf(q / (float)(M - 1)));
+  }
+}
+
 // Warp per candidate pair, lanes over t, one register accumulator per member (two for the logit mode's separate
 // returns); each fragment's normalisation is applied as its rewards are read.  Lane 0 then takes the mode's per-member
 // value and a two-pass mean / variance over the members, in member order.
@@ -1379,6 +1416,38 @@ extern "C" int imb_pref_uncertainty(const imb_pref_unc_desc* d, int64_t n_pairs,
   k_pref_score<<<(int)blocks, 256, 0, st>>>(*d, C, frag_len, mode, noise_prob, discount, threshold,
                                             ws + pu_aff_off(M, F), scores, member_out);
   IMB_CHECK_LAUNCH("k_pref_score");
+  return 0;
+}
+
+extern "C" int64_t imb_ensemble_relabel_ws_floats(int32_t n_members, int64_t n_steps) {
+  return pu_aff_off(n_members, (int)n_steps) + 2 * (int64_t)n_members * n_steps;
+}
+
+extern "C" int imb_ensemble_relabel(const imb_pref_unc_desc* d, float alpha, float* rollout, int32_t rw, int32_t col_rew,
+                                    int64_t n_envs, int64_t n_steps, float* ws, void* stream) {
+  const int M = d->n_members;
+  IMB_REQUIRE(M >= 2 && M <= IMB_PU_MAX_MEMBERS, "imb_ensemble_relabel: %d members (2 to %d)", M, IMB_PU_MAX_MEMBERS);
+  IMB_REQUIRE(n_envs >= 1 && n_steps >= 1 && n_envs * n_steps < (1ll << 31), "imb_ensemble_relabel: bad sizes");
+  IMB_REQUIRE(col_rew >= 0 && col_rew < rw, "imb_ensemble_relabel: reward column %d outside rows of %d", col_rew, rw);
+  bool any_norm = false;
+  for (int m = 0; m < M; ++m) {
+    IMB_REQUIRE(d->rews[m] != nullptr, "imb_ensemble_relabel: member %d has no rewards", m);
+    IMB_REQUIRE((d->norm_state[m] == nullptr) == (d->norm_count[m] == nullptr),
+                "imb_ensemble_relabel: member %d: norm state and count go together", m);
+    any_norm = any_norm || d->norm_state[m] != nullptr;
+  }
+  const cudaStream_t st = (cudaStream_t)stream;
+  const int F = (int)n_steps, L = (int)n_envs;  // fragment = one env step of E rewards
+  const int64_t cap = 4 * (int64_t)imb_num_sms();
+  if (any_norm) {
+    const int64_t blocks = std::min(((int64_t)M * F + 7) / 8, cap);
+    k_pref_frag_norm<<<(int)blocks, 256, 0, st>>>(*d, F, L, ws);
+    IMB_CHECK_LAUNCH("k_pref_frag_norm");
+  }
+  const int64_t blocks = std::min((n_envs * n_steps + 255) / 256, 8 * (int64_t)imb_num_sms());
+  k_ensemble_combine<<<(int)blocks, 256, 0, st>>>(*d, n_envs, n_steps, alpha, ws + pu_aff_off(M, F), rollout, rw,
+                                                  col_rew);
+  IMB_CHECK_LAUNCH("k_ensemble_combine");
   return 0;
 }
 

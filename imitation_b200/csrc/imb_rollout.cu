@@ -7,12 +7,13 @@ extern "C" int imb_rollout_row_width(const imb_policy_desc* pol) {
   return (pol->d_obs + (pol->discrete ? 1 : pol->d_act) + 5 + 3) / 4 * 4;
 }
 
-extern "C" int imb_rollout(const imb_env_desc* env, const float* env_params, float* env_obs,
-                           const imb_policy_desc* pol, const float* pol_params, const float* pol_norm,
-                           const imb_disc_desc* disc, const float* disc_params, const float* disc_norm,
-                           int reward_mode, const imb_ppo_hparams* hp, int64_t n_envs, int64_t n_steps,
-                           float* rollout, float* ring, int64_t ring_capacity, float* flat_out, float* aux,
-                           const float* noise, int flags, const int64_t* state, void* stream) {
+// members == nullptr: imb_rollout; otherwise imb_rollout_ensemble (reward_mode 2, member m's vectors from the table)
+static int rollout_common(const imb_env_desc* env, const float* env_params, float* env_obs, const imb_policy_desc* pol,
+                          const float* pol_params, const float* pol_norm, const imb_disc_desc* disc,
+                          const float* disc_params, const float* disc_norm, const imb_rollout_members* members,
+                          int reward_mode, const imb_ppo_hparams* hp, int64_t n_envs, int64_t n_steps, float* rollout,
+                          float* ring, int64_t ring_capacity, float* flat_out, float* aux, const float* noise, int flags,
+                          const int64_t* state, void* stream) {
   IMB_REQUIRE(n_envs >= 1 && n_steps >= 1, "rollout needs n_envs, n_steps >= 1");
   IMB_REQUIRE(env->d_obs == pol->d_obs && env->d_act == pol->d_act && env->discrete == pol->discrete,
               "env / policy space mismatch");
@@ -31,16 +32,58 @@ extern "C" int imb_rollout(const imb_env_desc* env, const float* env_params, flo
   DiscLaunch L;
   memset(&L, 0, sizeof(L));
   if (reward_mode != 0) {
-    IMB_REQUIRE(disc && disc_params, "reward_mode != 0 needs a reward net");
+    IMB_REQUIRE(disc && (disc_params || members), "reward_mode != 0 needs a reward net");
     const int onehot = env->discrete ? env->d_act : env->d_act;
     IMB_REQUIRE(disc->d_obs == env->d_obs && disc->d_act == onehot, "reward net / env space mismatch");
     imb_disc_desc dd = *disc;
     dd.subtract_logp = 0;  // reward_train.predict_processed never subtracts log pi (airl.py:121-124)
-    if (int rc = build_launch(&dd, disc_norm, nullptr, L)) return rc;
+    if (int rc = build_launch(&dd, members ? members->norm_state[0] : disc_norm, nullptr, L)) return rc;
   }
   cudaStream_t st = (cudaStream_t)stream;
-  return launch_rollout(A, L, env_params, env_obs, pol_params, pol_norm, disc_params, rollout, ring, flat_out, aux,
+  if (!members)
+    return launch_rollout(A, L, nullptr, env_params, env_obs, pol_params, pol_norm, disc_params, rollout, ring,
+                          flat_out, aux, noise, state, st);
+  const int M = members->n_members;
+  IMB_REQUIRE(M >= 2 && M <= IMB_PU_MAX_MEMBERS, "imb_rollout_ensemble: %d members (2 to %d)", M, IMB_PU_MAX_MEMBERS);
+  IMB_REQUIRE(members->raw != nullptr, "imb_rollout_ensemble: no raw-output buffer");
+  const bool in_norm = disc->base.has_norm || (disc->shaped && disc->potential.has_norm);
+  RolloutMembers Mb;
+  memset(&Mb, 0, sizeof(Mb));
+  Mb.M = M;
+  Mb.raw = members->raw;
+  for (int m = 0; m < M; ++m) {
+    IMB_REQUIRE(members->params[m] != nullptr, "imb_rollout_ensemble: member %d has no parameters", m);
+    IMB_REQUIRE(!in_norm || members->norm_state[m] != nullptr, "imb_rollout_ensemble: member %d has no input norm", m);
+    Mb.params[m] = members->params[m];
+    for (int p = 0; p < L.npass; ++p) {
+      const imb_mlp& mlp = p == 0 ? disc->base : disc->potential;
+      Mb.norm[m][p] = mlp.has_norm ? members->norm_state[m] + mlp.norm_off : nullptr;
+    }
+  }
+  return launch_rollout(A, L, &Mb, env_params, env_obs, pol_params, pol_norm, nullptr, rollout, ring, flat_out, aux,
                         noise, state, st);
+}
+
+extern "C" int imb_rollout(const imb_env_desc* env, const float* env_params, float* env_obs,
+                           const imb_policy_desc* pol, const float* pol_params, const float* pol_norm,
+                           const imb_disc_desc* disc, const float* disc_params, const float* disc_norm,
+                           int reward_mode, const imb_ppo_hparams* hp, int64_t n_envs, int64_t n_steps,
+                           float* rollout, float* ring, int64_t ring_capacity, float* flat_out, float* aux,
+                           const float* noise, int flags, const int64_t* state, void* stream) {
+  return rollout_common(env, env_params, env_obs, pol, pol_params, pol_norm, disc, disc_params, disc_norm, nullptr,
+                        reward_mode, hp, n_envs, n_steps, rollout, ring, ring_capacity, flat_out, aux, noise, flags,
+                        state, stream);
+}
+
+extern "C" int imb_rollout_ensemble(const imb_env_desc* env, const float* env_params, float* env_obs,
+                                    const imb_policy_desc* pol, const float* pol_params, const float* pol_norm,
+                                    const imb_disc_desc* disc, const imb_rollout_members* members,
+                                    const imb_ppo_hparams* hp, int64_t n_envs, int64_t n_steps, float* rollout,
+                                    float* ring, int64_t ring_capacity, float* flat_out, float* aux, const float* noise,
+                                    int flags, const int64_t* state, void* stream) {
+  IMB_REQUIRE(disc && members, "imb_rollout_ensemble needs a member architecture and a member table");
+  return rollout_common(env, env_params, env_obs, pol, pol_params, pol_norm, disc, nullptr, nullptr, members, 2, hp,
+                        n_envs, n_steps, rollout, ring, ring_capacity, flat_out, aux, noise, flags, state, stream);
 }
 
 extern "C" int imb_rollout_advance(int64_t* state, int64_t n_envs, int64_t n_steps, int32_t horizon,

@@ -45,6 +45,16 @@ struct RolloutArgs {
   int pol_off, env_off, img_off, img_sz, obsu_off, xn_off, h1_off, h2_off, nobs_off, vec_off, total;
 };
 
+// Ensemble relabel (imb_rollout_ensemble): M members of the one architecture DiscLaunch describes, member m with its own
+// parameter vector and per-pass input-norm state; member m's raw output of env e at step t goes to
+// raw[(m * T + t) * E + e] (step-major: a step's E rewards are contiguous, as imb_ensemble_relabel reads them).
+struct RolloutMembers {
+  int M;
+  const float* params[IMB_PU_MAX_MEMBERS];
+  const float* norm[IMB_PU_MAX_MEMBERS][MAX_PASS];  // nullptr where the pass has no input RunningNorm
+  float* raw;
+};
+
 // policy image (runtime tower width HP, zero padded):
 //   piW1t[Do][HP] pib1[HP] piW2t[HP][HP] pib2[HP] vfW1t vfb1 vfW2t vfb2 Wa[Da][HP] ba[64] wv[HP] bv[4] lstd[64] mean[64] istd[64]
 struct PolImg {
@@ -208,8 +218,10 @@ __device__ __forceinline__ void tile_layer(const float* __restrict__ A, int K, c
   }
 }
 
-template <int RPL>
-__global__ void __launch_bounds__(RT, 1) k_rollout(const RolloutArgs A, const DiscLaunch L,
+// ENS: evaluate the Mb.M ensemble members (raw outputs to Mb.raw) instead of the one net at disc_params (reward to the
+// table's reward column); the single-net variant is compiled without the member loop.
+template <int RPL, bool ENS>
+__global__ void __launch_bounds__(RT, 1) k_rollout(const RolloutArgs A, const DiscLaunch L, const RolloutMembers Mb,
                                                    const float* __restrict__ env_params, float* __restrict__ env_obs,
                                                    const float* __restrict__ pol_params,
                                                    const float* __restrict__ pol_norm,
@@ -234,11 +246,13 @@ __global__ void __launch_bounds__(RT, 1) k_rollout(const RolloutArgs A, const Di
   float* vec = smem + A.vec_off;   // lg[RT]
   float* lg = vec;
 
+  const int n_mem = ENS ? Mb.M : 1;
   // ---- one-time loads ------------------------------------------------------------------------------
   if (A.reward_mode != 0)
-    for (int p = 0; p < L.npass; ++p)
-      load_timg(smem + A.img_off + p * A.img_sz, L.pass[p], JP, disc_params,
-                L.pass[p].has_norm ? L.pass[p].norm : nullptr, L.pass[p].eps);
+    for (int m = 0; m < n_mem; ++m)
+      for (int p = 0; p < L.npass; ++p)
+        load_timg(smem + A.img_off + (m * L.npass + p) * A.img_sz, L.pass[p], JP, ENS ? Mb.params[m] : disc_params,
+                  ENS ? Mb.norm[m][p] : (L.pass[p].has_norm ? L.pass[p].norm : nullptr), L.pass[p].eps);
   load_policy_img(psm, S, A.pol, HP, pol_params, pol_norm);
   for (int i = tid; i < (KU + 2) * IP; i += RT) esm[i] = 0.f;
   __syncthreads();
@@ -433,56 +447,59 @@ __global__ void __launch_bounds__(RT, 1) k_rollout(const RolloutArgs A, const Di
     done = ((t0 + t + 1) % H) == 0;
     const float donef = done ? 1.f : 0.f;
 
-    // ---- learned reward on (obs, clipped act, terminal-fixed next obs, done) ----------------------------------------
+    // ---- learned reward on (obs, clipped act, terminal-fixed next obs, done); ensemble: every member in turn ---------
     float reward = rew_env;
     if (A.reward_mode != 0) {
-      for (int p = 0; p < L.npass; ++p) {
-        const PassDesc& Pd = L.pass[p];
-        const float* img = smem + A.img_off + p * A.img_sz;
-        const int din = Pd.din;
-        const float* mean = img + TImg::mean(din, JP);
-        const float* istd = img + TImg::istd(din, JP);
-        for (int i = tid; i < din * (RR / 4); i += RT) {
-          const int k = i / (RR / 4), r4 = (i - k * (RR / 4)) * 4;
-          const int fr = L.stage_row[Pd.in_slot[k]];  // batch feature row -> source tile row
-          float4 x;
-          if (fr < Do + Da) x = ld4(OBSU + fr * RRS + r4);
-          else if (fr < 2 * Do + Da) x = ld4(NOBS + (fr - Do - Da) * RRS + r4);
-          else x = make_float4(donef, donef, donef, donef);
-          const float m = mean[k], is = istd[k];
-          st4(XN + k * RRS + r4, make_float4((x.x - m) * is, (x.y - m) * is, (x.z - m) * is, (x.w - m) * is));
-        }
-        __syncthreads();
-        const float* HL = XN;
-        int hl = din;
-        if (Pd.n_hidden >= 1) {
-          tile_layer<ACT_RELU, RPL>(XN, din, img + TImg::w1t(din, JP), JP, img + TImg::b1(din, JP), H1, JP);
+      for (int mi = 0; mi < n_mem; ++mi) {
+        for (int p = 0; p < L.npass; ++p) {
+          const PassDesc& Pd = L.pass[p];
+          const float* img = smem + A.img_off + (mi * L.npass + p) * A.img_sz;
+          const int din = Pd.din;
+          const float* mean = img + TImg::mean(din, JP);
+          const float* istd = img + TImg::istd(din, JP);
+          for (int i = tid; i < din * (RR / 4); i += RT) {
+            const int k = i / (RR / 4), r4 = (i - k * (RR / 4)) * 4;
+            const int fr = L.stage_row[Pd.in_slot[k]];  // batch feature row -> source tile row
+            float4 x;
+            if (fr < Do + Da) x = ld4(OBSU + fr * RRS + r4);
+            else if (fr < 2 * Do + Da) x = ld4(NOBS + (fr - Do - Da) * RRS + r4);
+            else x = make_float4(donef, donef, donef, donef);
+            const float m = mean[k], is = istd[k];
+            st4(XN + k * RRS + r4, make_float4((x.x - m) * is, (x.y - m) * is, (x.z - m) * is, (x.w - m) * is));
+          }
           __syncthreads();
-          HL = H1;
-          hl = Pd.h1;
-        }
-        if (Pd.n_hidden >= 2) {
-          tile_layer<ACT_RELU, RPL>(H1, Pd.h1, img + TImg::w2t(din, JP), JP, img + TImg::b2(din, JP), H2, JP);
+          const float* HL = XN;
+          int hl = din;
+          if (Pd.n_hidden >= 1) {
+            tile_layer<ACT_RELU, RPL>(XN, din, img + TImg::w1t(din, JP), JP, img + TImg::b1(din, JP), H1, JP);
+            __syncthreads();
+            HL = H1;
+            hl = Pd.h1;
+          }
+          if (Pd.n_hidden >= 2) {
+            tile_layer<ACT_RELU, RPL>(H1, Pd.h1, img + TImg::w2t(din, JP), JP, img + TImg::b2(din, JP), H2, JP);
+            __syncthreads();
+            HL = H2;
+            hl = Pd.h2;
+          }
+          const float* wf = img + TImg::wf(din, JP);
+          float o0 = 0.f, o1 = 0.f;
+          int j = 0;
+          for (; j + 2 <= hl; j += 2) {
+            o0 = fmaf(wf[j], HL[j * RRS + rt], o0);
+            o1 = fmaf(wf[j + 1], HL[(j + 1) * RRS + rt], o1);
+          }
+          if (j < hl) o0 = fmaf(wf[j], HL[j * RRS + rt], o0);
+          const float o = img[TImg::bf(din, JP)] + (o0 + o1);
+          const float c = pass_coef(Pd.coef_kind, L.gamma, donef);
+          lg[tid] = (p == 0) ? c * o : fmaf(c, o, lg[tid]);
           __syncthreads();
-          HL = H2;
-          hl = Pd.h2;
         }
-        const float* wf = img + TImg::wf(din, JP);
-        float o0 = 0.f, o1 = 0.f;
-        int j = 0;
-        for (; j + 2 <= hl; j += 2) {
-          o0 = fmaf(wf[j], HL[j * RRS + rt], o0);
-          o1 = fmaf(wf[j + 1], HL[(j + 1) * RRS + rt], o1);
-        }
-        if (j < hl) o0 = fmaf(wf[j], HL[j * RRS + rt], o0);
-        const float o = img[TImg::bf(din, JP)] + (o0 + o1);
-        const float c = pass_coef(Pd.coef_kind, L.gamma, donef);
-        lg[tid] = (p == 0) ? c * o : fmaf(c, o, lg[tid]);
-        __syncthreads();
+        if (ENS && live) Mb.raw[((int64_t)mi * T + t) * E + e] = lg[tid];  // (lg[tid] is only rewritten by this thread)
       }
       reward = (A.reward_mode == 1) ? softplus_f(lg[tid]) : lg[tid];
     }
-    if (live) row[col_rew] = reward;
+    if (live && !ENS) row[col_rew] = reward;  // ensemble: imb_ensemble_relabel writes the combined reward
 
     // ---- time-limit bootstrap term gamma * V(terminal obs) (added after reward normalisation) -------------------
     float boot = 0.f;
@@ -590,11 +607,11 @@ __global__ void k_env_reset(float* __restrict__ env_obs, int64_t E, int d_obs, u
 
 }  // namespace
 
-template <int RPL>
-static int launch_rollout_t(RolloutArgs A, const DiscLaunch& L, const float* env_params, float* env_obs,
-                            const float* pol_params, const float* pol_norm, const float* disc_params, float* rollout,
-                            float* ring, float* flat_out, float* aux, const float* noise, const int64_t* state,
-                            cudaStream_t st) {
+template <int RPL, bool ENS>
+static int launch_rollout_t(RolloutArgs A, const DiscLaunch& L, const RolloutMembers& Mb, const float* env_params,
+                            float* env_obs, const float* pol_params, const float* pol_norm, const float* disc_params,
+                            float* rollout, float* ring, float* flat_out, float* aux, const float* noise,
+                            const int64_t* state, cudaStream_t st) {
   constexpr int RR = rows_of(RPL), RRS = RR + TILE_PAD;
   auto al = [](int x) { return (x + 31) / 32 * 32; };
   const int Do = A.env.d_obs, Da = A.env.d_act;
@@ -618,7 +635,8 @@ static int launch_rollout_t(RolloutArgs A, const DiscLaunch& L, const float* env
   o += al((A.KU + 2) * A.IP);
   A.img_off = o;
   A.img_sz = al(TImg::size(dmax, A.JP));
-  if (A.reward_mode != 0) o += L.npass * A.img_sz;
+  const int n_img = A.reward_mode != 0 ? (ENS ? Mb.M : 1) * L.npass : 0;  // every member's images stay resident
+  o += n_img * A.img_sz;
   A.obsu_off = o;
   o += al(A.KU * RRS);
   A.xn_off = o;
@@ -633,29 +651,37 @@ static int launch_rollout_t(RolloutArgs A, const DiscLaunch& L, const float* env
   o += al(RT);
   A.total = o;
   const size_t bytes = (size_t)o * 4;
+  IMB_REQUIRE(!ENS || bytes <= IMB_SMEM_MAX,
+              "rollout of a %d-member ensemble needs %zu B of shared memory (%zu B for the member images), more than "
+              "the %d B a CTA can hold: use fewer or narrower members", Mb.M, bytes, (size_t)n_img * A.img_sz * 4,
+              (int)IMB_SMEM_MAX);
   IMB_REQUIRE(bytes <= IMB_SMEM_MAX, "rollout kernel needs %zu B of shared memory", bytes);
   static size_t attr_bytes = 0;
   if (bytes > attr_bytes) {
-    cudaError_t e = cudaFuncSetAttribute(k_rollout<RPL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    cudaError_t e = cudaFuncSetAttribute(k_rollout<RPL, ENS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
     if (e != cudaSuccess) IMB_FAIL(-2, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
     attr_bytes = bytes;
   }
   const int blocks = (int)((A.E + RR - 1) / RR);
-  k_rollout<RPL><<<blocks, RT, bytes, st>>>(A, L, env_params, env_obs, pol_params, pol_norm, disc_params, rollout, ring,
-                                            flat_out, aux, noise, state);
+  k_rollout<RPL, ENS><<<blocks, RT, bytes, st>>>(A, L, Mb, env_params, env_obs, pol_params, pol_norm, disc_params,
+                                                 rollout, ring, flat_out, aux, noise, state);
   IMB_CHECK_LAUNCH("k_rollout");
   return 0;
 }
 
-static int launch_rollout(const RolloutArgs& A, const DiscLaunch& L, const float* env_params, float* env_obs,
-                          const float* pol_params, const float* pol_norm, const float* disc_params, float* rollout,
-                          float* ring, float* flat_out, float* aux, const float* noise, const int64_t* state,
-                          cudaStream_t st) {
+// Mb == nullptr: the single-net rollout
+static int launch_rollout(const RolloutArgs& A, const DiscLaunch& L, const RolloutMembers* Mb, const float* env_params,
+                          float* env_obs, const float* pol_params, const float* pol_norm, const float* disc_params,
+                          float* rollout, float* ring, float* flat_out, float* aux, const float* noise,
+                          const int64_t* state, cudaStream_t st) {
   // smallest tile that still covers the SMs: the kernel's duration is one CTA's latency
   const int64_t sms = imb_num_sms();
-#define IMB_RL(R) \
-  return launch_rollout_t<R>(A, L, env_params, env_obs, pol_params, pol_norm, disc_params, rollout, ring, flat_out, aux, \
-                             noise, state, st)
+  static const RolloutMembers no_members = {};
+#define IMB_RL(R)                                                                                                     \
+  return Mb ? launch_rollout_t<R, true>(A, L, *Mb, env_params, env_obs, pol_params, pol_norm, disc_params, rollout, \
+                                        ring, flat_out, aux, noise, state, st)                                      \
+            : launch_rollout_t<R, false>(A, L, no_members, env_params, env_obs, pol_params, pol_norm, disc_params,   \
+                                         rollout, ring, flat_out, aux, noise, state, st)
   if (A.E <= sms * 8 * 2) IMB_RL(0);
   if (A.E <= sms * 32) IMB_RL(1);
   if (A.E <= sms * 64 * 2) IMB_RL(2);

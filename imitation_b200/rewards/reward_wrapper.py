@@ -7,6 +7,7 @@ kernel evaluates the reward network in place (csrc/imb_rollout.cu), so `reward_f
 """
 import collections
 
+from .. import _lib
 from . import reward_nets
 
 
@@ -41,16 +42,28 @@ class RewardVecEnvWrapper:
         return self.venv.reset()
 
     def resolve(self):
-        """-> (fused net with engine, reward_mode, NormalizedRewardNet or None) for the rollout kernel."""
+        """-> (fused net with engine, reward_mode, NormalizedRewardNet or None) for the rollout kernel; for an ensemble
+        reward (`AddSTDRewardWrapper(RewardEnsemble)` or a bare `RewardEnsemble`) -> (EnsembleRelabel, 2, None)."""
         net = getattr(self.reward_fn, "__self__", None)
         if not isinstance(net, reward_nets.RewardNet) or getattr(self.reward_fn, "__name__", "") != "predict_processed":
             raise NotImplementedError("RewardVecEnvWrapper on the GPU path needs reward_fn = <RewardNet>.predict_processed")
+        if isinstance(net, (reward_nets.AddSTDRewardWrapper, reward_nets.RewardEnsemble)):
+            # built once per ensemble (its checks sync every member's engine); rebuilt when the members change
+            ens = net.base if isinstance(net, reward_nets.AddSTDRewardWrapper) else net
+            key = (id(net), tuple(id(m) for m in getattr(ens, "members", ())))
+            cached = self.__dict__.get("_ensemble")
+            if cached is None or cached[0] != key:
+                self._ensemble = (key, EnsembleRelabel(net))
+            return self._ensemble[1], 2, None
         mode, out_norm = 2, None
         from ..algorithms.adversarial import gail
 
         if isinstance(net, gail.RewardNetFromDiscriminatorLogit):
             mode, net = 1, net.base
         if isinstance(net, reward_nets.NormalizedRewardNet):
+            if isinstance(net.base, (reward_nets.AddSTDRewardWrapper, reward_nets.RewardNetWithVariance)):
+                raise NotImplementedError("a NormalizedRewardNet around an ensemble reward is not supported (the "
+                                          "reference rejects it too): normalise the members instead")
             if mode == 1:
                 net = net.base  # GAIL bypasses the output normaliser (gail.py:82-83, SURVEY Appendix A.6)
             else:
@@ -60,3 +73,43 @@ class RewardVecEnvWrapper:
         if not hasattr(net, "_engine"):
             raise NotImplementedError(f"reward net {type(net).__name__} has no fused sm_90a implementation")
         return net, mode, out_norm
+
+
+class EnsembleRelabel:
+    """An ensemble reward as the rollout evaluates it (reward_nets.py:926-989, :1045-1080): up to 16 members of one
+    fused architecture, each either plain or inside a `NormalizedRewardNet` (all members alike), combined per step into
+    mean + alpha * std.  `alpha` is read from the wrapper on every access, so a changed `default_alpha` takes effect at
+    the next rollout."""
+
+    def __init__(self, reward: reward_nets.RewardNet):
+        self.reward = reward  # (held: the resolve() cache is keyed on its identity)
+        self.wrapper = reward if isinstance(reward, reward_nets.AddSTDRewardWrapper) else None
+        ensemble = reward.base if self.wrapper is not None else reward
+        if not isinstance(ensemble, reward_nets.RewardEnsemble):
+            raise NotImplementedError(f"AddSTDRewardWrapper around {type(ensemble).__name__}: the GPU rollout fuses "
+                                      "only a RewardEnsemble's variance")
+        members = list(ensemble.members)
+        if len(members) > _lib.PU_MAX_MEMBERS:
+            raise NotImplementedError(f"the GPU rollout evaluates at most {_lib.PU_MAX_MEMBERS} ensemble members, "
+                                      f"got {len(members)}")
+        self.nets, self.out_norms = [], []
+        for k, m in enumerate(members):
+            out_norm = m if isinstance(m, reward_nets.NormalizedRewardNet) else None
+            net = m.base if out_norm is not None else m
+            if not hasattr(net, "_engine"):
+                raise NotImplementedError(f"ensemble member {k} ({type(net).__name__}) has no fused sm_90a "
+                                          "implementation")
+            self.nets.append(net)
+            self.out_norms.append(out_norm)
+        if len({o is None for o in self.out_norms}) > 1:
+            raise NotImplementedError("ensemble members must all be NormalizedRewardNets or all plain reward nets, "
+                                      "not a mix")
+        d0 = bytes(self.nets[0].engine().desc)
+        for k, net in enumerate(self.nets[1:], 1):
+            if bytes(net.engine().desc) != d0:
+                raise NotImplementedError(f"ensemble member {k} has a different architecture from member 0: the GPU "
+                                          "rollout evaluates members of one architecture")
+
+    @property
+    def alpha(self) -> float:
+        return float(self.wrapper.default_alpha) if self.wrapper is not None else 0.0

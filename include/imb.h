@@ -345,6 +345,40 @@ int imb_pref_uncertainty(const imb_pref_unc_desc* d, int64_t n_pairs, int32_t fr
                          float noise_prob, float discount, float threshold, float* ws, float* scores,
                          float* member_out, void* stream);
 
+/* ---- agent training on an ensemble reward ----------------------------------------------------------------------------
+ * RewardVecEnvWrapper with reward_fn = AddSTDRewardWrapper(RewardEnsemble(members), alpha).predict_processed or
+ * RewardEnsemble(members).predict_processed (rewards/reward_wrapper.py:92-133 -> rewards/reward_nets.py:1045-1080,
+ * :926-989 -> each member's predict_processed, :637-671 for a NormalizedRewardNet member).
+ *
+ * imb_rollout_ensemble = imb_rollout with reward_mode 2 for M members of the ONE architecture `disc`: member m has its
+ * own parameter vector params[m] and input-norm state norm_state[m] (both laid out as `disc` describes; NULL norm state
+ * when `disc` has no input RunningNorm).  Every member is evaluated in eval mode (input norms not updated) on the same
+ * (obs, clipped act, terminal-fixed next obs, done) as imb_rollout's single net, and its raw output for env e at step t
+ * goes to raw[(m * T + t) * E + e] instead of the rollout table's reward column.  All M member images are resident in
+ * shared memory; the call fails, naming the limit, when they do not fit. */
+typedef struct imb_rollout_members {
+  int32_t n_members;                            /* 2 .. IMB_PU_MAX_MEMBERS */
+  const float* params[IMB_PU_MAX_MEMBERS];
+  const float* norm_state[IMB_PU_MAX_MEMBERS];  /* input RunningNorm state [mean | var] per `disc`'s norm_off, or NULL */
+  float* raw;                                   /* [M][T][E] raw member outputs */
+} imb_rollout_members;
+int imb_rollout_ensemble(const imb_env_desc* env, const float* env_params, float* env_obs,
+                         const imb_policy_desc* pol, const float* pol_params, const float* pol_norm,
+                         const imb_disc_desc* disc, const imb_rollout_members* members,
+                         const imb_ppo_hparams* hp, int64_t n_envs, int64_t n_steps, float* rollout, float* ring,
+                         int64_t ring_capacity, float* flat_out, float* aux, const float* noise, int flags,
+                         const int64_t* state, void* stream);
+/* The relabel of the ensemble rollout, before imb_gae: d->rews[m] = member m's raw[T][E] from imb_rollout_ensemble.
+ * Per env step t, member m with d->norm_state[m] != NULL is normalised with its output statistics from before step t,
+ * then step t's E raw rewards are merged into them (RunningNorm.update_stats, util/networks.py:121-134), so the
+ * statistics and count end as E*T separate predict_processed calls leave them; a member without one is used raw.
+ * rollout[(e*T + t)*rw + col_rew] = mean_m v_m + alpha * sqrt(var_m(v_m, ddof 1)), the mean and variance two-pass in
+ * member order (alpha = 0 for a bare RewardEnsemble).  No atomics in the arithmetic: two calls give the same bits.
+ * ws: imb_ensemble_relabel_ws_floats(M, T) floats, zero-filled when allocated (word 0 is a ticket every call re-arms). */
+int64_t imb_ensemble_relabel_ws_floats(int32_t n_members, int64_t n_steps);
+int imb_ensemble_relabel(const imb_pref_unc_desc* d, float alpha, float* rollout, int32_t rw, int32_t col_rew,
+                         int64_t n_envs, int64_t n_steps, float* ws, void* stream);
+
 /* ---- multi-GPU: replica state around the ONE all-reduce of a round ---------------------------
  * (SURVEY.md section 8e; the reference is single-process, so there is no reference interface to
  * cite: the merge restates RunningNorm's Chan update, util/networks.py:96-134, in its additive
