@@ -72,7 +72,8 @@ PU_MAX_MEMBERS = 16
 class PrefUncDesc(C.Structure):
     _fields_ = [("n_members", C.c_int32), ("rews", C.c_void_p * PU_MAX_MEMBERS),
                 ("norm_state", C.c_void_p * PU_MAX_MEMBERS), ("norm_count", C.c_void_p * PU_MAX_MEMBERS),
-                ("norm_eps", C.c_float * PU_MAX_MEMBERS)]
+                ("norm_eps", C.c_float * PU_MAX_MEMBERS), ("norm_kind", C.c_int32 * PU_MAX_MEMBERS),
+                ("norm_decay", C.c_float * PU_MAX_MEMBERS)]
 
 
 PU_MODES = {"logit": 0, "probability": 1, "label": 2}
@@ -97,7 +98,8 @@ _lib: Optional[C.CDLL] = None
 # every symbol include/imb.h declares (tests check the library exports each of them)
 SYMBOLS = [
     "imb_version", "imb_last_error", "imb_disc_workspace_floats", "imb_disc_norm_update", "imb_disc_fwd_bwd",
-    "imb_disc_reduce", "imb_disc_adam", "imb_reward_forward", "imb_reward_norm_scan", "imb_table_store",
+    "imb_disc_reduce", "imb_disc_adam", "imb_reward_forward", "imb_reward_norm_scan", "imb_reward_ema_scan",
+    "imb_table_store",
     "imb_ring_advance", "imb_sample_indices", "imb_gather_rows", "imb_rollout", "imb_rollout_row_width", "imb_gae",
     "imb_rollout_advance", "imb_env_reset", "imb_ppo_update", "imb_policy_logp", "imb_state_init",
     "imb_sync_buffer_doubles", "imb_sync_snapshot", "imb_sync_pack", "imb_sync_unpack",
@@ -129,7 +131,8 @@ def lib() -> C.CDLL:
 LAUNCHES = {"count": 0}
 _KERNELS_PER_CALL = {
     "imb_state_init": 0, "imb_disc_norm_update": None, "imb_disc_fwd_bwd": 1, "imb_disc_reduce": 1,
-    "imb_disc_adam": 1, "imb_reward_forward": 1, "imb_reward_norm_scan": 1, "imb_table_store": 1,
+    "imb_disc_adam": 1, "imb_reward_forward": 1, "imb_reward_norm_scan": 1, "imb_reward_ema_scan": 1,
+    "imb_table_store": 1,
     "imb_ring_advance": 1, "imb_sample_indices": 2, "imb_gather_rows": 1, "imb_rollout": 1, "imb_gae": 1,
     "imb_rollout_advance": 1, "imb_env_reset": 1, "imb_ppo_update": 1, "imb_policy_logp": 1,
     "imb_disc_sample_gather": 1, "imb_sample_advance2": 1, "imb_disc_reduce_adam": 1, "imb_norm_batch_stats": 1,
@@ -269,8 +272,9 @@ def pref_loss(rews, n_pairs, frag_len, prefs, noise_prob, discount, threshold, g
 
 
 def pref_uncertainty_desc(rews, norms) -> PrefUncDesc:
-    """rews: one float32 CUDA tensor [2C * L] per member; norms: per member None or (state [mean, var], int32 count, eps)
-    of its output RunningNorm."""
+    """rews: one float32 CUDA tensor [2C * L] per member; norms: per member None, (state [mean, var], int32 [count],
+    eps) of its output RunningNorm or (state [mean, var, inv_learning_rate], int32 [count, num_batches], eps, decay) of
+    its output EMANorm."""
     if not 2 <= len(rews) <= PU_MAX_MEMBERS or len(norms) != len(rews):
         raise ImbError(f"imb_pref_uncertainty takes 2 to {PU_MAX_MEMBERS} members, got {len(rews)}")
     d = PrefUncDesc()
@@ -280,6 +284,8 @@ def pref_uncertainty_desc(rews, norms) -> PrefUncDesc:
         if nm is not None:
             d.norm_state[m], d.norm_count[m] = _p(nm[0], th.float32).value, _p(nm[1], th.int32).value
             d.norm_eps[m] = nm[2]
+            if len(nm) > 3:
+                d.norm_kind[m], d.norm_decay[m] = 1, nm[3]
     return d
 
 
@@ -297,11 +303,21 @@ def pref_uncertainty(d: PrefUncDesc, n_pairs, frag_len, mode, noise_prob, discou
                                       _stream()), "imb_pref_uncertainty", (1 + int(norm)) if n_pairs > 0 else 0)
 
 
-def reward_norm_scan(rews, n_envs, n_steps, step_stride, env_stride, norm_state2, norm_count, eps, update_stats):
-    _check(lib().imb_reward_norm_scan(_p(rews, th.float32), C.c_int64(n_envs), C.c_int64(n_steps),
-                                      C.c_int64(step_stride), C.c_int64(env_stride), _p(norm_state2, th.float32),
-                                      _p(norm_count, th.int32), C.c_float(eps), C.c_int(int(update_stats)),
-                                      _stream()), "imb_reward_norm_scan")
+def reward_norm_scan(rews, n_envs, n_steps, step_stride, env_stride, norm_state2, norm_count, eps, update_stats,
+                     ema_decay=None):
+    """NormalizedRewardNet output normalisation over n_steps env steps.  ema_decay None: RunningNorm, norm_state2
+    [mean, var], norm_count [count]; otherwise EMANorm with that decay, norm_state2 [mean, var, inv_learning_rate],
+    norm_count [count, num_batches]."""
+    if ema_decay is None:
+        _check(lib().imb_reward_norm_scan(_p(rews, th.float32), C.c_int64(n_envs), C.c_int64(n_steps),
+                                          C.c_int64(step_stride), C.c_int64(env_stride), _p(norm_state2, th.float32),
+                                          _p(norm_count, th.int32), C.c_float(eps), C.c_int(int(update_stats)),
+                                          _stream()), "imb_reward_norm_scan")
+    else:
+        _check(lib().imb_reward_ema_scan(_p(rews, th.float32), C.c_int64(n_envs), C.c_int64(n_steps),
+                                         C.c_int64(step_stride), C.c_int64(env_stride), _p(norm_state2, th.float32),
+                                         _p(norm_count, th.int32), C.c_float(ema_decay), C.c_float(eps),
+                                         C.c_int(int(update_stats)), _stream()), "imb_reward_ema_scan")
 
 
 def table_store(table, capacity, d_obs, d_act, obs, acts_f, acts_i, next_obs, dones, n, use_ring, state):

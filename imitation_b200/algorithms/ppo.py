@@ -130,8 +130,9 @@ class DevicePPO:
             _lib.ensemble_relabel(relabel, ens.alpha, self._tbl, rw, col_val + 1, E, T, self._ens_ws)
         elif out_norm is not None:
             ns, nc = out_norm.output_norm_vectors()
-            _lib.reward_norm_scan(self._tbl.view(-1)[col_val + 1:], E, T, rw, T * rw, ns, nc,
-                                  out_norm.normalize_output_layer.eps, True)
+            layer = out_norm.normalize_output_layer
+            _lib.reward_norm_scan(self._tbl.view(-1)[col_val + 1:], E, T, rw, T * rw, ns, nc, layer.eps, True,
+                                  ema_decay=layer.decay if out_norm.output_norm_is_ema else None)
         _lib.gae(self._tbl, rw, col_val, E, T, self._aux, self.hp.gamma, self.hp.gae_lambda, env.state, env.horizon)
         _lib.rollout_advance(env.state, E, T, env.horizon, ring.capacity if ring is not None else 0)
         if not self._capturing:
@@ -149,8 +150,7 @@ class DevicePPO:
         engines = [n.engine() for n in ens.nets]
         members = _lib.rollout_members([e.params for e in engines],
                                        [e.norm_state if e.has_norm else None for e in engines], self._ens_raw)
-        norms = [None if o is None else (*o.output_norm_vectors(), float(o.normalize_output_layer.eps))
-                 for o in ens.out_norms]
+        norms = [None if o is None else o.output_norm_args() for o in ens.out_norms]
         return members, _lib.pref_uncertainty_desc(list(self._ens_raw.view(M, T * E)), norms)
 
     def after_rollout_host(self, t0: int) -> None:
@@ -185,9 +185,14 @@ class DevicePPO:
                     key += [eng.params.data_ptr(), eng.norm_state.data_ptr(), id(o)]
                     if o is not None:
                         key += [t.data_ptr() for t in o.output_norm_vectors()]
+                        key += [o.output_norm_is_ema, getattr(o.normalize_output_layer, "decay", None)]
             else:
                 eng = net.engine()
                 key += [eng.params.data_ptr(), eng.norm_state.data_ptr(), mode, id(out_norm)]
+                if out_norm is not None:
+                    # the output norm's vectors and an EMANorm's decay are launch arguments of the scan
+                    key += [t.data_ptr() for t in out_norm.output_norm_vectors()]
+                    key += [out_norm.output_norm_is_ema, getattr(out_norm.normalize_output_layer, "decay", None)]
         if self._buffering is not None and self._buffering._ring is not None:
             key.append(self._buffering._ring.table.data_ptr())
         return tuple(key)

@@ -635,7 +635,7 @@ class PreferenceModel(nn.Module):
         for k, net in enumerate(nets):
             e = net.engine()
             _lib.reward_forward(e.desc, e.params, e.norm_state, batch, ld, n, 0, rews[k])
-        norms = [None if o is None else (*o.output_norm_vectors(), float(o.normalize_output_layer.eps)) for o in outs]
+        norms = [None if o is None else o.output_norm_args() for o in outs]
         desc = _lib.pref_uncertainty_desc(list(rews), norms)
         ws_n = _lib.pref_uncertainty_ws_floats(M, C)
         ws = self.__dict__.get("_pu_ws")

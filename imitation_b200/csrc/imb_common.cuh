@@ -287,6 +287,20 @@ __device__ __forceinline__ void norm_fold(float& mean, float& var, float cnt, fl
   var /= tot;
 }
 
+// EMANorm.update_stats (util/networks.py:175-201): fold the moments of one batch (mean, biased variance) into the
+// running (mean, var) with the learning rate 1 / inv_lr after inv_lr += decay^nb; nb counts the batches folded so
+// far.  Every operation is rounded on its own, as the reference's separate float32 torch ops are: no contraction into
+// fused multiply-adds.  powf is CUDA's, so decay^nb may differ from the host's in the last bit.
+__device__ __forceinline__ void ema_fold(float& mean, float& var, float& inv_lr, int32_t nb, float decay, float b_mean,
+                                         float b_var) {
+  inv_lr = __fadd_rn(inv_lr, powf(decay, (float)nb));
+  const float lr = __fdiv_rn(1.0f, inv_lr);
+  const float dm = __fsub_rn(b_mean, mean);
+  mean = __fadd_rn(mean, __fmul_rn(lr, dm));
+  const float dv = __fsub_rn(__fadd_rn(b_var, __fmul_rn(__fsub_rn(1.0f, lr), __fmul_rn(dm, dm))), var);
+  var = __fadd_rn(var, __fmul_rn(lr, dv));
+}
+
 // exact two-pass (mean, M2) of x[0, n), n >= 1, by one warp; every lane receives the result
 __device__ __forceinline__ void warp_moments(const float* x, int n, int lane, float& mean, float& m2) {
   float s = 0.f;

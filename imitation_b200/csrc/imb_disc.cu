@@ -790,7 +790,10 @@ __host__ __device__ __forceinline__ int64_t pu_aff_off(int M, int F) { return 1 
 
 // NormalizedRewardNet members: a warp per (member, fragment) computes the fragment's moments; the last CTA to finish
 // folds them into each member's output RunningNorm in fragment order, one thread per member.  The fold is a chain of
-// F dependent updates, as in the reference, which updates the statistics once per fragment.
+// F dependent updates, as in the reference, which updates the statistics once per fragment.  EMA = true is launched
+// when a member has an output EMANorm (d.norm_kind[m] == 1) and folds such members with ema_fold; EMA = false is the
+// RunningNorm-only kernel.
+template <bool EMA>
 __global__ void __launch_bounds__(256) k_pref_frag_norm(const imb_pref_unc_desc d, int F, int L, float* __restrict__ ws) {
   const int M = d.n_members;
   unsigned int* ticket = reinterpret_cast<unsigned int*>(ws);
@@ -824,6 +827,25 @@ __global__ void __launch_bounds__(256) k_pref_frag_norm(const imb_pref_unc_desc 
   const float eps = d.norm_eps[m];
   const float* bm = mom + 2 * (int64_t)m * F;
   float* out = aff + 2 * (int64_t)m * F;
+  if constexpr (EMA) {
+    if (d.norm_kind[m] == 1) {
+      float inv_lr = mv[2];
+      int32_t nb = d.norm_count[m][1];
+      const float decay = d.norm_decay[m];
+      for (int f = 0; f < F; ++f) {
+        out[2 * f] = mean;
+        out[2 * f + 1] = 1.0f / sqrtf(var + eps);
+        ema_fold(mean, var, inv_lr, nb, decay, __ldcg(bm + 2 * f), __ldcg(bm + 2 * f + 1));
+        ++nb;
+      }
+      mv[0] = mean;
+      mv[1] = var;
+      mv[2] = inv_lr;
+      *d.norm_count[m] = cnt + F * L;
+      d.norm_count[m][1] = nb;
+      return;
+    }
+  }
 #pragma unroll 4
   for (int f = 0; f < F; ++f) {
     out[2 * f] = mean;  // normalise fragment f with the statistics from before its own update
@@ -1008,15 +1030,24 @@ __global__ void __launch_bounds__(NT) k_reward_fwd(const DiscLaunch L, const flo
 
 // ---- NormalizedRewardNet.predict_processed over consecutive env steps ---------------------------
 // single CTA: for t in steps: normalise the E rewards of step t with the running stats, then merge
-// step t's raw rewards into the stats (reward_nets.py:637-671 + networks.py:111-134).
+// step t's raw rewards into the stats (reward_nets.py:637-671 + networks.py:111-134).  EMA = false: RunningNorm,
+// mv = [mean, var], count = [count]; EMA = true: EMANorm (networks.py:137-201), mv = [mean, var, inv_learning_rate],
+// count = [count, num_batches], and `decay` is read.
+template <bool EMA>
 __global__ void __launch_bounds__(1024) k_reward_norm_scan(float* __restrict__ rews, int64_t E, int64_t T,
                                                           int64_t step_stride, int64_t env_stride,
                                                           float* __restrict__ mv, int32_t* __restrict__ count,
-                                                          float eps, int update) {
+                                                          float eps, int update, float decay) {
   __shared__ float red[64];
   __shared__ float bc[2];
   float mean = mv[0], var = mv[1];
   int32_t cnt = *count;
+  float inv_lr = 0.f;
+  int32_t nb = 0;
+  if constexpr (EMA) {
+    inv_lr = mv[2];
+    nb = count[1];
+  }
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nw = blockDim.x >> 5;
   for (int64_t t = 0; t < T; ++t) {
     float* r = rews + t * step_stride;
@@ -1050,7 +1081,12 @@ __global__ void __launch_bounds__(1024) k_reward_norm_scan(float* __restrict__ r
     }
     __syncthreads();
     if (update) {
-      norm_fold(mean, var, (float)cnt, bmean, bc[1], (float)E);
+      if constexpr (EMA) {
+        ema_fold(mean, var, inv_lr, nb, decay, bmean, bc[1]);
+        ++nb;
+      } else {
+        norm_fold(mean, var, (float)cnt, bmean, bc[1], (float)E);
+      }
       cnt += (int32_t)E;
     }
     __syncthreads();
@@ -1059,6 +1095,10 @@ __global__ void __launch_bounds__(1024) k_reward_norm_scan(float* __restrict__ r
     mv[0] = mean;
     mv[1] = var;
     *count = cnt;
+    if constexpr (EMA) {
+      mv[2] = inv_lr;
+      count[1] = nb;
+    }
   }
 }
 
@@ -1358,17 +1398,33 @@ extern "C" int imb_reward_forward(const imb_disc_desc* d, const float* params, c
                            : launch_fwd<64>(L, params, batch, ld, n, out_mode, out, (cudaStream_t)stream);
 }
 
-extern "C" int imb_reward_norm_scan(float* rews, int64_t n_envs, int64_t n_steps, int64_t step_stride,
-                                    int64_t env_stride, float* norm_state2, int32_t* norm_count, float eps,
-                                    int update_stats, void* stream) {
+template <bool EMA>
+static int launch_reward_norm_scan(float* rews, int64_t n_envs, int64_t n_steps, int64_t step_stride,
+                                   int64_t env_stride, float* state, int32_t* counts, float eps, int update_stats,
+                                   float decay, void* stream) {
   IMB_REQUIRE(n_envs >= 1 && n_steps >= 0, "bad sizes");
   if (n_steps == 0) return 0;
   int threads = 1024;
   while (threads > 32 && threads / 2 >= n_envs) threads /= 2;
-  k_reward_norm_scan<<<1, threads, 0, (cudaStream_t)stream>>>(rews, n_envs, n_steps, step_stride, env_stride,
-                                                              norm_state2, norm_count, eps, update_stats);
+  k_reward_norm_scan<EMA><<<1, threads, 0, (cudaStream_t)stream>>>(rews, n_envs, n_steps, step_stride, env_stride,
+                                                                   state, counts, eps, update_stats, decay);
   IMB_CHECK_LAUNCH("k_reward_norm_scan");
   return 0;
+}
+
+extern "C" int imb_reward_norm_scan(float* rews, int64_t n_envs, int64_t n_steps, int64_t step_stride,
+                                    int64_t env_stride, float* norm_state2, int32_t* norm_count, float eps,
+                                    int update_stats, void* stream) {
+  return launch_reward_norm_scan<false>(rews, n_envs, n_steps, step_stride, env_stride, norm_state2, norm_count, eps,
+                                        update_stats, 0.f, stream);
+}
+
+extern "C" int imb_reward_ema_scan(float* rews, int64_t n_envs, int64_t n_steps, int64_t step_stride,
+                                   int64_t env_stride, float* ema_state3, int32_t* ema_counts2, float decay, float eps,
+                                   int update_stats, void* stream) {
+  IMB_REQUIRE(decay > 0.f && decay < 1.f, "imb_reward_ema_scan: decay %g outside (0, 1)", (double)decay);
+  return launch_reward_norm_scan<true>(rews, n_envs, n_steps, step_stride, env_stride, ema_state3, ema_counts2, eps,
+                                       update_stats, decay, stream);
 }
 
 extern "C" int imb_pref_loss(const float* rews, int64_t n_pairs, int32_t frag_len, const float* prefs, float noise_prob,
@@ -1385,6 +1441,15 @@ extern "C" int imb_pref_loss(const float* rews, int64_t n_pairs, int32_t frag_le
   return 0;
 }
 
+// norm_kind / norm_decay of member m of an imb_pref_unc_desc: 0 = RunningNorm, 1 = EMANorm with 0 < decay < 1
+static int check_norm_kind(const imb_pref_unc_desc* d, int m, const char* who) {
+  const int kind = d->norm_kind[m];
+  IMB_REQUIRE(kind == 0 || kind == 1, "%s: member %d: norm kind %d (0 RunningNorm, 1 EMANorm)", who, m, kind);
+  IMB_REQUIRE(kind == 0 || d->norm_state[m] == nullptr || (d->norm_decay[m] > 0.f && d->norm_decay[m] < 1.f),
+              "%s: member %d: EMANorm decay %g outside (0, 1)", who, m, (double)d->norm_decay[m]);
+  return 0;
+}
+
 extern "C" int64_t imb_pref_uncertainty_ws_floats(int32_t n_members, int64_t n_pairs) {
   return 1 + 4 * (int64_t)n_members * 2 * n_pairs;
 }
@@ -1396,12 +1461,14 @@ extern "C" int imb_pref_uncertainty(const imb_pref_unc_desc* d, int64_t n_pairs,
   IMB_REQUIRE(M >= 2 && M <= IMB_PU_MAX_MEMBERS, "imb_pref_uncertainty: %d members (2 to %d)", M, IMB_PU_MAX_MEMBERS);
   IMB_REQUIRE(n_pairs >= 0 && n_pairs < (1ll << 28) && frag_len >= 1, "imb_pref_uncertainty: bad sizes");
   IMB_REQUIRE(mode >= 0 && mode <= 2, "imb_pref_uncertainty: mode %d (0 logit, 1 probability, 2 label)", mode);
-  bool any_norm = false;
+  bool any_norm = false, any_ema = false;
   for (int m = 0; m < M; ++m) {
     IMB_REQUIRE(d->rews[m] != nullptr, "imb_pref_uncertainty: member %d has no rewards", m);
     IMB_REQUIRE((d->norm_state[m] == nullptr) == (d->norm_count[m] == nullptr),
                 "imb_pref_uncertainty: member %d: norm state and count go together", m);
+    if (int rc = check_norm_kind(d, m, "imb_pref_uncertainty")) return rc;
     any_norm = any_norm || d->norm_state[m] != nullptr;
+    any_ema = any_ema || (d->norm_state[m] != nullptr && d->norm_kind[m] == 1);
   }
   if (n_pairs == 0) return 0;
   const cudaStream_t st = (cudaStream_t)stream;
@@ -1409,7 +1476,10 @@ extern "C" int imb_pref_uncertainty(const imb_pref_unc_desc* d, int64_t n_pairs,
   const int64_t cap = 4 * (int64_t)imb_num_sms();
   if (any_norm) {
     const int64_t blocks = std::min(((int64_t)M * F + 7) / 8, cap);
-    k_pref_frag_norm<<<(int)blocks, 256, 0, st>>>(*d, F, frag_len, ws);
+    if (any_ema)
+      k_pref_frag_norm<true><<<(int)blocks, 256, 0, st>>>(*d, F, frag_len, ws);
+    else
+      k_pref_frag_norm<false><<<(int)blocks, 256, 0, st>>>(*d, F, frag_len, ws);
     IMB_CHECK_LAUNCH("k_pref_frag_norm");
   }
   const int64_t blocks = std::min(((int64_t)C + 7) / 8, cap);
@@ -1429,19 +1499,24 @@ extern "C" int imb_ensemble_relabel(const imb_pref_unc_desc* d, float alpha, flo
   IMB_REQUIRE(M >= 2 && M <= IMB_PU_MAX_MEMBERS, "imb_ensemble_relabel: %d members (2 to %d)", M, IMB_PU_MAX_MEMBERS);
   IMB_REQUIRE(n_envs >= 1 && n_steps >= 1 && n_envs * n_steps < (1ll << 31), "imb_ensemble_relabel: bad sizes");
   IMB_REQUIRE(col_rew >= 0 && col_rew < rw, "imb_ensemble_relabel: reward column %d outside rows of %d", col_rew, rw);
-  bool any_norm = false;
+  bool any_norm = false, any_ema = false;
   for (int m = 0; m < M; ++m) {
     IMB_REQUIRE(d->rews[m] != nullptr, "imb_ensemble_relabel: member %d has no rewards", m);
     IMB_REQUIRE((d->norm_state[m] == nullptr) == (d->norm_count[m] == nullptr),
                 "imb_ensemble_relabel: member %d: norm state and count go together", m);
+    if (int rc = check_norm_kind(d, m, "imb_ensemble_relabel")) return rc;
     any_norm = any_norm || d->norm_state[m] != nullptr;
+    any_ema = any_ema || (d->norm_state[m] != nullptr && d->norm_kind[m] == 1);
   }
   const cudaStream_t st = (cudaStream_t)stream;
   const int F = (int)n_steps, L = (int)n_envs;  // fragment = one env step of E rewards
   const int64_t cap = 4 * (int64_t)imb_num_sms();
   if (any_norm) {
     const int64_t blocks = std::min(((int64_t)M * F + 7) / 8, cap);
-    k_pref_frag_norm<<<(int)blocks, 256, 0, st>>>(*d, F, L, ws);
+    if (any_ema)
+      k_pref_frag_norm<true><<<(int)blocks, 256, 0, st>>>(*d, F, L, ws);
+    else
+      k_pref_frag_norm<false><<<(int)blocks, 256, 0, st>>>(*d, F, L, ws);
     IMB_CHECK_LAUNCH("k_pref_frag_norm");
   }
   const int64_t blocks = std::min((n_envs * n_steps + 255) / 256, 8 * (int64_t)imb_num_sms());

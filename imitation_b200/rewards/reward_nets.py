@@ -16,6 +16,7 @@ raises.
 """
 import abc
 import collections
+import functools
 from typing import Callable, Dict, Iterable, List, Optional, Sequence, Tuple, Type
 
 import numpy as np
@@ -503,15 +504,29 @@ class BasicShapedRewardNet(_FusedNetMixin, ShapedRewardNet):
         return out
 
 
+_OUTPUT_NORMS = {"RunningNorm": networks.RunningNorm, "EMANorm": networks.EMANorm}
+
+
 class NormalizedRewardNet(PredictProcessedWrapper):
     """Normalises `predict_processed` output with a running norm, updating it on every call
-    (reward_nets.py:613-671)."""
+    (reward_nets.py:613-671).  `normalize_output_layer` is RunningNorm or EMANorm (this package's or the reference's
+    class, matched by name), or a `functools.partial` of one carrying its keyword arguments (EMANorm's `decay`, `eps`);
+    the layer is built as `normalize_output_layer(1)`, as the reference builds it."""
 
     def __init__(self, base: RewardNet, normalize_output_layer: Type[nn.Module]):
         super().__init__(base=base)
-        if not _is_running_norm(normalize_output_layer):
-            raise NotImplementedError("normalize_output_layer must be RunningNorm (EMANorm out of scope)")
-        self.normalize_output_layer = networks.RunningNorm(1)
+        layer = normalize_output_layer
+        func, args, kw = ((layer.func, layer.args, layer.keywords) if isinstance(layer, functools.partial)
+                          else (layer, (), {}))
+        cls = _OUTPUT_NORMS.get(getattr(func, "__name__", ""))
+        if cls is None:
+            raise NotImplementedError("normalize_output_layer must be RunningNorm or EMANorm (or a functools.partial "
+                                      f"of one), got {layer!r}")
+        self.normalize_output_layer = cls(*args, 1, **kw)
+
+    @property
+    def output_norm_is_ema(self) -> bool:
+        return isinstance(self.normalize_output_layer, networks.EMANorm)
 
     def predict_processed(self, state, action, next_state, done, update_stats: bool = True, **kwargs) -> np.ndarray:
         with networks.evaluating(self):
@@ -525,19 +540,32 @@ class NormalizedRewardNet(PredictProcessedWrapper):
         return rew
 
     def output_norm_vectors(self) -> Tuple[th.Tensor, th.Tensor]:
-        """[mean, var] float vector + int32 count aliased by the norm's buffers (for the kernels)."""
+        """Float vector + int32 vector aliased by the norm's buffers (for the kernels): RunningNorm [mean, var] and
+        [count]; EMANorm [mean, var, inv_learning_rate] and [count, num_batches]."""
         n = self.normalize_output_layer
+        ema = self.output_norm_is_ema
+        fl = [n.running_mean, n.running_var] + ([n.inv_learning_rate] if ema else [])
+        it = [n.count] + ([n.num_batches] if ema else [])
         dev = self.device
-        st = getattr(self, "_out_state", None)
-        if (st is None or st.device != dev or n.running_mean.data_ptr() != st.data_ptr()
-                or n.running_var.data_ptr() != st.data_ptr() + 4 or n.count.data_ptr() != self._out_count.data_ptr()):
-            st = th.cat([n.running_mean.detach().float().reshape(1), n.running_var.detach().float().reshape(1)]).to(dev)
-            ct = n.count.detach().to(th.int32).reshape(1).to(dev).contiguous()
+        st, ct = getattr(self, "_out_state", None), getattr(self, "_out_count", None)
+        if (st is None or st.device != dev or st.numel() != len(fl) or ct.numel() != len(it)
+                or any(b.data_ptr() != st.data_ptr() + 4 * k for k, b in enumerate(fl))
+                or any(b.data_ptr() != ct.data_ptr() + 4 * k for k, b in enumerate(it))):
+            st = th.cat([b.detach().float().reshape(1) for b in fl]).to(dev)
+            ct = th.cat([b.detach().to(th.int32).reshape(1) for b in it]).to(dev).contiguous()
             n._buffers["running_mean"], n._buffers["running_var"] = st[0:1], st[1:2]
-            n._buffers["count"] = ct.view(())
+            n._buffers["count"] = ct[0].view(())
+            if ema:
+                n._buffers["inv_learning_rate"] = st[2].view(())
+                n._buffers["num_batches"] = ct[1].view(())
             object.__setattr__(self, "_out_state", st)
             object.__setattr__(self, "_out_count", ct)
         return self._out_state, self._out_count
+
+    def output_norm_args(self) -> tuple:
+        """The member entry `_lib.pref_uncertainty_desc` takes: (state, count, eps), plus decay for an EMANorm."""
+        n = self.normalize_output_layer
+        return (*self.output_norm_vectors(), float(n.eps)) + ((float(n.decay),) if self.output_norm_is_ema else ())
 
     def __getstate__(self):
         state = self.__dict__.copy()

@@ -77,7 +77,8 @@ class RewardVecEnvWrapper:
 
 class EnsembleRelabel:
     """An ensemble reward as the rollout evaluates it (reward_nets.py:926-989, :1045-1080): up to 16 members of one
-    fused architecture, each either plain or inside a `NormalizedRewardNet` (all members alike), combined per step into
+    fused architecture, each either plain or inside a `NormalizedRewardNet` (all members alike, with output norms of one
+    kind), combined per step into
     mean + alpha * std.  `alpha` is read from the wrapper on every access, so a changed `default_alpha` takes effect at
     the next rollout."""
 
@@ -104,6 +105,9 @@ class EnsembleRelabel:
         if len({o is None for o in self.out_norms}) > 1:
             raise NotImplementedError("ensemble members must all be NormalizedRewardNets or all plain reward nets, "
                                       "not a mix")
+        if len({o.output_norm_is_ema for o in self.out_norms if o is not None}) > 1:
+            raise NotImplementedError("ensemble members' output norms must all be RunningNorm or all EMANorm, not a "
+                                      "mix")
         d0 = bytes(self.nets[0].engine().desc)
         for k, net in enumerate(self.nets[1:], 1):
             if bytes(net.engine().desc) != d0:

@@ -1,4 +1,4 @@
-"""RunningNorm + train/eval helpers with the reference's semantics.
+"""RunningNorm, EMANorm + train/eval helpers with the reference's semantics.
 
 Mirrors imitation.util.networks: `training` / `evaluating` context managers
 (util/networks.py:12-34) and `RunningNorm` (util/networks.py:47-134: in train mode update
@@ -78,6 +78,38 @@ class RunningNorm(BaseNorm):
         self.running_var += th.square(delta) * self.count * b_n / tot
         self.running_var /= tot
         self.count += b_n
+
+
+class EMANorm(BaseNorm):
+    """Exponentially weighted running statistics (util/networks.py:137-201): the k-th batch (k = num_batches, from 0)
+    is folded with learning rate 1 / inv_learning_rate after inv_learning_rate += decay ** k, each line one float32
+    torch op as in the reference.  Buffers, shapes and dtypes are the reference's, so state dicts load both ways.  As an
+    output layer of a fused reward net the kernels update the aliased buffers instead."""
+
+    def __init__(self, num_features: int, decay: float = 0.99, eps: float = 1e-5):
+        super().__init__(num_features, eps=eps)
+        if not 0 < decay < 1:
+            raise ValueError("decay must be between 0 and 1")
+        self.decay = decay
+        self.register_buffer("inv_learning_rate", th.zeros(()))
+        self.register_buffer("num_batches", th.zeros((), dtype=th.int))
+
+    def reset_running_stats(self) -> None:
+        super().reset_running_stats()
+        self.inv_learning_rate.zero_()
+        self.num_batches.zero_()
+
+    def update_stats(self, batch: th.Tensor) -> None:
+        if batch.ndim == 1:
+            batch = batch.reshape(-1, 1)
+        self.inv_learning_rate += th.pow(self.decay, self.num_batches)
+        lr = 1 / self.inv_learning_rate
+        delta = th.mean(batch, dim=0) - self.running_mean
+        self.running_mean += lr * delta
+        delta_var = th.var(batch, dim=0, unbiased=False) + (1 - lr) * th.square(delta) - self.running_var
+        self.running_var += lr * delta_var
+        self.count += batch.shape[0]
+        self.num_batches += 1
 
 
 class SqueezeLayer(nn.Module):

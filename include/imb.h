@@ -172,6 +172,14 @@ int imb_reward_forward(const imb_disc_desc* d, const float* params, const float*
 int imb_reward_norm_scan(float* rews, int64_t n_envs, int64_t n_steps, int64_t step_stride,
                          int64_t env_stride, float* norm_state2, int32_t* norm_count, float eps,
                          int update_stats, void* stream);
+/* The same scan for an output EMANorm (util/networks.py:137-201): ema_state3 = [running_mean, running_var,
+ * inv_learning_rate] (float32), ema_counts2 = [count, num_batches] (int32).  Per step, after normalising with the
+ * statistics from before it: inv_learning_rate += decay^num_batches (float32 powf), lr = 1 / inv_learning_rate,
+ * dm = batch mean - mean, mean += lr * dm, var += lr * (batch var + (1 - lr) * dm^2 - var) (biased batch variance,
+ * every operation rounded on its own), count += E, num_batches += 1.  0 < decay < 1. */
+int imb_reward_ema_scan(float* rews, int64_t n_envs, int64_t n_steps, int64_t step_stride, int64_t env_stride,
+                        float* ema_state3, int32_t* ema_counts2, float decay, float eps, int update_stats,
+                        void* stream);
 
 /* ---- stage 2: tables, ring buffer, sampling --------------------------------------------- */
 
@@ -324,7 +332,8 @@ int imb_pref_loss(const float* rews, int64_t n_pairs, int32_t frag_len, const fl
  * predict_processed twice per pair.  Member m's raw rewards are rews[m][2C][L] (fragment f = 2 i + s is pair i's first
  * (s = 0) or second (s = 1) fragment).  A member with norm_state[m] != NULL is a NormalizedRewardNet
  * (reward_nets.py:637-671): fragment f is normalised with its output statistics as they stood before f, then f's raw
- * rewards are merged into them (RunningNorm.update_stats, util/networks.py:121-134), in the order f = 0, 1, ..., 2C - 1;
+ * rewards are merged into them (RunningNorm.update_stats, util/networks.py:121-134, or EMANorm.update_stats,
+ * :175-201, by norm_kind[m]), in the order f = 0, 1, ..., 2C - 1;
  * the final statistics and count are written back.  mode 0 (logit): v_m = sum_t r1 - sum_t r2 (undiscounted), score =
  * variance with ddof 1; mode 1 (probability): v_m = PreferenceModel.probability (:487-530), score = variance with ddof 0;
  * mode 2 (label): v_m = (probability > 0.5), score = q (1 - q) with q = mean_m v_m.  Outputs: scores[C] and, optional,
@@ -339,6 +348,11 @@ typedef struct imb_pref_unc_desc {
   float* norm_state[IMB_PU_MAX_MEMBERS];   /* [mean, var] of the output RunningNorm, or NULL */
   int32_t* norm_count[IMB_PU_MAX_MEMBERS];
   float norm_eps[IMB_PU_MAX_MEMBERS];
+  /* 0 (zero-filled) = output RunningNorm; 1 = output EMANorm (util/networks.py:137-201): norm_state[m] =
+   * [mean, var, inv_learning_rate], norm_count[m] = [count, num_batches], folded per fragment as
+   * imb_reward_ema_scan folds per step, with decay norm_decay[m] (0 < decay < 1) */
+  int32_t norm_kind[IMB_PU_MAX_MEMBERS];
+  float norm_decay[IMB_PU_MAX_MEMBERS];
 } imb_pref_unc_desc;
 int64_t imb_pref_uncertainty_ws_floats(int32_t n_members, int64_t n_pairs);
 int imb_pref_uncertainty(const imb_pref_unc_desc* d, int64_t n_pairs, int32_t frag_len, int32_t mode,
@@ -370,7 +384,8 @@ int imb_rollout_ensemble(const imb_env_desc* env, const float* env_params, float
                          const int64_t* state, void* stream);
 /* The relabel of the ensemble rollout, before imb_gae: d->rews[m] = member m's raw[T][E] from imb_rollout_ensemble.
  * Per env step t, member m with d->norm_state[m] != NULL is normalised with its output statistics from before step t,
- * then step t's E raw rewards are merged into them (RunningNorm.update_stats, util/networks.py:121-134), so the
+ * then step t's E raw rewards are merged into them (RunningNorm.update_stats, util/networks.py:121-134, or
+ * EMANorm.update_stats, :175-201, by norm_kind[m]), so the
  * statistics and count end as E*T separate predict_processed calls leave them; a member without one is used raw.
  * rollout[(e*T + t)*rw + col_rew] = mean_m v_m + alpha * sqrt(var_m(v_m, ddof 1)), the mean and variance two-pass in
  * member order (alpha = 0 for a bare RewardEnsemble).  No atomics in the arithmetic: two calls give the same bits.
