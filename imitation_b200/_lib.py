@@ -105,8 +105,11 @@ SYMBOLS = [
     "imb_sync_buffer_doubles", "imb_sync_snapshot", "imb_sync_pack", "imb_sync_unpack",
     "imb_disc_sample_gather", "imb_sample_advance2", "imb_disc_reduce_adam", "imb_norm_batch_stats", "imb_norm_fold",
     "imb_disc_set_rows", "imb_stats_publish", "imb_pref_loss", "imb_pref_uncertainty_ws_floats", "imb_pref_uncertainty",
-    "imb_rollout_ensemble", "imb_ensemble_relabel_ws_floats", "imb_ensemble_relabel",
+    "imb_rollout_ensemble", "imb_ensemble_relabel_ws_floats", "imb_ensemble_relabel", "imb_disc_plan",
 ]
+
+# imb_disc_plan codes: the kernel imb_disc_fwd_bwd runs
+PLAN_TC, PLAN_FFMA128X2, PLAN_FFMA256, PLAN_FFMA128 = 1, 2, 3, 4
 
 
 def lib() -> C.CDLL:
@@ -243,6 +246,15 @@ def disc_fwd_bwd(d, params, norm_state, batch, ld, n, n_expert, loss_scale, grad
                                   _p(batch, th.float32), C.c_int64(ld), C.c_int64(n), C.c_int64(n_expert),
                                   C.c_float(loss_scale), _p(grad_out), _p(logits_out), C.c_int(flags),
                                   _p(ws, th.float32), _stream()), "imb_disc_fwd_bwd")
+
+
+def disc_plan(d: DiscDesc, n: int) -> int:
+    """PLAN_* code of the kernel `disc_fwd_bwd` runs for `d` over n rows (host only, no GPU needed); ImbError naming
+    the shared-memory limit when the fused kernels cannot run the shape."""
+    rc = int(lib().imb_disc_plan(C.byref(d), C.c_int64(n)))
+    if rc < 0:
+        raise ImbError(f"imb_disc_plan: {lib().imb_last_error().decode()} (rc={rc})")
+    return rc
 
 
 def disc_reduce(d, ws, grad_out_flat=None):

@@ -21,6 +21,7 @@ class AIRL(common.AdversarialTrainer):
         if self._fused:
             # the fused kernels subtract log pi(a|s) inside the logit (airl.py:118-119)
             self._fused_net._engine.desc.subtract_logp = 1
+            self._fused_net._engine.check_plan()  # the log pi row is one more staged batch row
 
     def logits_expert_is_high(self, state, action, next_state, done, log_policy_act_prob: Optional[th.Tensor] = None
                               ) -> th.Tensor:

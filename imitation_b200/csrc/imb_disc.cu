@@ -1276,6 +1276,42 @@ static int launch_fwdbwd(const DiscLaunch& L, const TPlan& t, const float* param
   return 0;
 }
 
+// Which k_disc_fwdbwd* kernel runs for this shape and row count (the IMB_PLAN_* codes of imb_disc_plan); the tiled
+// plans are returned in t128 / t256.  Tensor cores (wgmma, 3xTF32 split) whenever the network shape fits them; else
+// 128-row tiles with TWO resident CTAs per SM (independent CTAs overlap each other's barriers and epilogues); else one
+// 256-row CTA; else one 128-row CTA.
+static int fwdbwd_plan(const DiscLaunch& L, int64_t n, int flags, TPlan& t128, TPlan& t256) {
+  if (!(flags & IMB_F_NO_TENSOR) && tc_applicable(L)) {
+    const size_t bytes = (size_t)tc_plan(L).total * 4 + 128;
+    IMB_REQUIRE(bytes <= IMB_SMEM_MAX, "tensor-core disc kernel: %zu B of shared memory", bytes);
+    return IMB_PLAN_TC;
+  }
+  t256 = plan_tiled(L, 256);
+  t128 = plan_tiled(L, 128);
+  if (2 * ((size_t)t128.total * 4 + 1024 + 512) <= 228 * 1024) return IMB_PLAN_FFMA128X2;
+  if ((size_t)t256.total * 4 <= IMB_SMEM_MAX && n > 128) return IMB_PLAN_FFMA256;
+  if ((size_t)t128.total * 4 <= IMB_SMEM_MAX) return IMB_PLAN_FFMA128;
+  IMB_FAIL(-1, "discriminator too large for the fused kernel: its 128-row tile needs %zu B of shared memory per CTA, "
+           "the limit is %d B", (size_t)t128.total * 4, IMB_SMEM_MAX);
+}
+
+// imb_reward_forward's kernel: hidden width H (32 or 64) and its dynamic shared memory
+template <int H>
+static size_t reward_fwd_bytes(const DiscLaunch& L) {
+  return (size_t)plan_smem<H>(L, false).total_floats * 4;
+}
+
+extern "C" int imb_disc_plan(const imb_disc_desc* d, int64_t n) {
+  IMB_REQUIRE(n >= 1, "disc plan needs n >= 1");
+  DiscLaunch L;
+  if (int rc = build_launch(d, nullptr, nullptr, L)) return rc;
+  const size_t fb = pick_H(L) == 32 ? reward_fwd_bytes<32>(L) : reward_fwd_bytes<64>(L);
+  IMB_REQUIRE(fb <= IMB_SMEM_MAX, "reward net too large for the fused forward kernel: %zu B of shared memory, the "
+              "limit is %d B", fb, IMB_SMEM_MAX);
+  TPlan t128, t256;
+  return fwdbwd_plan(L, n, 0, t128, t256);
+}
+
 extern "C" int imb_disc_fwd_bwd(const imb_disc_desc* d, const float* params, const float* norm_state,
                                 const float* batch, int64_t ld, int64_t n, int64_t n_expert, float loss_scale,
                                 const float* grad_out, float* logits_out, int flags, float* ws, void* stream) {
@@ -1288,12 +1324,14 @@ extern "C" int imb_disc_fwd_bwd(const imb_disc_desc* d, const float* params, con
   // in training mode the Phi(s') pass uses the stats snapshot taken between the two norm updates
   const bool snap = d->shaped && d->potential.has_norm && (flags & IMB_F_TRAIN_NORM);
   if (int rc = build_launch(d, norm_state, snap ? ws + w.snap : nullptr, L)) return rc;
+  TPlan t128, t256;
+  const int plan = fwdbwd_plan(L, n, flags, t128, t256);
+  if (plan < 0) return plan;
   if (flags & IMB_F_ZERO_GRAD) {
     cudaError_t e = cudaMemsetAsync(ws + w.gacc, 0, sizeof(float) * d->n_params, st);
     if (e != cudaSuccess) IMB_FAIL(-2, "memset: %s", cudaGetErrorString(e));
   }
-  // Tensor-core path (wgmma, 3xTF32 split) whenever the network shape fits it
-  if (!(flags & IMB_F_NO_TENSOR) && tc_applicable(L)) {
+  if (plan == IMB_PLAN_TC) {
     const TcPlan T = tc_plan(L);
     const size_t bytes = (size_t)T.total * 4 + 128;
     static bool attr_set = false;
@@ -1302,7 +1340,6 @@ extern "C" int imb_disc_fwd_bwd(const imb_disc_desc* d, const float* params, con
       if (e != cudaSuccess) IMB_FAIL(-2, "cudaFuncSetAttribute(tc): %s", cudaGetErrorString(e));
       attr_set = true;
     }
-    IMB_REQUIRE(bytes <= IMB_SMEM_MAX, "tensor-core disc kernel: %zu B of shared memory", bytes);
     const int64_t ntiles = (n + 127) / 128;
     int64_t Gt = imb_num_sms();
     if (Gt > MAXG) Gt = MAXG;
@@ -1313,16 +1350,10 @@ extern "C" int imb_disc_fwd_bwd(const imb_disc_desc* d, const float* params, con
     IMB_CHECK_LAUNCH("k_disc_fwdbwd_tc");
     return 0;
   }
-  // Preferred: 128-row tiles with TWO resident CTAs per SM (independent CTAs overlap each other's
-  // barriers and epilogues); else one 256-row CTA; else one 128-row CTA.
-  TPlan t256 = plan_tiled(L, 256), t128 = plan_tiled(L, 128);
-  if (2 * ((size_t)t128.total * 4 + 1024 + 512) <= 228 * 1024)
-    return launch_fwdbwd<128>(L, t128, params, batch, ld, n, n_expert, loss_scale, grad_out, logits_out, ws, w, st, 2);
-  if ((size_t)t256.total * 4 <= IMB_SMEM_MAX && n > 128)
+  if (plan == IMB_PLAN_FFMA256)
     return launch_fwdbwd<256>(L, t256, params, batch, ld, n, n_expert, loss_scale, grad_out, logits_out, ws, w, st, 1);
-  if ((size_t)t128.total * 4 <= IMB_SMEM_MAX)
-    return launch_fwdbwd<128>(L, t128, params, batch, ld, n, n_expert, loss_scale, grad_out, logits_out, ws, w, st, 1);
-  IMB_FAIL(-1, "discriminator too large for the fused kernel (%zu B of shared memory)", (size_t)t128.total * 4);
+  return launch_fwdbwd<128>(L, t128, params, batch, ld, n, n_expert, loss_scale, grad_out, logits_out, ws, w, st,
+                            plan == IMB_PLAN_FFMA128X2 ? 2 : 1);
 }
 
 // warp per parameter and per statistic, at most two blocks per SM

@@ -41,6 +41,15 @@ class FusedEngine:
         self.norm_count: Optional[th.Tensor] = None
         self.ws: Optional[th.Tensor] = None
         self.bw = _desc.batch_rows(desc.d_obs, desc.d_act)
+        self.check_plan()
+
+    def check_plan(self) -> None:
+        """Raise NotImplementedError now, rather than at the first discriminator update, when the fused kernels cannot
+        run this network shape (imb_disc_plan: the kernel's shared-memory need exceeds what one CTA can have)."""
+        try:
+            _lib.disc_plan(self.desc, _lib.IMB_TILE_ROWS)
+        except _lib.ImbError as e:
+            raise NotImplementedError(f"reward network shape not supported by the fused sm_90a kernels: {e}") from None
 
     # -- aliasing ---------------------------------------------------------------------------------
     def _param_list(self) -> List[nn.Parameter]:

@@ -21,7 +21,8 @@
  *    row = [obs(d_obs) | act(d_act; Discrete -> one-hot) | next_obs(d_obs) | done(1)],
  *    tw = 2*d_obs + d_act + 1.  Random row gathers read whole contiguous rows.
  *  - disc BATCH: SoA / feature-major [bw][ld], bw = tw + 1 (last feature row = log pi(a|s)),
- *    ld = row count rounded up to IMB_TILE_ROWS (padding zero).  Streaming kernels read it
+ *    ld = row count rounded up to IMB_TILE_ROWS; padding columns [n, ld) are never used, so
+ *    their contents do not matter (the tests fill them with NaN).  Streaming kernels read it
  *    in [feature][128-row] tiles staged into shared memory by cp.async.bulk (TMA unit).
  *  - ROLLOUT table (PPO): row-major [E*T][rw], row index = env*T + step,
  *    row = [obs(d_obs) | act(da_store) | logp | value | reward | adv | ret].
@@ -148,6 +149,15 @@ int imb_disc_fwd_bwd(const imb_disc_desc* d, const float* params, const float* n
                      const float* batch, int64_t ld, int64_t n, int64_t n_expert,
                      float loss_scale, const float* grad_out, float* logits_out,
                      int flags, float* ws, void* stream);
+
+/* Which kernel imb_disc_fwd_bwd (flags without IMB_F_NO_TENSOR) runs for the network `d` over n rows; host only, no
+ * GPU needed.  <0 (imb_last_error() names the shared-memory need and limit) when imb_disc_fwd_bwd or
+ * imb_reward_forward cannot run the shape at all; which of them fits does not depend on n. */
+#define IMB_PLAN_TC 1          /* wgmma tensor-core kernel: unshaped 32x32 net, din <= 31, no done input, no log pi */
+#define IMB_PLAN_FFMA128X2 2   /* fp32-FFMA kernel, 128-row tiles, two CTAs per SM */
+#define IMB_PLAN_FFMA256 3     /* fp32-FFMA kernel, 256-row tiles, one CTA per SM (only for n > 128) */
+#define IMB_PLAN_FFMA128 4     /* fp32-FFMA kernel, 128-row tiles, one CTA per SM */
+int imb_disc_plan(const imb_disc_desc* d, int64_t n);
 
 /* Finish the update: deterministic reduction of the per-CTA partials, optional copy of the
  * gradient to grad_out_flat (for external optimisers / all-reduce), optional Adam step
