@@ -105,11 +105,13 @@ SYMBOLS = [
     "imb_sync_buffer_doubles", "imb_sync_snapshot", "imb_sync_pack", "imb_sync_unpack",
     "imb_disc_sample_gather", "imb_sample_advance2", "imb_disc_reduce_adam", "imb_norm_batch_stats", "imb_norm_fold",
     "imb_disc_set_rows", "imb_stats_publish", "imb_pref_loss", "imb_pref_uncertainty_ws_floats", "imb_pref_uncertainty",
-    "imb_rollout_ensemble", "imb_ensemble_relabel_ws_floats", "imb_ensemble_relabel", "imb_disc_plan",
+    "imb_rollout_ensemble", "imb_ensemble_relabel_ws_floats", "imb_ensemble_relabel", "imb_disc_plan", "imb_ppo_plan",
 ]
 
 # imb_disc_plan codes: the kernel imb_disc_fwd_bwd runs
 PLAN_TC, PLAN_FFMA128X2, PLAN_FFMA256, PLAN_FFMA128 = 1, 2, 3, 4
+# imb_ppo_plan codes: the kernel imb_ppo_update runs
+PPO_PLAN_UPDATE, PPO_PLAN_GEN1, PPO_PLAN_GEN2 = 1, 2, 3
 
 
 def lib() -> C.CDLL:
@@ -449,6 +451,15 @@ def ppo_update(pol, params, norm, norm_count, exp_avg, exp_avg_sq, rollout_tbl, 
                                 _p(exp_avg, th.float32), _p(exp_avg_sq, th.float32), _p(rollout_tbl, th.float32),
                                 C.c_int64(n_rows), C.byref(hp), _p(perm), C.c_uint64(seed), _p(loss_log),
                                 _p(state, th.int64), _stream()), "imb_ppo_update")
+
+
+def ppo_plan(pol: PolicyDesc, batch_size: int) -> int:
+    """PPO_PLAN_* code of the kernel `ppo_update` runs for `pol` at minibatch size batch_size (host only, no GPU
+    needed); ImbError naming the shared-memory need and limit when no PPO kernel can run the shape."""
+    rc = int(lib().imb_ppo_plan(C.byref(pol), C.c_int32(batch_size)))
+    if rc < 0:
+        raise ImbError(f"imb_ppo_plan: {lib().imb_last_error().decode()} (rc={rc})")
+    return rc
 
 
 def policy_logp(pol, params, norm, batch, ld, n, row_logp):

@@ -50,6 +50,10 @@ class DevicePPO:
             if self._user_seed is not None:
                 th.manual_seed(self._user_seed)
             self.policy = cls(self._base_env.observation_space, self._base_env.action_space, **kw).to(self.device)
+        try:  # refuse a policy / minibatch no PPO kernel can run now, not at the first train()
+            _lib.ppo_plan(self.policy.desc, self.batch_size)
+        except _lib.ImbError as e:
+            raise NotImplementedError(f"policy / minibatch not supported by the PPO update kernels: {e}") from None
         n = self.policy.desc.n_params
         self.exp_avg = th.zeros(n, device=self.device)
         self.exp_avg_sq = th.zeros(n, device=self.device)

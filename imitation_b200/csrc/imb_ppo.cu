@@ -450,7 +450,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
   // A CTA never sends to itself: the slice sum reads its own partial from GP, the owner stores its new slice into its
   // own Pm directly, so both exchanges expect the bytes of the CL - 1 peers.
   const uint32_t xbytes = (uint32_t)((CL - 1) * S * 4);
-  const unsigned qmagic = (unsigned)(0x100000000ull / (unsigned)(S / 4)) + 1u;  // exact quotient for the < 2^16 quads here
+  const unsigned qmagic = (unsigned)(0x100000000ull / (unsigned)(S / 4)) + 1u;  // exact quotient; S / 4 >= 2 (host)
   const uint32_t recv_sa = smem_u32(RECV), pm_sa = smem_u32(Pm), ssq_sa = smem_u32(SSQ);
   const uint32_t xbar0_sa = smem_u32(&xbar[0]), xbar1_sa = smem_u32(&xbar[1]), xbar2_sa = smem_u32(&xbar[2]);
   if (tid == 0) {
@@ -1055,52 +1055,79 @@ static int launch_cluster(K kernel, const char* name, size_t smem_bytes, size_t*
   return 0;
 }
 
-static int launch_ppo(const PpoArgs& A0, float* params, float* norm, int32_t* norm_count, float* m, float* v,
-                      const float* rollout, const int64_t* perm, float* loss_log, int64_t* state, cudaStream_t st) {
-  PpoArgs A = A0;
+extern "C" int imb_rollout_row_width(const imb_policy_desc* pol);
+
+// Which PPO kernel runs the policy A.pol at minibatch A.hp.batch_size (the IMB_PPO_PLAN_* codes of imb_ppo_plan), with
+// the launch geometry (rw, KP, S, RS2, HP) filled into A and the dynamic shared memory into *bytes.  k_ppo_update
+// (64-row minibatch resident in shared memory, one lane per hidden unit) for tower width <= 32 and minibatches <= 64
+// rows when its shared memory and slice fit; else k_ppo_update_gen with U = 1 or 2 hidden units per lane.
+static int ppo_plan(PpoArgs& A, size_t* bytes) {
+  const imb_policy_desc& pd = A.pol;
+  IMB_REQUIRE(pd.hidden >= 1 && pd.hidden <= 64, "policy tower width must be <= 64");
+  IMB_REQUIRE(pd.d_obs >= 1 && pd.d_obs <= IMB_MAX_DIN && pd.d_act >= 1 && pd.d_act <= IMB_MAX_DIN,
+              "d_obs/d_act must be in [1, %d]", IMB_MAX_DIN);
   IMB_REQUIRE(A.hp.batch_size >= 1 && A.hp.batch_size <= GEN_MAX_MB, "PPO minibatch size must be in [1, %d]", GEN_MAX_MB);
+  A.rw = imb_rollout_row_width(&pd);
   IMB_REQUIRE(A.rw % 4 == 0, "rollout row width must be a multiple of 4 floats (bulk row copies)");
-  A.KP = A.pol.d_obs <= 32 ? 32 : 64;
-  A.S = ((make_play(A.pol).total + CL - 1) / CL + 3) / 4 * 4;
+  A.KP = pd.d_obs <= 32 ? 32 : 64;
+  // at least two quads per slice: k_ppo_update finds a quad's owner as qq / (S / 4) through the 32-bit reciprocal
+  // 2^32 / (S / 4) + 1, which does not fit for S / 4 = 1 (policies of <= 32 padded parameters, e.g. width 1)
+  A.S = max(8, ((make_play(pd).total + CL - 1) / CL + 3) / 4 * 4);
   A.RS2 = ((A.rw + 4) % 8 == 4) ? A.rw + 4 : A.rw + 8;
   // IMB_PPO_FORCE_GENERAL=1 (tests): run the general kernel on shapes the specialised one covers
   const char* force = getenv("IMB_PPO_FORCE_GENERAL");
-  const bool general = A.pol.hidden > 32 || A.hp.batch_size > PR || (force && force[0] == '1');
-  if (!general) {
-    // 64-row minibatch resident in shared memory, one lane per hidden unit (k_ppo_update)
+  if (pd.hidden <= 32 && A.hp.batch_size <= PR && !(force && force[0] == '1')) {
     A.HP = 32;
-    IMB_REQUIRE(A.S / 4 <= PT, "policy too large for the PPO update kernel (%d parameters per slice)", A.S);
-    static size_t attr_bytes = 0;
-    return launch_cluster(k_ppo_update<32>, "k_ppo_update", ppo_smem_floats(A) * 4, &attr_bytes, st, A, params, norm,
-                          norm_count, m, v, rollout, perm, loss_log, state);
+    *bytes = ppo_smem_floats(A) * 4;
+    if (A.S / 4 <= PT && *bytes <= IMB_SMEM_MAX) return IMB_PPO_PLAN_UPDATE;
   }
-  // tower width up to 64 and / or minibatches of more than 64 rows (k_ppo_update_gen)
-  A.HP = A.pol.hidden <= 32 ? 32 : 64;
-  const size_t bytes = (size_t)gen_layout(A.S, A.HP, A.KP, A.pol.d_act, A.hp.batch_size).total * 4;
-  if (A.HP == 32) {
+  A.HP = pd.hidden <= 32 ? 32 : 64;
+  *bytes = (size_t)gen_layout(A.S, A.HP, A.KP, pd.d_act, A.hp.batch_size).total * 4;
+  IMB_REQUIRE(*bytes <= IMB_SMEM_MAX, "policy / minibatch too large for the PPO update: k_ppo_update_gen<%d> needs %zu B "
+              "of shared memory per CTA, the limit is %d B", A.HP / 32, *bytes, (int)IMB_SMEM_MAX);
+  return A.HP == 32 ? IMB_PPO_PLAN_GEN1 : IMB_PPO_PLAN_GEN2;
+}
+
+extern "C" int imb_ppo_plan(const imb_policy_desc* pol, int32_t batch_size) {
+  PpoArgs A = {};
+  A.pol = *pol;
+  A.hp.batch_size = batch_size;
+  size_t bytes;
+  return ppo_plan(A, &bytes);
+}
+
+static int launch_ppo(const PpoArgs& A0, float* params, float* norm, int32_t* norm_count, float* m, float* v,
+                      const float* rollout, const int64_t* perm, float* loss_log, int64_t* state, cudaStream_t st) {
+  PpoArgs A = A0;
+  size_t bytes;
+  const int plan = ppo_plan(A, &bytes);
+  if (plan == IMB_PPO_PLAN_UPDATE) {
+    static size_t attr_bytes = 0;
+    return launch_cluster(k_ppo_update<32>, "k_ppo_update", bytes, &attr_bytes, st, A, params, norm, norm_count, m, v,
+                          rollout, perm, loss_log, state);
+  }
+  if (plan == IMB_PPO_PLAN_GEN1) {
     static size_t attr_bytes = 0;
     return launch_cluster(k_ppo_update_gen<1>, "k_ppo_update_gen<1>", bytes, &attr_bytes, st, A, params, norm, norm_count, m,
                           v, rollout, perm, loss_log, state);
   }
-  static size_t attr_bytes2 = 0;
-  return launch_cluster(k_ppo_update_gen<2>, "k_ppo_update_gen<2>", bytes, &attr_bytes2, st, A, params, norm, norm_count, m,
-                        v, rollout, perm, loss_log, state);
+  if (plan == IMB_PPO_PLAN_GEN2) {
+    static size_t attr_bytes2 = 0;
+    return launch_cluster(k_ppo_update_gen<2>, "k_ppo_update_gen<2>", bytes, &attr_bytes2, st, A, params, norm, norm_count,
+                          m, v, rollout, perm, loss_log, state);
+  }
+  return plan;
 }
-
-extern "C" int imb_rollout_row_width(const imb_policy_desc* pol);
 
 extern "C" int imb_ppo_update(const imb_policy_desc* pol, float* pol_params, float* pol_norm,
                               int32_t* pol_norm_count, float* exp_avg, float* exp_avg_sq, const float* rollout,
                               int64_t n_rows, const imb_ppo_hparams* hp, const int64_t* perm, uint64_t seed,
                               float* loss_log, int64_t* state, void* stream) {
-  IMB_REQUIRE(pol->hidden >= 1 && pol->hidden <= 64, "policy tower width must be <= 64");
-  IMB_REQUIRE(pol->d_obs <= IMB_MAX_DIN && pol->d_act <= IMB_MAX_DIN, "d_obs/d_act must be <= %d", IMB_MAX_DIN);
   IMB_REQUIRE(n_rows >= 1 && n_rows < (1ll << 31), "bad n_rows");
   PpoArgs A;
   A.pol = *pol;
   A.hp = *hp;
   A.n_rows = n_rows;
-  A.rw = imb_rollout_row_width(pol);
   A.seed = seed;
   return launch_ppo(A, pol_params, pol_norm, pol_norm_count, exp_avg, exp_avg_sq, rollout, perm, loss_log, state,
                     (cudaStream_t)stream);

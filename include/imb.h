@@ -311,6 +311,15 @@ int imb_ppo_update(const imb_policy_desc* pol, float* pol_params, float* pol_nor
                    const int64_t* perm, uint64_t seed, float* loss_log, int64_t* state,
                    void* stream);
 
+/* Which kernel imb_ppo_update runs for the policy `pol` at minibatch size batch_size; host only, no GPU needed.
+ * Honours IMB_PPO_FORCE_GENERAL.  <0 (imb_last_error() names the shared-memory need and limit) when no kernel can run
+ * the shape.  Shapes within k_ppo_update's width and minibatch whose shared memory or parameter slice does not fit it
+ * run on k_ppo_update_gen<1>. */
+#define IMB_PPO_PLAN_UPDATE 1  /* k_ppo_update: tower width <= 32, minibatch <= 64 rows */
+#define IMB_PPO_PLAN_GEN1 2    /* k_ppo_update_gen<1>: tower width <= 32 */
+#define IMB_PPO_PLAN_GEN2 3    /* k_ppo_update_gen<2>: tower width 33 to 64 */
+int imb_ppo_plan(const imb_policy_desc* pol, int32_t batch_size);
+
 /* log pi(a|s) of the generator policy for the disc batch (common.py:476-519 ->
  * ActorCriticPolicy.evaluate_actions), written into the batch's last feature row. */
 int imb_policy_logp(const imb_policy_desc* pol, const float* pol_params, const float* pol_norm,
