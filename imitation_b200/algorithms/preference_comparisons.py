@@ -32,6 +32,7 @@ from ..data import rollout, types
 from ..data.types import TrajectoryWithRew
 from ..rewards import reward_nets
 from ..util import logger as imit_logger
+from ..util.flat import views
 
 TrajectoryWithRewPair = Tuple[TrajectoryWithRew, TrajectoryWithRew]
 
@@ -889,16 +890,13 @@ class BasicRewardTrainer(RewardTrainer):
         if fo is None or fo["ptr"] != e.params.data_ptr():
             n, dev = e.desc.n_params, e.params.device
             m, v = th.zeros(n, device=dev), th.zeros(n, device=dev)
-            off = 0
-            for p in plist:
-                k = p.numel()
+            shapes = [p.shape for p in plist]
+            for p, pm, pv in zip(plist, views(m, shapes), views(v, shapes)):
                 st = self.optim.state.get(p)
                 if st:
-                    m[off:off + k] = st["exp_avg"].reshape(-1)
-                    v[off:off + k] = st["exp_avg_sq"].reshape(-1)
-                self.optim.state[p] = {"step": th.tensor(float(st["step"]) if st else 0.0),
-                                       "exp_avg": m[off:off + k].view(p.shape), "exp_avg_sq": v[off:off + k].view(p.shape)}
-                off += k
+                    pm.copy_(st["exp_avg"])
+                    pv.copy_(st["exp_avg_sq"])
+                self.optim.state[p] = {"step": th.tensor(float(st["step"]) if st else 0.0), "exp_avg": pm, "exp_avg_sq": pv}
             fo = dict(ptr=e.params.data_ptr(), m=m, v=v, state=th.zeros(_lib.ST_WORDS, dtype=th.int64, device=dev))
             self._fused_opt = fo
         g = self.optim.param_groups[0]

@@ -150,7 +150,7 @@ def trainer_round_sync(trainer, group=None) -> RoundSync:
         k = gen.policy.d_obs
         norms.append(NormStat(pn[:k], pn[k:2 * k], pc[0:1]))
     off = 0
-    for i, n in enumerate([m for m in eng._norms() if m is not None]):
+    for i, n in enumerate(eng.norms):
         k = n.running_mean.numel()
         if not disc_is_global:
             norms.append(NormStat(eng.norm_state[off:off + k], eng.norm_state[off + k:off + 2 * k],

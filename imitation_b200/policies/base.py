@@ -17,6 +17,7 @@ from torch import nn
 
 from .. import _desc, _lib, spaces
 from ..util import networks
+from ..util.flat import FlatAlias
 
 
 class NormalizeFeaturesExtractor(nn.Module):
@@ -76,8 +77,7 @@ class ActorCriticPolicy(nn.Module):
     def __getstate__(self):
         st = self.__dict__.copy()
         st["_flat"] = None
-        st.pop("_plist_cache", None)
-        st.pop("_flat_cache", None)
+        st.pop("_aliases", None)
         st.pop("_norm_state", None)
         st.pop("_norm_count", None)
         return st
@@ -87,61 +87,29 @@ class ActorCriticPolicy(nn.Module):
         self.desc = _desc.policy_desc(self.d_obs, self.d_act, self.discrete, self.hidden, self.normalize_features)
 
     # -- flat vectors for the kernels --------------------------------------------------------------------
-    def _plist(self):
-        out = self.__dict__.get("_plist_cache")
-        if out is None:
-            sd = dict(self.named_parameters())
-            out = [sd[name] for name, _ in _desc.policy_param_shapes(self.d_obs, self.d_act, self.discrete, self.hidden)]
-            self.__dict__["_plist_cache"] = out  # Parameter objects are stable (only .data is re-pointed)
-        return out
-
     def flat_vectors(self) -> Tuple[th.Tensor, th.Tensor, th.Tensor]:
         """(params, norm_state[mean|var], norm_count) aliased by the module's parameters/buffers."""
-        from ..rewards.reward_nets import FusedEngine
-
-        plist = self._plist()
-        # fast path: no parameter / buffer was re-pointed since the last full check
-        sig = [p.data_ptr() for p in plist]
-        if self.normalize_features:
-            n = self.features_extractor.normalize
-            sig += [n.running_mean.data_ptr(), n.running_var.data_ptr(), n.count.data_ptr()]
-        sig = tuple(sig)
-        cached = self.__dict__.get("_flat_cache")
-        if cached is not None and cached[0] == sig:
-            return cached[1]
-        dev = plist[0].device
+        aliases = self.__dict__.get("_aliases")
+        if aliases is None:
+            names = [name.rpartition(".") for name, _ in
+                     _desc.policy_param_shapes(self.d_obs, self.d_act, self.discrete, self.hidden)]
+            aliases = [FlatAlias([(self.get_submodule(path), attr) for path, _, attr in names])]
+            if self.normalize_features:
+                n = self.features_extractor.normalize
+                aliases += [FlatAlias([(n, "running_mean"), (n, "running_var")]), FlatAlias([(n, "count")])]
+            self.__dict__["_aliases"] = aliases
+        dev = aliases[0].tensors()[0].device
         if dev.type != "cuda":
             raise _lib.ImbError("imitation_b200 policies run on CUDA only (no CPU fallback)")
-        flat = FusedEngine._contiguous_view([p.data for p in plist], th.float32)
-        if flat is None:
-            flat = th.cat([p.detach().reshape(-1).float() for p in plist]).contiguous()
-            off = 0
-            for p in plist:
-                p.data = flat[off:off + p.numel()].view(p.shape)
-                off += p.numel()
+        flat = aliases[0].get(th.float32, dev)
         assert flat.numel() == self.desc.n_params
         if self.normalize_features:
-            n = self.features_extractor.normalize
-            ns = FusedEngine._contiguous_view([n.running_mean, n.running_var], th.float32)
-            nc = n.count.reshape(1) if (n.count.is_cuda and n.count.dtype == th.int32) else None
-            if ns is None or nc is None:
-                ns = th.cat([n.running_mean.detach().float(), n.running_var.detach().float()]).to(dev).contiguous()
-                nc = n.count.detach().to(th.int32).reshape(1).to(dev).contiguous()
-                k = self.d_obs
-                n._buffers["running_mean"], n._buffers["running_var"] = ns[:k], ns[k:]
-                n._buffers["count"] = nc.view(())
-        else:
-            ns = getattr(self, "_norm_state", None)
-            if ns is None or ns.device != dev:
-                object.__setattr__(self, "_norm_state", th.zeros(2, device=dev))
-                object.__setattr__(self, "_norm_count", th.zeros(1, dtype=th.int32, device=dev))
-            ns, nc = self._norm_state, self._norm_count
-        sig = [p.data_ptr() for p in plist]
-        if self.normalize_features:
-            n = self.features_extractor.normalize
-            sig += [n.running_mean.data_ptr(), n.running_var.data_ptr(), n.count.data_ptr()]
-        self.__dict__["_flat_cache"] = (tuple(sig), (flat, ns, nc))
-        return flat, ns, nc
+            return flat, aliases[1].get(th.float32, dev), aliases[2].get(th.int32, dev)
+        ns = self.__dict__.get("_norm_state")
+        if ns is None or ns.device != dev:
+            self.__dict__["_norm_state"] = th.zeros(2, device=dev)
+            self.__dict__["_norm_count"] = th.zeros(1, dtype=th.int32, device=dev)
+        return flat, self._norm_state, self._norm_count
 
     # -- SB3-compatible API (torch ops; not on the hot path) ------------------------------------------------
     def set_training_mode(self, mode: bool) -> None:

@@ -25,6 +25,7 @@ from torch import nn
 
 from .. import _desc, _lib, spaces
 from ..util import networks
+from ..util.flat import FlatAlias, views
 
 
 # ------------------------------------------------------------------------------------------------
@@ -36,6 +37,13 @@ class FusedEngine:
     def __init__(self, desc: _lib.DiscDesc, mlps: Sequence[nn.Sequential]):
         self.desc = desc
         self.mlps = list(mlps)  # [base mlp, (potential mlp)]
+        linears = [mod for m in self.mlps for mod in m if isinstance(mod, nn.Linear)]
+        self.norms = [m.normalize_input for m in self.mlps if hasattr(m, "normalize_input")]
+        self._params = FlatAlias([(lin, k) for lin in linears for k in ("weight", "bias")])
+        self._norm_state = self._norm_count = None
+        if self.norms:
+            self._norm_state = FlatAlias([(n, k) for n in self.norms for k in ("running_mean", "running_var")])
+            self._norm_count = FlatAlias([(n, "count") for n in self.norms])
         self.params: Optional[th.Tensor] = None
         self.norm_state: Optional[th.Tensor] = None
         self.norm_count: Optional[th.Tensor] = None
@@ -53,92 +61,28 @@ class FusedEngine:
 
     # -- aliasing ---------------------------------------------------------------------------------
     def _param_list(self) -> List[nn.Parameter]:
-        out = getattr(self, "_plist_cache", None)
-        if out is None:
-            out = []
-            for m in self.mlps:
-                for mod in m:
-                    if isinstance(mod, nn.Linear):
-                        out += [mod.weight, mod.bias]
-            self._plist_cache = out  # Parameter objects are stable (only their .data is re-pointed)
-        return out
-
-    def _norms(self) -> List[Optional[networks.BaseNorm]]:
-        return [getattr(m, "normalize_input", None) if hasattr(m, "normalize_input") else None for m in self.mlps]
+        return self._params.tensors()
 
     def device(self) -> th.device:
         return self._param_list()[0].device
-
-    @staticmethod
-    def _contiguous_view(tensors: List[th.Tensor], dtype) -> Optional[th.Tensor]:
-        """If `tensors` already sit back-to-back in one storage, return the flat view over them."""
-        t0 = tensors[0]
-        if t0.dtype != dtype or not t0.is_cuda:
-            return None
-        esz = t0.element_size()
-        ptr = t0.data_ptr()
-        total = 0
-        for t in tensors:
-            if (t.dtype != dtype or t.data_ptr() != ptr + esz * total or not t.is_contiguous()
-                    or t.untyped_storage().data_ptr() != t0.untyped_storage().data_ptr()):
-                return None
-            total += t.numel()
-        return t0.detach().as_strided((total,), (1,), t0.storage_offset())
 
     def sync(self) -> None:
         """(Re)establish that every parameter/buffer is a view of one flat vector.  Cheap when
         nothing moved; after `.to(device)` it re-flattens.  A sub-network (e.g. the base of a
         shaped net) accepts the enclosing net's flat vector because its slice is contiguous."""
-        plist = self._param_list()
-        # fast path (this runs on every kernel call of the API): nothing was re-pointed since the last full check
-        sig = self._signature(plist)
-        if sig == getattr(self, "_sig", None) and self.params is not None:
-            return
-        dev = plist[0].device
+        dev = self.device()
         if dev.type != "cuda":
             raise _lib.ImbError("imitation_b200 reward nets run on CUDA only (no CPU fallback): call .to('cuda')")
-        flat = self._contiguous_view([p.data for p in plist], th.float32)
-        if flat is None:
-            flat = th.cat([p.detach().reshape(-1).float() for p in plist]).contiguous()
-            off = 0
-            for p in plist:
-                p.data = flat[off:off + p.numel()].view(p.shape)
-                off += p.numel()
-        assert flat.numel() == self.desc.n_params, (flat.numel(), self.desc.n_params)
-        self.params = flat
-        norms = [n for n in self._norms() if n is not None]
-        if norms:
-            fl = []
-            for n in norms:
-                fl += [n.running_mean, n.running_var]
-            ns = self._contiguous_view(fl, th.float32)
-            nc = self._contiguous_view([n.count.reshape(1) for n in norms], th.int32)
-            if ns is None or nc is None:
-                ns = th.cat([t.detach().float().reshape(-1) for t in fl]).to(dev).contiguous()
-                nc = th.stack([n.count.detach().to(th.int32).reshape(()) for n in norms]).to(dev).contiguous()
-                off = 0
-                for i, n in enumerate(norms):
-                    k = n.running_mean.numel()
-                    n._buffers["running_mean"] = ns[off:off + k]
-                    n._buffers["running_var"] = ns[off + k:off + 2 * k]
-                    n._buffers["count"] = nc[i:i + 1].view(())
-                    off += 2 * k
-            self.norm_state, self.norm_count = ns, nc
+        self.params = self._params.get(th.float32, dev)
+        assert self.params.numel() == self.desc.n_params, (self.params.numel(), self.desc.n_params)
+        if self._norm_state is not None:
+            self.norm_state = self._norm_state.get(th.float32, dev)
+            self.norm_count = self._norm_count.get(th.int32, dev)
         elif self.norm_state is None or self.norm_state.device != dev:
             self.norm_state = th.zeros(2, device=dev)
             self.norm_count = th.zeros(2, dtype=th.int32, device=dev)
         if self.ws is None or self.ws.device != dev:
             self.ws = th.zeros(_lib.disc_workspace_floats(self.desc), device=dev)
-        self._sig = self._signature(plist)
-
-    def _signature(self, plist) -> tuple:
-        """Addresses of every tensor the kernels alias (parameters, RunningNorm buffers): unchanged addresses = the flat
-        vectors established by the last full `sync()` are still what the modules point at."""
-        sig = [p.data_ptr() for p in plist]
-        for n in self._norms():
-            if n is not None:
-                sig += [n.running_mean.data_ptr(), n.running_var.data_ptr(), n.count.data_ptr()]
-        return tuple(sig)
 
     @property
     def has_norm(self) -> bool:
@@ -207,12 +151,7 @@ class _FusedForward(th.autograd.Function):
         flat = th.empty(e.desc.n_params, device=grad_out.device)
         e.fwd_bwd(ctx.batch, ctx.ld, ctx.n, ctx.n, 0.0, grad_out.contiguous().float(), None, True, ctx.train_norm)
         e.reduce(flat)
-        grads, off = [], 0
-        for s in ctx.shapes:
-            k = int(np.prod(s))
-            grads.append(flat[off:off + k].view(s))
-            off += k
-        return (None, None, None, None, None, *grads)
+        return (None, None, None, None, None, *views(flat, ctx.shapes))
 
 
 # ------------------------------------------------------------------------------------------------
@@ -552,24 +491,15 @@ class NormalizedRewardNet(PredictProcessedWrapper):
         """Float vector + int32 vector aliased by the norm's buffers (for the kernels): RunningNorm [mean, var] and
         [count]; EMANorm [mean, var, inv_learning_rate] and [count, num_batches]."""
         n = self.normalize_output_layer
-        ema = self.output_norm_is_ema
-        fl = [n.running_mean, n.running_var] + ([n.inv_learning_rate] if ema else [])
-        it = [n.count] + ([n.num_batches] if ema else [])
+        alias = self.__dict__.get("_out_alias")
+        if alias is None or alias[0] is not n:
+            ema = self.output_norm_is_ema
+            fl = ["running_mean", "running_var"] + (["inv_learning_rate"] if ema else [])
+            it = ["count"] + (["num_batches"] if ema else [])
+            alias = (n, FlatAlias([(n, k) for k in fl]), FlatAlias([(n, k) for k in it]))
+            self.__dict__["_out_alias"] = alias
         dev = self.device
-        st, ct = getattr(self, "_out_state", None), getattr(self, "_out_count", None)
-        if (st is None or st.device != dev or st.numel() != len(fl) or ct.numel() != len(it)
-                or any(b.data_ptr() != st.data_ptr() + 4 * k for k, b in enumerate(fl))
-                or any(b.data_ptr() != ct.data_ptr() + 4 * k for k, b in enumerate(it))):
-            st = th.cat([b.detach().float().reshape(1) for b in fl]).to(dev)
-            ct = th.cat([b.detach().to(th.int32).reshape(1) for b in it]).to(dev).contiguous()
-            n._buffers["running_mean"], n._buffers["running_var"] = st[0:1], st[1:2]
-            n._buffers["count"] = ct[0].view(())
-            if ema:
-                n._buffers["inv_learning_rate"] = st[2].view(())
-                n._buffers["num_batches"] = ct[1].view(())
-            object.__setattr__(self, "_out_state", st)
-            object.__setattr__(self, "_out_count", ct)
-        return self._out_state, self._out_count
+        return alias[1].get(th.float32, dev), alias[2].get(th.int32, dev)
 
     def output_norm_args(self) -> tuple:
         """The member entry `_lib.pref_uncertainty_desc` takes: (state, count, eps), plus decay for an EMANorm."""
@@ -578,8 +508,7 @@ class NormalizedRewardNet(PredictProcessedWrapper):
 
     def __getstate__(self):
         state = self.__dict__.copy()
-        state.pop("_out_state", None)
-        state.pop("_out_count", None)
+        state.pop("_out_alias", None)
         return state
 
 

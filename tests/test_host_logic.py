@@ -222,6 +222,7 @@ def _install_cpu_stand_ins():
     subsets, minibatch order (torch RNG bookkeeping for skipped members) or the broadcasts changes the result."""
     from imitation_b200 import _lib
     from imitation_b200.rewards import reward_nets
+    from imitation_b200.util.flat import views
 
     E = reward_nets.FusedEngine
 
@@ -233,10 +234,8 @@ def _install_cpu_stand_ins():
             return
         plist = self._param_list()
         flat = th.cat([p.detach().reshape(-1) for p in plist])
-        off = 0
-        for p in plist:
-            p.data = flat[off:off + p.numel()].view(p.shape)
-            off += p.numel()
+        for p, v in zip(plist, views(flat, [p.shape for p in plist])):
+            p.data = v
         self.params, self.norm_state, self.norm_count = flat, th.zeros(2), th.zeros(2, dtype=th.int32)
         self.ws = th.zeros(8)
         self._cpu_synced = True
