@@ -106,6 +106,7 @@ SYMBOLS = [
     "imb_disc_sample_gather", "imb_sample_advance2", "imb_disc_reduce_adam", "imb_norm_batch_stats", "imb_norm_fold",
     "imb_disc_set_rows", "imb_stats_publish", "imb_pref_loss", "imb_pref_uncertainty_ws_floats", "imb_pref_uncertainty",
     "imb_rollout_ensemble", "imb_ensemble_relabel_ws_floats", "imb_ensemble_relabel", "imb_disc_plan", "imb_ppo_plan",
+    "imb_ppo_update_variant",
 ]
 
 # imb_disc_plan codes: the kernel imb_disc_fwd_bwd runs
@@ -460,6 +461,12 @@ def ppo_plan(pol: PolicyDesc, batch_size: int) -> int:
     if rc < 0:
         raise ImbError(f"imb_ppo_plan: {lib().imb_last_error().decode()} (rc={rc})")
     return rc
+
+
+def ppo_update_variant(pol: PolicyDesc) -> int:
+    """Instantiation of k_ppo_update that `ppo_update` runs for `pol` when `ppo_plan` gives PPO_PLAN_UPDATE (host only):
+    0 = the runtime-shape one, 1-3 = the shape-specialised ones (include/imb.h); IMB_PPO_FORCE_RUNTIME_SHAPE=1 forces 0."""
+    return int(lib().imb_ppo_update_variant(C.byref(pol)))
 
 
 def policy_logp(pol, params, norm, batch, ld, n, row_logp):

@@ -27,6 +27,12 @@ extern thread_local char g_imb_err[512];
     if (!(cond)) IMB_FAIL(-1, __VA_ARGS__); \
   } while (0)
 
+// floats per rollout-table row: obs | action (one column when discrete) | 5 scalars, padded to a multiple of 4 floats so
+// that rows are 16-byte aligned and the PPO update can stage a minibatch row with 16-byte copies
+__host__ __device__ constexpr int imb_row_width(int d_obs, int d_act, bool discrete) {
+  return (d_obs + (discrete ? 1 : d_act) + 5 + 3) / 4 * 4;
+}
+
 static inline int imb_num_sms() {
   static int n = 0;
   if (n == 0) {

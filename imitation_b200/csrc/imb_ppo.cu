@@ -66,9 +66,8 @@ struct PpoArgs {
 struct PLay {
   int w1[2], b1[2], w2[2], b2[2], wa, ba, wv, bv, ls, ldo, ldh, total;
 };
-__host__ __device__ inline PLay make_play(const imb_policy_desc& pd) {
-  PLay L;
-  const int Do = pd.d_obs, Da = pd.d_act, h = pd.hidden;
+__host__ __device__ inline PLay make_play(const int Do, const int Da, const int h, const bool discrete) {
+  PLay L{};
   L.ldo = Do | 1;
   L.ldh = h | 1;
   int o = 0;
@@ -82,10 +81,21 @@ __host__ __device__ inline PLay make_play(const imb_policy_desc& pd) {
   L.ba = o; o += Da;
   L.wv = o; o += h;
   L.bv = o; o += 1;
-  L.ls = o; o += pd.discrete ? 0 : Da;
+  L.ls = o; o += discrete ? 0 : Da;
   L.total = o;
   return L;
 }
+__host__ __device__ inline PLay make_play(const imb_policy_desc& pd) {
+  return make_play(pd.d_obs, pd.d_act, pd.hidden, pd.discrete != 0);
+}
+// Launch geometry of k_ppo_update, from the shape alone (the host plans with these, a shape-specialised instantiation
+// folds them into constants): obs width padded to 32 or 64; padded-layout parameters per slice, a multiple of 4 and at
+// least two quads (a quad's owner is qq / (S / 4), found through the 32-bit reciprocal 2^32 / (S / 4) + 1 when S is not
+// a compile-time constant, which does not fit for S / 4 = 1: policies of <= 32 padded parameters, e.g. width 1); staged
+// row stride >= rw, = 4 (mod 8).
+__host__ __device__ inline int ppo_kp(const int Do) { return Do <= 32 ? 32 : 64; }
+__host__ __device__ inline int ppo_slice(const PLay& L) { return max(8, ((L.total + CL - 1) / CL + 3) / 4 * 4); }
+__host__ __device__ inline int ppo_row_stride(const int rw) { return ((rw + 4) % 8 == 4) ? rw + 4 : rw + 8; }
 // torch-flat parameter index -> P-layout index
 __device__ inline int flat_to_play(const imb_policy_desc& pd, const PLay& L, int p) {
   const int Do = pd.d_obs, Da = pd.d_act, h = pd.hidden;
@@ -188,7 +198,12 @@ __device__ __forceinline__ void tower_wgrad(const int tnet, const int gj, const 
         if (i < h) GP[o.w2 + gj * o.ldh + i] = r[t];
       }
     }
-    for (int k0 = wq; k0 < Do; k0 += 4 * NQ) {  // dW1[gj][k], four at a time
+    // (the loops over inputs run from 0 with the thread's offset added inside, so that their trip counts are compile-time
+    // constants when the shape is)
+#pragma unroll
+    for (int kb = 0; kb < Do; kb += 4 * NQ) {  // dW1[gj][k], four at a time
+      const int k0 = kb + wq;
+      if (k0 >= Do) break;
       float r[4];
 #pragma unroll
       for (int t = 0; t < 4; ++t) {
@@ -202,8 +217,10 @@ __device__ __forceinline__ void tower_wgrad(const int tnet, const int gj, const 
       }
     }
     if (tnet == 0) {
-      for (int a0 = wq; a0 < Da; a0 += 2 * NQ) {
-        const int a1 = a0 + NQ;
+#pragma unroll
+      for (int ab = 0; ab < Da; ab += 2 * NQ) {
+        const int a0 = ab + wq, a1 = a0 + NQ;
+        if (a0 >= Da) break;
         const float ra = dot8r(lt, DM + a0 * RLc), rb = dot8r(lt, DM + (a1 < Da ? a1 : a0) * RLc);
         GP[o.wa + a0 * o.ldh + gj] = ra;
         if (a1 < Da) GP[o.wa + a1 * o.ldh + gj] = rb;
@@ -216,7 +233,10 @@ __device__ __forceinline__ void tower_wgrad(const int tnet, const int gj, const 
   }
   if (wq == NQ - 1) {
     if (tnet == 0) {  // ba, log_std
-      for (int t = gj; t < 2 * Da; t += HPx) {
+#pragma unroll
+      for (int tb = 0; tb < 2 * Da; tb += HPx) {
+        const int t = tb + gj;
+        if (t >= 2 * Da) break;
         if (t < Da) {
           load8(dz2, DM + t * RLc);
           GP[o.ba + t] = sum8(dz2);
@@ -252,7 +272,12 @@ __device__ __forceinline__ void tower_wgrad(const int tnet, const int gj, const 
 //     own with a local store).
 // No cluster barrier inside the step loop (the exchanged data signals mbarriers at the receivers), three CTA
 // barriers per optimiser step; the only global-memory traffic inside a step is the asynchronous minibatch prefetch.
-template <int HP>
+// DO != 0: an instantiation for one policy shape (DO obs, DA actions, DISC discrete, NORM feature RunningNorm, tower width
+// HP), whose loop bounds, layout offsets and slice geometry are compile-time constants -- the loops of the step unroll
+// completely and every shared-memory address is an immediate offset, instead of unrolled blocks plus guarded remainder
+// iterations that expose a shared-memory latency on the dependent FMA chain at every block boundary.  The arithmetic and
+// its order are the same in every instantiation.  DO = 0: the shape is read from A.pol (every other shape).
+template <int HP, int DO = 0, int DA = 0, int DISC = 0, int NORM = 0>
 __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __restrict__ g_params,
                                                       float* __restrict__ g_norm, int32_t* __restrict__ g_norm_count,
                                                       float* __restrict__ g_m, float* __restrict__ g_v,
@@ -271,7 +296,13 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
   __shared__ float SSQ[CL];                  // squared gradient norms of the 8 slices (each written by its owner)
   __shared__ float nred[PT / 32];            // per-warp partial sums of the owned slice's squared norm
   const imb_policy_desc& pd = A.pol;
-  const int Do = pd.d_obs, Da = pd.d_act, h = pd.hidden, NP = pd.n_params, KP = A.KP, S = A.S;
+  constexpr bool SPEC = DO != 0;
+  const int Do = SPEC ? DO : pd.d_obs, Da = SPEC ? DA : pd.d_act, h = SPEC ? HP : pd.hidden, NP = pd.n_params;
+  const bool discrete = SPEC ? DISC != 0 : pd.discrete != 0, has_norm = SPEC ? NORM != 0 : pd.has_norm != 0;
+  const PLay PL = make_play(Do, Da, h, discrete);
+  const int KP = SPEC ? ppo_kp(Do) : A.KP, S = SPEC ? ppo_slice(PL) : A.S;
+  // unroll factors of the chain's loops: complete for a compile-time shape
+  constexpr int U_DO = SPEC ? DO : 8, U_H = SPEC ? HP : 8, U_DA = SPEC ? DA : 4;
   // Thread t < S / 4 owns quad t of this CTA's slice, so warps 0 .. n_own_w - 1 hold owned quads.  The warps above them
   // and above the chain's warps 0-3 run the next minibatch's statistics in the TAIL of the step, beside the slice sum,
   // norm exchange and Adam, so that nothing shared-memory heavy competes with the chain for issue slots; they issue the
@@ -280,12 +311,12 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
   const int n_own_w = (S / 4 + 31) / 32;
   const bool tail_stats = n_own_w <= PT / 32 - 2;
   const int st0 = tail_stats ? 32 * max(n_own_w, 4) : 128, nst = PT - st0;  // first statistics thread, their count
-  const PLay PL = make_play(pd);
   const int ldo = PL.ldo, ldh = PL.ldh;
-  const int da_store = pd.discrete ? 1 : Da;
+  const int da_store = discrete ? 1 : Da;
   const int col_logp = Do + da_store, col_adv = col_logp + 3, col_ret = col_logp + 4;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int rw = A.rw, RS2 = A.RS2;          // rollout row width (multiple of 4) / staged row stride (= 4 mod 8)
+  // rollout row width (multiple of 4) / staged row stride (= 4 mod 8)
+  const int rw = SPEC ? imb_row_width(Do, Da, discrete) : A.rw, RS2 = SPEC ? ppo_row_stride(rw) : A.RS2;
   auto al = [](int x) { return (x + 31) / 32 * 32; };
 
   // ---- shared-memory carve-up (identical in every CTA: DSMEM addresses are rank + offset) ---------------
@@ -316,8 +347,8 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
   for (int i = tid; i < 3 * rsz; i += PT) ROWS[i] = 0.f;
   for (int i = tid; i < 2 * xsz + 8 * HP * RL + 3 * DAP * RL + 32; i += PT) XNo[i] = 0.f;  // XNo .. DVAL contiguous
   if (tid < 64) {
-    rstat[tid] = (pd.has_norm && tid < Do) ? g_norm[tid] : 0.f;
-    rstat[64 + tid] = (pd.has_norm && tid < Do) ? g_norm[Do + tid] : 1.f;
+    rstat[tid] = (has_norm && tid < Do) ? g_norm[tid] : 0.f;
+    rstat[64 + tid] = (has_norm && tid < Do) ? g_norm[Do + tid] : 1.f;
     LOSS[tid & 31] = 0.f;
   }
   if (tid == 0) {
@@ -336,7 +367,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
     Ms[q] = g_m[p];
     Vs[q] = g_v[p];
   }
-  int32_t run_count = pd.has_norm ? *g_norm_count : 0;
+  int32_t run_count = has_norm ? *g_norm_count : 0;
 
   const int64_t N = A.n_rows;
   const int Ni = (int)N;
@@ -358,8 +389,10 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
   auto issue_gather = [&](int ep, int start, int buf) {
     if (tid < st0) return;
     const int nbx = min(mb, Ni - start);
-    for (int t = tid - st0; t < 2 * PR; t += nst) {
-      const int r = t >> 1, half = t & 1;
+#pragma unroll
+    for (int tb = 0; tb < 2 * PR; tb += nst) {
+      const int t = tb + tid - st0, r = t >> 1, half = t & 1;
+      if (t >= 2 * PR) break;
       if (r >= nbx) continue;
       int64_t idx;
       if (perm_in) {
@@ -371,7 +404,12 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
       const float* src = rollout + idx * rw;
       float* dst = ROWS + buf * rsz + r * RS2;
       const int nq = rw >> 2, q0 = half ? (nq + 1) >> 1 : 0, q1 = half ? nq : (nq + 1) >> 1;
-      for (int q = q0; q < q1; ++q) cp_async16(dst + 4 * q, src + 4 * q);
+#pragma unroll
+      for (int qi = 0; qi < (nq + 1) >> 1; ++qi) {
+        const int q = q0 + qi;
+        if (q >= q1) break;
+        cp_async16(dst + 4 * q, src + 4 * q);
+      }
     }
     cp_async_mbar_arrive(&mbar[buf]);
   };
@@ -388,6 +426,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
     const int gl = tid & 7;
     const float inv_nbx = 1.0f / (float)nbx;
     mbar_wait(&mbar[buf], (uint32_t)((gs2 / 3) & 1));  // all 64 row copies have landed
+#pragma unroll
     for (int task0 = 0; task0 <= Do; task0 += ngrp) {
       const int task = task0 + gidx;
       const bool is_feat = task < Do, is_adv = task == Do;
@@ -408,7 +447,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
       const float ssd = group8_sum(q);
       if (is_feat) {
         float mean = 0.f, istd = 1.f;
-        if (pd.has_norm) {  // every lane of the group computes the update; lane 0 stores it
+        if (has_norm) {  // every lane of the group computes the update; lane 0 stores it
           mean = rstat[task];
           float var = rstat[64 + task];
           const float bvar = ssd * inv_nbx;
@@ -441,7 +480,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
   issue_gather(0, 0, 0);
   if (n_steps > 1) issue_gather(mb >= Ni ? 1 : 0, mb >= Ni ? 0 : mb, 1);
   minibatch_stats(0, min(mb, Ni), tid >> 3, PT / 8);
-  if (pd.has_norm) run_count += min(mb, Ni);  // (every thread keeps the count; the statistics' owners use it)
+  if (has_norm) run_count += min(mb, Ni);  // (every thread keeps the count; the statistics' owners use it)
   // The gradient exchange is synchronised by the data itself: every 16-byte DSMEM store (st.async) completes
   // bytes on an mbarrier of the RECEIVING CTA, which waits until the expected byte count of the phase has
   // landed -- no cluster-wide barrier inside the step loop.  Each barrier is re-armed (one arrival + expected
@@ -530,7 +569,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
       const int c_b1 = cnet ? PL.b1[1] : PL.b1[0], c_b2 = cnet ? PL.b2[1] : PL.b2[0];
       // policy warps: everything the loss needs that does not depend on the forward pass is fetched now, so its
       // latency (shared-memory loads, the exponential) hides behind the layers
-      const bool gfast = cnet == 0 && !pd.discrete && Da <= 8;  // one action per lane of the octet
+      const bool gfast = cnet == 0 && !discrete && Da <= 8;  // one action per lane of the octet
       float pre_adv = 0.f, pre_lpo = 0.f, pre_act = 0.f, pre_ls = 0.f, pre_ivar = 0.f;
       if (cnet == 0) {
         pre_adv = row[col_adv];
@@ -545,7 +584,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
       float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
       {
         const float* wp = cW1 + jc * ldo;
-#pragma unroll 8
+#pragma unroll U_DO
         for (int k = 0; k < Do; ++k) {
           const float w = wp[k];
           const float4 x = ld4(XNc + k * RL + r0);
@@ -565,7 +604,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
       a0 = a1 = a2 = a3 = 0.f;
       {
         const float* wp = cW2 + jc * ldh;
-#pragma unroll 8
+#pragma unroll U_H
         for (int i = 0; i < h; ++i) {
           const float w = wp[i];
           const float4 x = ld4(cH1 + i * RL + r0);
@@ -620,6 +659,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
         {
           const int asub = lane >> 2, q = lane & 3;
           const bool b0 = (lane & 1) != 0, b1 = (lane & 2) != 0;
+#pragma unroll
           for (int ab = 0; ab < Da; ab += 8) {
             const int a = ab + asub, ac = a < Da ? a : 0;
             const float* wr = Wa + ac * ldh + q;
@@ -657,7 +697,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
             r_dm = diff * pre_ivar;
             r_dls = d2 - 1.0f;
           }
-        } else if (!pd.discrete) {
+        } else if (!discrete) {
           const float* lstd = Pm + PL.ls;
           for (int a = la; a < Da; a += 8) {
             const float ls = lstd[a], ivar = __expf(-2.0f * ls);
@@ -687,7 +727,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
         }
         logp = oct_sum(logp);
         PPO_WCLK(6);
-        if (pd.discrete || loss_log) ent = oct_sum(ent);  // (Gaussian: the entropy only feeds the loss log)
+        if (discrete || loss_log) ent = oct_sum(ent);  // (Gaussian: the entropy only feeds the loss log)
         const float ratio = __expf(logp - logp_old);
         const float lo = 1.0f - A.hp.clip_range, hi = 1.0f + A.hp.clip_range;
         const float pl1 = adv * ratio, pl2 = adv * fminf(fmaxf(ratio, lo), hi);
@@ -708,7 +748,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
             DLS[la * RL + r0 + rr] = dl_dlogp * r_dls + dent;  // dH/dlog_std = 1
             DM[la * RL + r0 + rr] = dl_dlogp * r_dm;
           }
-        } else if (!pd.discrete) {
+        } else if (!discrete) {
           for (int a = la; a < Da; a += 8) {
             DLS[a * RL + r0 + rr] = dl_dlogp * DLS[a * RL + r0 + rr] + dent;  // dH/dlog_std = 1
             DM[a * RL + r0 + rr] = dl_dlogp * DM[a * RL + r0 + rr];
@@ -722,7 +762,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
         }
         __syncwarp();
         PPO_WCLK(7);
-#pragma unroll 4
+#pragma unroll U_DA
         for (int a = 0; a < Da; ++a) {
           const float waj = Wa[a * ldh + jc];
           const float4 d = ld4(DM + a * RL + r0);
@@ -741,7 +781,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
       a0 = a1 = a2 = a3 = 0.f;
       {
         const float* wp = cW2 + jc;
-#pragma unroll 8
+#pragma unroll U_H
         for (int jj = 0; jj < h; ++jj) {
           const float w = wp[jj * ldh];
           const float4 d = ld4(cDZ2 + jj * RL + r0);
@@ -761,7 +801,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
     //          warps 2-7 meet on a named barrier and compute them while warps 0, 1 are still in the policy chain ------
     if (warp >= 2) {
       asm volatile("bar.sync 1, 192;" ::: "memory");
-      tower_wgrad<6, HP>(1, lane, warp - 2, h, Do, Da, pd.discrete != 0, wo_v, GP, TH1 + HP * RL, TLAT + HP * RL,
+      tower_wgrad<6, HP>(1, lane, warp - 2, h, Do, Da, discrete, wo_v, GP, TH1 + HP * RL, TLAT + HP * RL,
                          TDZ2 + HP * RL, TDZ1 + HP * RL, XNc, DM, DLS, DVAL);
     }
     PPO_WCLK(8);
@@ -780,16 +820,20 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
     __syncthreads();
     PPO_TICK(3);
     // ---- 2. the POLICY tower's weight gradients (and the action head's) by all eight warps ------------------------------
-    tower_wgrad<PT / 32, HP>(0, lane, warp, h, Do, Da, pd.discrete != 0, wo_p, GP, TH1, TLAT, TDZ2, TDZ1, XNc, DM, DLS, DVAL);
+    tower_wgrad<PT / 32, HP>(0, lane, warp, h, Do, Da, discrete, wo_p, GP, TH1, TLAT, TDZ2, TDZ1, XNc, DM, DLS, DVAL);
     __syncthreads();
     PPO_TICK(7);
     // ---- 3. push the partials to the PEER slice owners: RECV[this CTA][i], one 16-byte DSMEM store per quad ------------
     // CTA c starts with the quads owned by CTA c+1 and stops before its own slice (which its slice sum reads from GP),
     // so at any time the 8 senders target 8 different receivers
-    for (int q = tid; q < (CL - 1) * (S / 4); q += PT) {
+#pragma unroll
+    for (int qb = 0; qb < (CL - 1) * (S / 4); qb += PT) {
+      const int q = qb + tid;
+      if (q >= (CL - 1) * (S / 4)) break;
       int qq = q + ((crank + 1) & (CL - 1)) * (S / 4);
       if (qq >= CL * S / 4) qq -= CL * S / 4;
-      const int p0 = 4 * qq, owner = (int)__umulhi((unsigned)qq, qmagic);  // = qq / (S / 4)
+      // owner = qq / (S / 4): a plain division when S is a compile-time constant
+      const int p0 = 4 * qq, owner = SPEC ? qq / (S / 4) : (int)__umulhi((unsigned)qq, qmagic);
       st_async_v4(mapa_u32(recv_sa + (uint32_t)(crank * S + (p0 - owner * S)) * 4u, owner), ld4(GP + p0),
                   mapa_u32(xbar0_sa, owner));
     }
@@ -889,7 +933,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
       if (tid == 0) mbar_expect_tx(&xbar[1], xbytes);  // re-arm for the next step
       PPO_TICK(12);
     }
-    if (pd.has_norm && gs + 1 < n_steps) run_count += min(mb, Ni - start_next);  // (after the statistics that read it)
+    if (has_norm && gs + 1 < n_steps) run_count += min(mb, Ni - start_next);  // (after the statistics that read it)
     ep_now = ep_next;
     start = start_next;
     // (the barrier at the top of the next step orders these parameter writes before their first use)
@@ -912,7 +956,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
   }
   if (crank == 0) {
     for (int p = tid; p < NP; p += PT) g_params[p] = Pm[flat_to_play(pd, PL, p)];
-    if (pd.has_norm) {
+    if (has_norm) {
       if (tid < Do) {
         g_norm[tid] = rstat[tid];
         g_norm[Do + tid] = rstat[64 + tid];
@@ -1069,11 +1113,9 @@ static int ppo_plan(PpoArgs& A, size_t* bytes) {
   IMB_REQUIRE(A.hp.batch_size >= 1 && A.hp.batch_size <= GEN_MAX_MB, "PPO minibatch size must be in [1, %d]", GEN_MAX_MB);
   A.rw = imb_rollout_row_width(&pd);
   IMB_REQUIRE(A.rw % 4 == 0, "rollout row width must be a multiple of 4 floats (bulk row copies)");
-  A.KP = pd.d_obs <= 32 ? 32 : 64;
-  // at least two quads per slice: k_ppo_update finds a quad's owner as qq / (S / 4) through the 32-bit reciprocal
-  // 2^32 / (S / 4) + 1, which does not fit for S / 4 = 1 (policies of <= 32 padded parameters, e.g. width 1)
-  A.S = max(8, ((make_play(pd).total + CL - 1) / CL + 3) / 4 * 4);
-  A.RS2 = ((A.rw + 4) % 8 == 4) ? A.rw + 4 : A.rw + 8;
+  A.KP = ppo_kp(pd.d_obs);
+  A.S = ppo_slice(make_play(pd));
+  A.RS2 = ppo_row_stride(A.rw);
   // IMB_PPO_FORCE_GENERAL=1 (tests): run the general kernel on shapes the specialised one covers
   const char* force = getenv("IMB_PPO_FORCE_GENERAL");
   if (pd.hidden <= 32 && A.hp.batch_size <= PR && !(force && force[0] == '1')) {
@@ -1096,15 +1138,51 @@ extern "C" int imb_ppo_plan(const imb_policy_desc* pol, int32_t batch_size) {
   return ppo_plan(A, &bytes);
 }
 
+// The policy shapes with their own instantiation of k_ppo_update (tower width 32): the policies bench.py trains.
+// Entry i is instantiation i + 1 of imb_ppo_update_variant.
+struct PpoShape {
+  int d_obs, d_act, discrete, has_norm;
+};
+constexpr PpoShape kPpoShapes[] = {
+    {17, 6, 0, 1},  // HalfCheetah-shaped Box with NormalizeFeaturesExtractor (GAIL and AIRL)
+    {27, 8, 0, 1},  // Ant-shaped Box with NormalizeFeaturesExtractor
+    {4, 2, 1, 0},   // CartPole-shaped Discrete
+};
+template <int I>
+constexpr auto k_ppo_update_spec =
+    k_ppo_update<32, kPpoShapes[I].d_obs, kPpoShapes[I].d_act, kPpoShapes[I].discrete, kPpoShapes[I].has_norm>;
+constexpr decltype(&k_ppo_update<32>) kPpoUpdateKernels[] = {k_ppo_update<32>, k_ppo_update_spec<0>, k_ppo_update_spec<1>,
+                                                            k_ppo_update_spec<2>};
+constexpr const char* kPpoUpdateNames[] = {"k_ppo_update", "k_ppo_update<17x6 Box, norm>", "k_ppo_update<27x8 Box, norm>",
+                                           "k_ppo_update<4x2 Discrete>"};
+constexpr int kNumPpoVariants = sizeof(kPpoUpdateKernels) / sizeof(kPpoUpdateKernels[0]);
+
+// Which instantiation of k_ppo_update runs `pd` (when it runs k_ppo_update at all): 1 + its index in kPpoShapes, or 0
+// for the runtime-shape one.  IMB_PPO_FORCE_RUNTIME_SHAPE=1 (tests), read at every call, forces 0.
+static int ppo_variant(const imb_policy_desc& pd) {
+  const char* force = getenv("IMB_PPO_FORCE_RUNTIME_SHAPE");
+  if ((force && force[0] == '1') || pd.hidden != 32) return 0;
+  for (int i = 0; i < kNumPpoVariants - 1; ++i) {
+    const PpoShape& s = kPpoShapes[i];
+    if (pd.d_obs == s.d_obs && pd.d_act == s.d_act && (pd.discrete != 0) == (s.discrete != 0) &&
+        (pd.has_norm != 0) == (s.has_norm != 0))
+      return i + 1;
+  }
+  return 0;
+}
+
+extern "C" int imb_ppo_update_variant(const imb_policy_desc* pol) { return ppo_variant(*pol); }
+
 static int launch_ppo(const PpoArgs& A0, float* params, float* norm, int32_t* norm_count, float* m, float* v,
                       const float* rollout, const int64_t* perm, float* loss_log, int64_t* state, cudaStream_t st) {
   PpoArgs A = A0;
   size_t bytes;
   const int plan = ppo_plan(A, &bytes);
   if (plan == IMB_PPO_PLAN_UPDATE) {
-    static size_t attr_bytes = 0;
-    return launch_cluster(k_ppo_update<32>, "k_ppo_update", bytes, &attr_bytes, st, A, params, norm, norm_count, m, v,
-                          rollout, perm, loss_log, state);
+    static size_t attr_bytes[kNumPpoVariants] = {};
+    const int var = ppo_variant(A.pol);
+    return launch_cluster(kPpoUpdateKernels[var], kPpoUpdateNames[var], bytes, &attr_bytes[var], st, A, params, norm,
+                          norm_count, m, v, rollout, perm, loss_log, state);
   }
   if (plan == IMB_PPO_PLAN_GEN1) {
     static size_t attr_bytes = 0;

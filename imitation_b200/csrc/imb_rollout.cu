@@ -2,9 +2,7 @@
 #include "imb_rollout_impl.cuh"
 
 extern "C" int imb_rollout_row_width(const imb_policy_desc* pol) {
-  // padded to a multiple of 4 floats: rows are 16-byte aligned, so the PPO update can stage a minibatch row
-  // with one bulk-async copy
-  return (pol->d_obs + (pol->discrete ? 1 : pol->d_act) + 5 + 3) / 4 * 4;
+  return imb_row_width(pol->d_obs, pol->d_act, pol->discrete != 0);
 }
 
 // members == nullptr: imb_rollout; otherwise imb_rollout_ensemble (reward_mode 2, member m's vectors from the table)

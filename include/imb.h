@@ -320,6 +320,13 @@ int imb_ppo_update(const imb_policy_desc* pol, float* pol_params, float* pol_nor
 #define IMB_PPO_PLAN_GEN2 3    /* k_ppo_update_gen<2>: tower width 33 to 64 */
 int imb_ppo_plan(const imb_policy_desc* pol, int32_t batch_size);
 
+/* Which instantiation of k_ppo_update imb_ppo_update runs for `pol` when imb_ppo_plan returns IMB_PPO_PLAN_UPDATE; host
+ * only.  0: the one that reads the shape at run time (every shape without its own); 1: 17 obs / 6 actions Box with a
+ * feature RunningNorm; 2: 27 / 8 Box with a feature RunningNorm; 3: 4 obs / Discrete(2) without one (all of width 32).
+ * The shape-specialised instantiations compute bit for bit what the runtime-shape one computes.  Honours
+ * IMB_PPO_FORCE_RUNTIME_SHAPE=1, which imb_ppo_update reads at every call and which makes it run instantiation 0. */
+int imb_ppo_update_variant(const imb_policy_desc* pol);
+
 /* log pi(a|s) of the generator policy for the disc batch (common.py:476-519 ->
  * ActorCriticPolicy.evaluate_actions), written into the batch's last feature row. */
 int imb_policy_logp(const imb_policy_desc* pol, const float* pol_params, const float* pol_norm,
