@@ -980,47 +980,28 @@ __global__ void k_stats_publish(const float* __restrict__ stats_dev, int n, floa
 }
 
 // ---- forward only (reward relabel / predict) ---------------------------------------------------
-// thread per row straight from global memory (coalesced over rows for each feature).
-template <int H>
+// thread per row straight from global memory (coalesced over rows for each feature); one TImg per pass, img_sz apart,
+// then xn_ld >= din normalised inputs per thread.
+template <int JP>
 __global__ void __launch_bounds__(NT) k_reward_fwd(const DiscLaunch L, const float* __restrict__ params,
-                                                  const float* __restrict__ batch, int64_t ld, int64_t n,
-                                                  int out_mode, float* __restrict__ out, int img1_off, int xn_off,
-                                                  int xn_ld) {
+                                                   const float* __restrict__ batch, int64_t ld, int64_t n,
+                                                   int out_mode, float* __restrict__ out, int img_sz, int xn_ld) {
   extern __shared__ __align__(128) float smem[];
-  float* img[MAX_PASS] = {smem, smem + img1_off, smem + img1_off};
-  float* XN = smem + xn_off;
   const int tid = threadIdx.x;
-  load_mlp<H>(img[0], L.pass[0], params);
-  float* mean2 = nullptr;
-  float* istd2 = nullptr;
-  if (L.npass == 3) {
-    load_mlp<H>(img[1], L.pass[1], params);
-    const int din = L.pass[2].din;
-    mean2 = img[1] + MlpSm<H>::size(din);
-    istd2 = mean2 + IMB_MAX_DIN;
-    for (int i = tid; i < din; i += NT) {
-      if (L.pass[2].has_norm) {
-        mean2[i] = L.pass[2].norm[i];
-        istd2[i] = 1.0f / sqrtf(L.pass[2].norm[din + i] + L.pass[2].eps);
-      } else {
-        mean2[i] = 0.f;
-        istd2[i] = 1.f;
-      }
-    }
-  }
+  for (int p = 0; p < L.npass; ++p) load_timg(smem + p * img_sz, L.pass[p], JP, params, L.pass[p].norm, L.pass[p].eps);
   __syncthreads();
-  float h1[H], h2[H];
+  float* xn = smem + L.npass * img_sz + tid * xn_ld;
   for (int64_t row = (int64_t)blockIdx.x * NT + tid; row < n; row += (int64_t)gridDim.x * NT) {
     const float done = (L.done_slot >= 0) ? batch[(int64_t)L.stage_row[L.done_slot] * ld + row] : 0.f;
     float logit = 0.f;
     for (int p = 0; p < L.npass; ++p) {
       const PassDesc& P = L.pass[p];
-      const float* mean = (p == 2) ? mean2 : img[p] + MlpSm<H>::mean_off(P.din);
-      const float* istd = (p == 2) ? istd2 : img[p] + MlpSm<H>::istd_off(P.din);
-      float* xn = XN + tid * xn_ld;
+      const float* img = smem + p * img_sz;
+      const float* mean = img + TImg::mean(P.din, JP);
+      const float* istd = img + TImg::istd(P.din, JP);
       for (int k = 0; k < P.din; ++k)
         xn[k] = (batch[(int64_t)L.stage_row[P.in_slot[k]] * ld + row] - mean[k]) * istd[k];
-      const float o = mlp_forward_row<H, false>(img[p], P, xn, h1, h2);
+      const float o = timg_forward_row<JP>(img, P, xn);
       logit = fmaf(pass_coef(P.coef_kind, L.gamma, done), o, logit);
     }
     if (out_mode >= 1 && L.logp_slot >= 0) logit -= batch[(int64_t)L.stage_row[L.logp_slot] * ld + row];
@@ -1100,36 +1081,6 @@ __global__ void __launch_bounds__(1024) k_reward_norm_scan(float* __restrict__ r
       count[1] = nb;
     }
   }
-}
-
-// ---- host-side launch helpers -----------------------------------------------------------------
-template <int H>
-struct SmemPlan {
-  int img1_off, xn_off, xn_ld, total_floats;
-};
-template <int H>
-SmemPlan<H> plan_smem(const DiscLaunch& L, bool) {
-  SmemPlan<H> s;
-  auto al = [](int x) { return (x + 31) / 32 * 32; };
-  int o = al(MlpSm<H>::size(L.pass[0].din));
-  s.img1_off = o;
-  if (L.npass == 3) o += al(MlpSm<H>::size(L.pass[1].din) + 2 * IMB_MAX_DIN);
-  int maxdin = 0;
-  for (int p = 0; p < L.npass; ++p) maxdin = L.pass[p].din > maxdin ? L.pass[p].din : maxdin;
-  s.xn_ld = maxdin | 1;
-  s.xn_off = o;
-  o += al(NT * s.xn_ld);
-  s.total_floats = o;
-  return s;
-}
-
-inline int pick_H(const DiscLaunch& L) {
-  int h = 0;
-  for (int p = 0; p < L.npass; ++p) {
-    if (L.pass[p].n_hidden >= 1 && L.pass[p].h1 > h) h = L.pass[p].h1;
-    if (L.pass[p].n_hidden >= 2 && L.pass[p].h2 > h) h = L.pass[p].h2;
-  }
-  return h <= 32 ? 32 : 64;
 }
 
 }  // namespace
@@ -1229,15 +1180,10 @@ static TPlan plan_tiled(const DiscLaunch& L, int R) {
   TPlan t;
   auto al = [](int x) { return (x + 31) / 32 * 32; };
   const int RS = R + TILE_PAD;
-  int h = 1, dmax = 1;
-  for (int p = 0; p < L.npass; ++p) {
-    if (L.pass[p].n_hidden >= 1 && L.pass[p].h1 > h) h = L.pass[p].h1;
-    if (L.pass[p].n_hidden >= 2 && L.pass[p].h2 > h) h = L.pass[p].h2;
-    if (L.pass[p].din > dmax) dmax = L.pass[p].din;
-  }
-  t.JP = h <= 32 ? 32 : 64;
-  t.KP = dmax <= 32 ? 32 : 64;
-  t.img_sz = al(TImg::size(dmax, t.JP));
+  const LaunchWidths lw = launch_widths(L);
+  t.JP = lw.JP;
+  t.KP = lw.dmax <= 32 ? 32 : 64;
+  t.img_sz = al(TImg::size(lw.dmax, t.JP));
   int o = L.npass * t.img_sz;
   t.nsl = (t.JP == 32 && R == 256) ? 4 : 2;  // row slices of the weight-gradient phase (>= 2: slice 1 holds dwf)
   t.aw_off = o;
@@ -1295,17 +1241,26 @@ static int fwdbwd_plan(const DiscLaunch& L, int64_t n, int flags, TPlan& t128, T
            "the limit is %d B", (size_t)t128.total * 4, IMB_SMEM_MAX);
 }
 
-// imb_reward_forward's kernel: hidden width H (32 or 64) and its dynamic shared memory
-template <int H>
-static size_t reward_fwd_bytes(const DiscLaunch& L) {
-  return (size_t)plan_smem<H>(L, false).total_floats * 4;
+// imb_reward_forward's shared memory (floats): one TImg per pass, img_sz apart, then xn_ld normalised inputs per thread
+struct FwdPlan {
+  LaunchWidths lw;
+  int img_sz, xn_ld, total;
+};
+static FwdPlan fwd_plan(const DiscLaunch& L) {
+  auto al = [](int x) { return (x + 31) / 32 * 32; };
+  FwdPlan f;
+  f.lw = launch_widths(L);
+  f.img_sz = al(TImg::size(f.lw.dmax, f.lw.JP));
+  f.xn_ld = f.lw.dmax | 1;
+  f.total = L.npass * f.img_sz + al(NT * f.xn_ld);
+  return f;
 }
 
 extern "C" int imb_disc_plan(const imb_disc_desc* d, int64_t n) {
   IMB_REQUIRE(n >= 1, "disc plan needs n >= 1");
   DiscLaunch L;
   if (int rc = build_launch(d, nullptr, nullptr, L)) return rc;
-  const size_t fb = pick_H(L) == 32 ? reward_fwd_bytes<32>(L) : reward_fwd_bytes<64>(L);
+  const size_t fb = (size_t)fwd_plan(L).total * 4;
   IMB_REQUIRE(fb <= IMB_SMEM_MAX, "reward net too large for the fused forward kernel: %zu B of shared memory, the "
               "limit is %d B", fb, IMB_SMEM_MAX);
   TPlan t128, t256;
@@ -1396,23 +1351,21 @@ extern "C" int imb_disc_reduce_adam(const imb_disc_desc* d, const imb_adam* opt,
   return 0;
 }
 
-template <int H>
-static int launch_fwd(const DiscLaunch& L, const float* params, const float* batch, int64_t ld, int64_t n,
-                      int out_mode, float* out, cudaStream_t st) {
-  const SmemPlan<H> s = plan_smem<H>(L, false);
-  const size_t bytes = (size_t)s.total_floats * 4;
+template <int JP>
+static int launch_fwd(const DiscLaunch& L, const FwdPlan& f, const float* params, const float* batch, int64_t ld,
+                      int64_t n, int out_mode, float* out, cudaStream_t st) {
+  const size_t bytes = (size_t)f.total * 4;
   IMB_REQUIRE(bytes <= IMB_SMEM_MAX, "reward net too large for the fused kernel (%zu B smem)", bytes);
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(k_reward_fwd<H>, cudaFuncAttributeMaxDynamicSharedMemorySize, IMB_SMEM_MAX);
+    cudaError_t e = cudaFuncSetAttribute(k_reward_fwd<JP>, cudaFuncAttributeMaxDynamicSharedMemorySize, IMB_SMEM_MAX);
     if (e != cudaSuccess) IMB_FAIL(-2, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
     attr_set = true;
   }
   int64_t blocks = (n + NT - 1) / NT;
   const int64_t cap = (int64_t)imb_num_sms() * 4;
   if (blocks > cap) blocks = cap;
-  k_reward_fwd<H><<<(int)blocks, NT, bytes, st>>>(L, params, batch, ld, n, out_mode, out, s.img1_off, s.xn_off,
-                                                   s.xn_ld);
+  k_reward_fwd<JP><<<(int)blocks, NT, bytes, st>>>(L, params, batch, ld, n, out_mode, out, f.img_sz, f.xn_ld);
   IMB_CHECK_LAUNCH("k_reward_fwd");
   return 0;
 }
@@ -1425,8 +1378,9 @@ extern "C" int imb_reward_forward(const imb_disc_desc* d, const float* params, c
   imb_disc_desc dd = *d;
   if (out_mode == 0) dd.subtract_logp = 0;
   if (int rc = build_launch(&dd, norm_state, nullptr, L)) return rc;
-  return (pick_H(L) == 32) ? launch_fwd<32>(L, params, batch, ld, n, out_mode, out, (cudaStream_t)stream)
-                           : launch_fwd<64>(L, params, batch, ld, n, out_mode, out, (cudaStream_t)stream);
+  const FwdPlan f = fwd_plan(L);
+  return (f.lw.JP == 32) ? launch_fwd<32>(L, f, params, batch, ld, n, out_mode, out, (cudaStream_t)stream)
+                         : launch_fwd<64>(L, f, params, batch, ld, n, out_mode, out, (cudaStream_t)stream);
 }
 
 template <bool EMA>

@@ -1,5 +1,5 @@
-// imb_mlp.cuh -- shared-memory MLP images and the per-row forward used by the discriminator
-// kernels (imb_disc.cu) and by the reward relabel inside the rollout kernel (imb_rollout.cu).
+// imb_mlp.cuh -- the reward net's launch descriptor (which batch rows each pass reads, and its network widths) used
+// by the discriminator kernels (imb_disc.cu) and by the reward relabel inside the rollout kernel (imb_rollout.cu).
 #pragma once
 #include "imb_common.cuh"
 
@@ -31,13 +31,20 @@ struct DiscLaunch {
   PassDesc pass[MAX_PASS];
 };
 
-__host__ __attribute__((unused)) inline int mlp_params(const imb_mlp& m) {
-  int hl = m.n_hidden == 0 ? m.din : (m.n_hidden == 1 ? m.h1 : m.h2);
-  int p = 0;
-  if (m.n_hidden >= 1) p += m.h1 * m.din + m.h1;
-  if (m.n_hidden >= 2) p += m.h2 * m.h1 + m.h2;
-  p += hl * m.n_out + m.n_out;
-  return p;
+// The widths every kernel sizes its network images by: JP, the hidden width padded to 32 or 64 columns (the widest
+// hidden layer over the launch's passes), and dmax, the widest pass input.
+struct LaunchWidths {
+  int JP, dmax;
+};
+inline LaunchWidths launch_widths(const DiscLaunch& L) {
+  int h = 0, dmax = 1;
+  for (int p = 0; p < L.npass; ++p) {
+    const PassDesc& q = L.pass[p];
+    if (q.n_hidden >= 1 && q.h1 > h) h = q.h1;
+    if (q.n_hidden >= 2 && q.h2 > h) h = q.h2;
+    if (q.din > dmax) dmax = q.din;
+  }
+  return {h <= 32 ? 32 : 64, dmax};
 }
 
 // Build the launch descriptor: which batch feature rows are staged and how each pass maps its
@@ -122,146 +129,9 @@ __host__ int build_launch(const imb_disc_desc* d, const float* norm_state, const
   return 0;
 }
 
-// ---- shared-memory image of one MLP -----------------------------------------------------------
-// W1t[k][j] (din x H, zero padded), b1[H], W2[j][i] and W2t[i][j] (H x H), b2[H], wf[H], bf.
-template <int H>
-struct MlpSm {
-  static constexpr int W1T = 0;
-  __host__ __device__ static constexpr int b1_off(int din) { return din * H; }
-  __host__ __device__ static constexpr int w2_off(int din) { return din * H + H; }
-  __host__ __device__ static constexpr int w2t_off(int din) { return din * H + H + H * H; }
-  __host__ __device__ static constexpr int b2_off(int din) { return din * H + H + 2 * H * H; }
-  __host__ __device__ static constexpr int wf_off(int din) { return din * H + 2 * H + 2 * H * H; }
-  __host__ __device__ static constexpr int mean_off(int din) { return din * H + 3 * H + 2 * H * H + 4; }
-  __host__ __device__ static constexpr int istd_off(int din) { return mean_off(din) + IMB_MAX_DIN; }
-  __host__ __device__ static constexpr int size(int din) { return istd_off(din) + IMB_MAX_DIN; }
-};
-
-// Load one MLP's parameters (torch layout) into its shared-memory image.  wf/bf: for n_hidden==0
-// the "final" weights act on the (normalised) inputs and are stored in the W1t column 0.
-template <int H>
-__device__ void load_mlp(float* sm, const PassDesc& p, const float* __restrict__ params) {
-  const int din = p.din;
-  const float* q = params + p.param_off;
-  const int tid = threadIdx.x, nt = blockDim.x;
-  float* W1t = sm;
-  float* b1 = sm + MlpSm<H>::b1_off(din);
-  float* W2 = sm + MlpSm<H>::w2_off(din);
-  float* W2t = sm + MlpSm<H>::w2t_off(din);
-  float* b2 = sm + MlpSm<H>::b2_off(din);
-  float* wf = sm + MlpSm<H>::wf_off(din);
-  for (int i = tid; i < MlpSm<H>::mean_off(din); i += nt) sm[i] = 0.f;
-  __syncthreads();
-  int off = 0;
-  int hl = din;
-  if (p.n_hidden >= 1) {
-    for (int i = tid; i < p.h1 * din; i += nt) {
-      int j = i / din, k = i - j * din;
-      W1t[k * H + j] = q[off + i];
-    }
-    off += p.h1 * din;
-    for (int i = tid; i < p.h1; i += nt) b1[i] = q[off + i];
-    off += p.h1;
-    hl = p.h1;
-  }
-  if (p.n_hidden >= 2) {
-    for (int i = tid; i < p.h2 * p.h1; i += nt) {
-      int j = i / p.h1, ii = i - j * p.h1;
-      float v = q[off + i];
-      W2[j * H + ii] = v;
-      W2t[ii * H + j] = v;
-    }
-    off += p.h2 * p.h1;
-    for (int i = tid; i < p.h2; i += nt) b2[i] = q[off + i];
-    off += p.h2;
-    hl = p.h2;
-  }
-  if (p.n_hidden == 0) {
-    for (int i = tid; i < din; i += nt) W1t[i * H] = q[off + i];  // column 0 holds wf over inputs
-  } else {
-    for (int i = tid; i < hl; i += nt) wf[i] = q[off + i];
-  }
-  off += hl;
-  if (tid == 0) wf[H] = q[off];  // bf
-  float* mean = sm + MlpSm<H>::mean_off(din);
-  float* istd = sm + MlpSm<H>::istd_off(din);
-  for (int i = tid; i < din; i += nt) {
-    if (p.has_norm) {
-      mean[i] = p.norm[i];
-      istd[i] = 1.0f / sqrtf(p.norm[din + i] + p.eps);
-    } else {
-      mean[i] = 0.f;
-      istd[i] = 1.f;
-    }
-  }
-}
-
-// Forward for one row held by this thread.  xn: this row's normalised inputs in shared memory
-// (stride 1).  KEEP: also return h1/h2 (post-ReLU) for the backward.
-template <int H, bool KEEP>
-__device__ __forceinline__ float mlp_forward_row(const float* __restrict__ sm, const PassDesc& p,
-                                                 const float* __restrict__ xn, float (&h1)[H], float (&h2)[H]) {
-  const int din = p.din;
-  const float* W1t = sm;
-  const float* wf = sm + MlpSm<H>::wf_off(din);
-  if (p.n_hidden == 0) {
-    float acc = wf[H];
-    for (int k = 0; k < din; ++k) acc = fmaf(W1t[k * H], xn[k], acc);
-    return acc;
-  }
-  const float* b1 = sm + MlpSm<H>::b1_off(din);
-#pragma unroll
-  for (int j = 0; j < H; ++j) h1[j] = b1[j];
-  for (int k = 0; k < din; ++k) {
-    const float xv = xn[k];
-    const float4* w = reinterpret_cast<const float4*>(W1t + k * H);
-#pragma unroll
-    for (int j4 = 0; j4 < H / 4; ++j4) {
-      const float4 ww = w[j4];
-      h1[4 * j4 + 0] = fmaf(ww.x, xv, h1[4 * j4 + 0]);
-      h1[4 * j4 + 1] = fmaf(ww.y, xv, h1[4 * j4 + 1]);
-      h1[4 * j4 + 2] = fmaf(ww.z, xv, h1[4 * j4 + 2]);
-      h1[4 * j4 + 3] = fmaf(ww.w, xv, h1[4 * j4 + 3]);
-    }
-  }
-#pragma unroll
-  for (int j = 0; j < H; ++j) h1[j] = fmaxf(h1[j], 0.f);
-  if (p.n_hidden == 1) {
-    float acc = wf[H];
-#pragma unroll
-    for (int j = 0; j < H; ++j) acc = fmaf(wf[j], h1[j], acc);
-    return acc;
-  }
-  const float* W2t = sm + MlpSm<H>::w2t_off(din);
-  const float* b2 = sm + MlpSm<H>::b2_off(din);
-#pragma unroll
-  for (int j = 0; j < H; ++j) h2[j] = b2[j];
-#pragma unroll
-  for (int i = 0; i < H; ++i) {
-    const float hv = h1[i];
-    const float4* w = reinterpret_cast<const float4*>(W2t + i * H);
-#pragma unroll
-    for (int j4 = 0; j4 < H / 4; ++j4) {
-      const float4 ww = w[j4];
-      h2[4 * j4 + 0] = fmaf(ww.x, hv, h2[4 * j4 + 0]);
-      h2[4 * j4 + 1] = fmaf(ww.y, hv, h2[4 * j4 + 1]);
-      h2[4 * j4 + 2] = fmaf(ww.z, hv, h2[4 * j4 + 2]);
-      h2[4 * j4 + 3] = fmaf(ww.w, hv, h2[4 * j4 + 3]);
-    }
-  }
-  float acc = wf[H];
-#pragma unroll
-  for (int j = 0; j < H; ++j) {
-    h2[j] = fmaxf(h2[j], 0.f);
-    acc = fmaf(wf[j], h2[j], acc);
-  }
-  return acc;
-}
-
 // coefficient of a pass's output in the logit: r + gamma*(1-done)*Phi(s') - Phi(s)
 __device__ __forceinline__ float pass_coef(int kind, float gamma, float done) {
   return kind == 0 ? 1.0f : (kind == 1 ? gamma * (1.0f - done) : -1.0f);
 }
-
 
 }  // namespace

@@ -972,32 +972,22 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
 }
 
 // ---- log pi(a|s) for the AIRL discriminator batch --------------------------------------------------------------
-// thread per batch column; obs rows [0,Do), act rows [Do, Do+Da_onehot) of the feature-major batch.
+// thread per batch column; obs rows [0,Do), act rows [Do, Do+Da_onehot) of the feature-major batch.  The pi tower, the
+// action head and log_std come from the policy's PolImg; then xn_ld >= Do inputs per thread.
 template <int HP>
 __global__ void __launch_bounds__(128) k_policy_logp(const imb_policy_desc pd, const float* __restrict__ params,
                                                     const float* __restrict__ norm, float* __restrict__ batch,
-                                                    int64_t ld, int64_t n, int row_logp, int w1t_off, int w2t_off,
-                                                    int xn_off, int xn_ld) {
+                                                    int64_t ld, int64_t n, int row_logp, int xn_off, int xn_ld) {
   extern __shared__ __align__(128) float smem[];
   const int Do = pd.d_obs, Da = pd.d_act, h = pd.hidden;
-  float* Pm = smem;
-  float* w1t = smem + w1t_off;
-  float* w2t = smem + w2t_off;
-  float* XNs = smem + xn_off;
+  const PolImg S(Do, Da, HP);
   const int tid = threadIdx.x;
-  for (int i = tid; i < pd.n_params; i += blockDim.x) Pm[i] = params[i];
-  for (int i = tid; i < Do * HP + HP * HP; i += blockDim.x) w1t[i] = 0.f;
+  load_policy_img(smem, S, pd, HP, params, norm);
   __syncthreads();
-  for (int i = tid; i < h * Do; i += blockDim.x) {
-    const int j = i / Do, k = i - j * Do;
-    w1t[k * HP + j] = Pm[pd.off_pi_w1 + i];
-  }
-  for (int i = tid; i < h * h; i += blockDim.x) {
-    const int j = i / h, ii = i - j * h;
-    w2t[ii * HP + j] = Pm[pd.off_pi_w2 + i];
-  }
-  __syncthreads();
-  float* x = XNs + tid * xn_ld;
+  const float* w1t = smem + S.w1p;
+  const float* w2t = smem + S.w2p;
+  const float* wa = smem + S.wa;
+  float* x = smem + xn_off + tid * xn_ld;
   for (int64_t col = (int64_t)blockIdx.x * blockDim.x + tid; col < n; col += (int64_t)gridDim.x * blockDim.x) {
     for (int k = 0; k < Do; ++k) {
       float v = batch[(int64_t)k * ld + col];
@@ -1006,7 +996,7 @@ __global__ void __launch_bounds__(128) k_policy_logp(const imb_policy_desc pd, c
     }
     float h1[HP], lat[HP];
 #pragma unroll
-    for (int j = 0; j < HP; ++j) h1[j] = (j < h) ? Pm[pd.off_pi_b1 + j] : 0.f;
+    for (int j = 0; j < HP; ++j) h1[j] = smem[S.b1p + j];
     for (int k = 0; k < Do; ++k) {
       const float xv = x[k];
 #pragma unroll
@@ -1015,7 +1005,7 @@ __global__ void __launch_bounds__(128) k_policy_logp(const imb_policy_desc pd, c
 #pragma unroll
     for (int j = 0; j < HP; ++j) {
       h1[j] = tanhf(h1[j]);
-      lat[j] = (j < h) ? Pm[pd.off_pi_b2 + j] : 0.f;
+      lat[j] = smem[S.b2p + j];
     }
 #pragma unroll
     for (int i = 0; i < HP; ++i) {
@@ -1028,10 +1018,10 @@ __global__ void __launch_bounds__(128) k_policy_logp(const imb_policy_desc pd, c
     float logp = 0.f;
     if (!pd.discrete) {
       for (int a = 0; a < Da; ++a) {
-        float m = Pm[pd.off_act_b + a];
+        float m = smem[S.ba + a];
 #pragma unroll
-        for (int j = 0; j < HP; ++j) m = (j < h) ? fmaf(Pm[pd.off_act_w + a * h + j], lat[j], m) : m;
-        const float ls = Pm[pd.off_log_std + a], sd = expf(ls);
+        for (int j = 0; j < HP; ++j) m = (j < h) ? fmaf(wa[a * HP + j], lat[j], m) : m;
+        const float ls = smem[S.lstd + a], sd = expf(ls);
         const float diff = batch[(int64_t)(Do + a) * ld + col] - m;
         logp += -(diff * diff) / (2.0f * sd * sd) - ls - 0.9189385332046727f;
       }
@@ -1039,9 +1029,9 @@ __global__ void __launch_bounds__(128) k_policy_logp(const imb_policy_desc pd, c
       float mx = -INFINITY, chosen = 0.f;
       float lg[IMB_MAX_DIN];
       for (int a = 0; a < Da; ++a) {
-        float m = Pm[pd.off_act_b + a];
+        float m = smem[S.ba + a];
 #pragma unroll
-        for (int j = 0; j < HP; ++j) m = (j < h) ? fmaf(Pm[pd.off_act_w + a * h + j], lat[j], m) : m;
+        for (int j = 0; j < HP; ++j) m = (j < h) ? fmaf(wa[a * HP + j], lat[j], m) : m;
         lg[a] = m;
         mx = fmaxf(mx, m);
         if (batch[(int64_t)(Do + a) * ld + col] > 0.5f) chosen = m;  // one-hot action rows
@@ -1215,27 +1205,19 @@ template <int HP>
 static int launch_logp(const imb_policy_desc* pol, const float* params, const float* norm, float* batch, int64_t ld,
                        int64_t n, int row_logp, cudaStream_t st) {
   auto al = [](int x) { return (x + 31) / 32 * 32; };
-  const int Do = pol->d_obs;
-  int o = al(pol->n_params);
-  const int w1t_off = o;
-  o += Do * HP;
-  const int w2t_off = o;
-  o += al(HP * HP);
-  const int xn_ld = Do | 1;
-  const int xn_off = al(o);
-  o = xn_off + al(128 * xn_ld);
-  const size_t bytes = (size_t)o * 4;
+  const int xn_off = al(PolImg(pol->d_obs, pol->d_act, HP).total), xn_ld = pol->d_obs | 1;
+  const size_t bytes = (size_t)(xn_off + al(128 * xn_ld)) * 4;
   IMB_REQUIRE(bytes <= IMB_SMEM_MAX, "policy too large");
   static bool attr_set = false;
   if (!attr_set) {
-    cudaFuncSetAttribute(k_policy_logp<HP>, cudaFuncAttributeMaxDynamicSharedMemorySize, IMB_SMEM_MAX);
+    cudaError_t e = cudaFuncSetAttribute(k_policy_logp<HP>, cudaFuncAttributeMaxDynamicSharedMemorySize, IMB_SMEM_MAX);
+    if (e != cudaSuccess) IMB_FAIL(-2, "cudaFuncSetAttribute(k_policy_logp): %s", cudaGetErrorString(e));
     attr_set = true;
   }
   int64_t blocks = (n + 127) / 128;
   const int64_t cap = (int64_t)imb_num_sms() * 2;
   if (blocks > cap) blocks = cap;
-  k_policy_logp<HP><<<(int)blocks, 128, bytes, st>>>(*pol, params, norm, batch, ld, n, row_logp, w1t_off, w2t_off,
-                                                      xn_off, xn_ld);
+  k_policy_logp<HP><<<(int)blocks, 128, bytes, st>>>(*pol, params, norm, batch, ld, n, row_logp, xn_off, xn_ld);
   IMB_CHECK_LAUNCH("k_policy_logp");
   return 0;
 }

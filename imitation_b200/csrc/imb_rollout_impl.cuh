@@ -55,71 +55,6 @@ struct RolloutMembers {
   float* raw;
 };
 
-// policy image (runtime tower width HP, zero padded):
-//   piW1t[Do][HP] pib1[HP] piW2t[HP][HP] pib2[HP] vfW1t vfb1 vfW2t vfb2 Wa[Da][HP] ba[64] wv[HP] bv[4] lstd[64] mean[64] istd[64]
-struct PolImg {
-  int w1p, b1p, w2p, b2p, w1v, b1v, w2v, b2v, wa, ba, wv, bv, lstd, mean, istd, total;
-  __host__ __device__ PolImg(int Do, int Da, int HP) {
-    int o = 0;
-    w1p = o; o += Do * HP;
-    b1p = o; o += HP;
-    w2p = o; o += HP * HP;
-    b2p = o; o += HP;
-    w1v = o; o += Do * HP;
-    b1v = o; o += HP;
-    w2v = o; o += HP * HP;
-    b2v = o; o += HP;
-    wa = o; o += Da * HP;
-    ba = o; o += 64;
-    wv = o; o += HP;
-    bv = o; o += 4;
-    lstd = o; o += 64;
-    mean = o; o += 64;
-    istd = o; o += 64;
-    total = o;
-  }
-};
-
-__device__ void load_policy_img(float* sm, const PolImg& S, const imb_policy_desc& pd, int HP,
-                                const float* __restrict__ q, const float* __restrict__ norm) {
-  const int tid = threadIdx.x, nt = blockDim.x;
-  const int Do = pd.d_obs, Da = pd.d_act, h = pd.hidden;
-  for (int i = tid; i < S.total; i += nt) sm[i] = 0.f;
-  __syncthreads();
-#pragma unroll 4
-  for (int i = tid; i < h * Do; i += nt) {
-    const int j = i / Do, k = i - j * Do;
-    sm[S.w1p + k * HP + j] = q[pd.off_pi_w1 + i];
-    sm[S.w1v + k * HP + j] = q[pd.off_vf_w1 + i];
-  }
-#pragma unroll 4
-  for (int i = tid; i < h * h; i += nt) {
-    const int j = i / h, ii = i - j * h;
-    sm[S.w2p + ii * HP + j] = q[pd.off_pi_w2 + i];
-    sm[S.w2v + ii * HP + j] = q[pd.off_vf_w2 + i];
-  }
-  for (int i = tid; i < h; i += nt) {
-    sm[S.b1p + i] = q[pd.off_pi_b1 + i];
-    sm[S.b2p + i] = q[pd.off_pi_b2 + i];
-    sm[S.b1v + i] = q[pd.off_vf_b1 + i];
-    sm[S.b2v + i] = q[pd.off_vf_b2 + i];
-    sm[S.wv + i] = q[pd.off_val_w + i];
-  }
-  for (int i = tid; i < Da * h; i += nt) {
-    const int a = i / h, ii = i - a * h;
-    sm[S.wa + a * HP + ii] = q[pd.off_act_w + i];
-  }
-  for (int i = tid; i < Da; i += nt) {
-    sm[S.ba + i] = q[pd.off_act_b + i];
-    if (!pd.discrete) sm[S.lstd + i] = q[pd.off_log_std + i];
-  }
-  if (tid == 0) sm[S.bv] = q[pd.off_val_b];
-  for (int i = tid; i < Do; i += nt) {
-    sm[S.mean + i] = pd.has_norm ? norm[i] : 0.f;
-    sm[S.istd + i] = pd.has_norm ? 1.0f / sqrtf(norm[Do + i] + pd.norm_eps) : 1.f;
-  }
-}
-
 // flattened (reference-order) index of local step t of env e; see file header
 __device__ __forceinline__ int64_t flat_index(int64_t e, int64_t t, int64_t E, int64_t T, int64_t t0, int64_t H) {
   const int64_t seg = (t0 + t) / H;
@@ -618,15 +553,9 @@ static int launch_rollout_t(RolloutArgs A, const DiscLaunch& L, const RolloutMem
   A.HP = A.pol.hidden <= 32 ? 32 : 64;
   A.IP = Do <= 32 ? 32 : 64;
   A.KU = Do + Da;
-  int jp = 32, dmax = Do;
-  if (A.reward_mode != 0) {
-    for (int p = 0; p < L.npass; ++p) {
-      if (L.pass[p].n_hidden >= 1 && L.pass[p].h1 > jp) jp = 64;
-      if (L.pass[p].n_hidden >= 2 && L.pass[p].h2 > jp) jp = 64;
-      if (L.pass[p].din > dmax) dmax = L.pass[p].din;
-    }
-  }
-  A.JP = jp;
+  const LaunchWidths lw = A.reward_mode != 0 ? launch_widths(L) : LaunchWidths{32, Do};
+  A.JP = lw.JP;
+  const int dmax = lw.dmax > Do ? lw.dmax : Do;
   const int wmax = A.HP > A.JP ? A.HP : A.JP;
   int o = 0;
   A.pol_off = o;

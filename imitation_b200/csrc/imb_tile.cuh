@@ -1,4 +1,5 @@
-// imb_tile.cuh -- shared-memory tiled fp32 GEMM building blocks for the small-MLP kernels.
+// imb_tile.cuh -- shared-memory tiled fp32 GEMM building blocks for the small-MLP kernels, and the shared-memory images
+// of the reward net (TImg) and the policy (PolImg) that every kernel evaluating them builds.
 //
 // Why: a thread-per-row MLP reads one broadcast weight per FMA from shared memory; the LSU
 // delivers 4 B/lane/cycle, i.e. one operand per lane per cycle per SM, while the FMA pipes want
@@ -170,6 +171,132 @@ __device__ void load_timg(float* sm, const PassDesc& p, int JP, const float* __r
   for (int i = tid; i < din; i += nt) {
     sm[TImg::mean(din, JP) + i] = norm ? norm[i] : 0.f;
     sm[TImg::istd(din, JP) + i] = norm ? 1.0f / sqrtf(norm[din + i] + eps) : 1.f;
+  }
+}
+
+// Forward of one row held by this thread through the TImg image `img` (hidden width JP): xn holds the row's
+// normalised inputs (stride 1); register accumulators, one broadcast weight per FMA.
+template <int JP>
+__device__ __forceinline__ float timg_forward_row(const float* __restrict__ img, const PassDesc& p,
+                                                  const float* __restrict__ xn) {
+  const int din = p.din;
+  const float* wf = img + TImg::wf(din, JP);
+  const float bf = img[TImg::bf(din, JP)];
+  if (p.n_hidden == 0) {
+    float acc = bf;
+    for (int k = 0; k < din; ++k) acc = fmaf(wf[k], xn[k], acc);
+    return acc;
+  }
+  const float* W1t = img + TImg::w1t(din, JP);
+  const float* b1 = img + TImg::b1(din, JP);
+  float h1[JP], h2[JP];
+#pragma unroll
+  for (int j = 0; j < JP; ++j) h1[j] = b1[j];
+  for (int k = 0; k < din; ++k) {
+    const float xv = xn[k];
+    const float4* w = reinterpret_cast<const float4*>(W1t + k * JP);
+#pragma unroll
+    for (int j4 = 0; j4 < JP / 4; ++j4) {
+      const float4 ww = w[j4];
+      h1[4 * j4 + 0] = fmaf(ww.x, xv, h1[4 * j4 + 0]);
+      h1[4 * j4 + 1] = fmaf(ww.y, xv, h1[4 * j4 + 1]);
+      h1[4 * j4 + 2] = fmaf(ww.z, xv, h1[4 * j4 + 2]);
+      h1[4 * j4 + 3] = fmaf(ww.w, xv, h1[4 * j4 + 3]);
+    }
+  }
+#pragma unroll
+  for (int j = 0; j < JP; ++j) h1[j] = fmaxf(h1[j], 0.f);
+  if (p.n_hidden == 1) {
+    float acc = bf;
+#pragma unroll
+    for (int j = 0; j < JP; ++j) acc = fmaf(wf[j], h1[j], acc);
+    return acc;
+  }
+  const float* W2t = img + TImg::w2t(din, JP);
+  const float* b2 = img + TImg::b2(din, JP);
+#pragma unroll
+  for (int j = 0; j < JP; ++j) h2[j] = b2[j];
+#pragma unroll
+  for (int i = 0; i < JP; ++i) {
+    const float hv = h1[i];
+    const float4* w = reinterpret_cast<const float4*>(W2t + i * JP);
+#pragma unroll
+    for (int j4 = 0; j4 < JP / 4; ++j4) {
+      const float4 ww = w[j4];
+      h2[4 * j4 + 0] = fmaf(ww.x, hv, h2[4 * j4 + 0]);
+      h2[4 * j4 + 1] = fmaf(ww.y, hv, h2[4 * j4 + 1]);
+      h2[4 * j4 + 2] = fmaf(ww.z, hv, h2[4 * j4 + 2]);
+      h2[4 * j4 + 3] = fmaf(ww.w, hv, h2[4 * j4 + 3]);
+    }
+  }
+  float acc = bf;
+#pragma unroll
+  for (int j = 0; j < JP; ++j) acc = fmaf(wf[j], fmaxf(h2[j], 0.f), acc);
+  return acc;
+}
+
+// Shared-memory image of the policy (SB3 ActorCriticPolicy, tower width padded to HP, everything zero padded):
+//   piW1t[Do][HP] pib1[HP] piW2t[HP][HP] pib2[HP] vfW1t vfb1 vfW2t vfb2 Wa[Da][HP] ba[64] wv[HP] bv[4] lstd[64] mean[64] istd[64]
+struct PolImg {
+  int w1p, b1p, w2p, b2p, w1v, b1v, w2v, b2v, wa, ba, wv, bv, lstd, mean, istd, total;
+  __host__ __device__ PolImg(int Do, int Da, int HP) {
+    int o = 0;
+    w1p = o; o += Do * HP;
+    b1p = o; o += HP;
+    w2p = o; o += HP * HP;
+    b2p = o; o += HP;
+    w1v = o; o += Do * HP;
+    b1v = o; o += HP;
+    w2v = o; o += HP * HP;
+    b2v = o; o += HP;
+    wa = o; o += Da * HP;
+    ba = o; o += 64;
+    wv = o; o += HP;
+    bv = o; o += 4;
+    lstd = o; o += 64;
+    mean = o; o += 64;
+    istd = o; o += 64;
+    total = o;
+  }
+};
+
+__device__ void load_policy_img(float* sm, const PolImg& S, const imb_policy_desc& pd, int HP,
+                                const float* __restrict__ q, const float* __restrict__ norm) {
+  const int tid = threadIdx.x, nt = blockDim.x;
+  const int Do = pd.d_obs, Da = pd.d_act, h = pd.hidden;
+  for (int i = tid; i < S.total; i += nt) sm[i] = 0.f;
+  __syncthreads();
+#pragma unroll 4
+  for (int i = tid; i < h * Do; i += nt) {
+    const int j = i / Do, k = i - j * Do;
+    sm[S.w1p + k * HP + j] = q[pd.off_pi_w1 + i];
+    sm[S.w1v + k * HP + j] = q[pd.off_vf_w1 + i];
+  }
+#pragma unroll 4
+  for (int i = tid; i < h * h; i += nt) {
+    const int j = i / h, ii = i - j * h;
+    sm[S.w2p + ii * HP + j] = q[pd.off_pi_w2 + i];
+    sm[S.w2v + ii * HP + j] = q[pd.off_vf_w2 + i];
+  }
+  for (int i = tid; i < h; i += nt) {
+    sm[S.b1p + i] = q[pd.off_pi_b1 + i];
+    sm[S.b2p + i] = q[pd.off_pi_b2 + i];
+    sm[S.b1v + i] = q[pd.off_vf_b1 + i];
+    sm[S.b2v + i] = q[pd.off_vf_b2 + i];
+    sm[S.wv + i] = q[pd.off_val_w + i];
+  }
+  for (int i = tid; i < Da * h; i += nt) {
+    const int a = i / h, ii = i - a * h;
+    sm[S.wa + a * HP + ii] = q[pd.off_act_w + i];
+  }
+  for (int i = tid; i < Da; i += nt) {
+    sm[S.ba + i] = q[pd.off_act_b + i];
+    if (!pd.discrete) sm[S.lstd + i] = q[pd.off_log_std + i];
+  }
+  if (tid == 0) sm[S.bv] = q[pd.off_val_b];
+  for (int i = tid; i < Do; i += nt) {
+    sm[S.mean + i] = pd.has_norm ? norm[i] : 0.f;
+    sm[S.istd + i] = pd.has_norm ? 1.0f / sqrtf(norm[Do + i] + pd.norm_eps) : 1.f;
   }
 }
 
