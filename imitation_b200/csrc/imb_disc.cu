@@ -10,13 +10,16 @@
 //   k_norm_stats   per-chunk (n, mean, M2) per input feature of 1-3 normaliser updates (blockIdx.y = job);
 //                  the last CTA Chan-merges each job's chunks in fixed order and folds the jobs, in order,
 //                  into their running stats (RunningNorm.update_stats).
-//   k_disc_fwdbwd  persistent CTAs over 128-row tiles of the feature-major batch.  The tile is
-//                  staged [feature][row] into shared memory by cp.async.bulk (TMA unit) with a
-//                  2-stage mbarrier pipeline.  Phase A (thread per row): normalise, MLP forward,
-//                  BCE-with-logits, backward to dL/dz per layer, activations to smem tiles.
-//                  Phase B (warps split output columns): the three weight-gradient contractions
-//                  dW = D^T . Act over the tile, accumulated in shared memory across tiles.
-//                  Weights (<34 KB) stay in shared memory; activations never touch HBM.
+//   k_disc_fwdbwd<R>  the fp32-FFMA form (k_disc_fwdbwd_tc in imb_disc_tc.cuh is the tensor-core one):
+//                  persistent CTAs of R threads over R-row tiles (R = 128 or 256) of the feature-major batch.  A
+//                  tile's feature rows arrive in shared memory by cp.async.bulk on an mbarrier; the next tile's
+//                  copy is issued once the last forward that reads them is done.  Per pass, the inputs are
+//                  normalised into a feature-major tile and the hidden layers run as register-tiled GEMMs
+//                  (tile_layer, imb_tile.cuh); the head's dot product gives each row's logit.  Per row:
+//                  BCE-with-logits (or the caller's dL/dlogit) and the statistics.  Backward, last pass first
+//                  (earlier passes are recomputed): dL/dz1 by gemm_acc, then the weight-gradient contractions
+//                  dW = D^T . Act (wgrad_tile) into per-slice shared-memory accumulators that leave the CTA as
+//                  one partial vector.  Weights stay in shared memory; activations never touch HBM.
 //   k_disc_reduce  warp-per-parameter deterministic sum of the per-CTA partials (G = meta[0], written by
 //                  the fwd/bwd kernel).
 //   k_disc_adam    torch.optim.Adam step + the 9 train statistics.
@@ -192,6 +195,47 @@ __global__ void k_norm_fold(int din, float* __restrict__ defer, float* __restric
 }
 
 // ---- the fused forward / BCE / backward kernel (tiled-GEMM form, see imb_tile.cuh) ------------------
+// One weight-gradient contraction over the R-row tile, by the `gthreads` threads of a contraction group (tgw = this
+// thread's index in it):  dW[j][i] += sum_r D[j][r] * ACT[i][r],  db[j] += sum_r D[j][r]  for j < nj, i < ni, into
+// the parameter vector's [off_w, off_w + nj * ni) and [off_b, off_b + nj).  The (JP / 32) x (IP / 32) blocks of 32 x 32
+// take a warp each (wgrad_acc); when the group has threads to spare, the tile's rows are split into slices whose
+// accumulators are private (slice s at AW + s * P).  MASK: D = dL/dz2 generated from H2 and the upstream g as in
+// wgrad_acc, with per-j scale wf.
+template <int R, bool MASK>
+__device__ __forceinline__ void wgrad_tile(float* AW, int P, int nsl, int tgw, int gthreads, int JP, int IP,
+                                           const float* D, const float* ACT, const float* g, const float* wf, int nj,
+                                           int ni, int off_w, int off_b) {
+  constexpr int RS = R + TILE_PAD;
+  const int lane = threadIdx.x & 31, jl = lane & 7, il = lane >> 3;
+  const int nblk = (JP / 32) * (IP / 32), ntl = nblk * 32;
+  const int slices = min(gthreads / ntl, nsl);
+  const int lt = tgw % ntl, sl = tgw / ntl, blk = lt >> 5;
+  const int jb = (blk % (JP / 32)) * 32, ib = (blk / (JP / 32)) * 32;
+  float acc[4][8], bacc[4], sj[4];
+#pragma unroll
+  for (int jj = 0; jj < 4; ++jj) {
+    bacc[jj] = 0.f;
+    sj[jj] = MASK ? wf[jb + jl + 8 * jj] : 0.f;
+#pragma unroll
+    for (int ii = 0; ii < 8; ++ii) acc[jj][ii] = 0.f;
+  }
+  const int rows = R / slices;
+  if (sl < slices) wgrad_acc<MASK>(acc, bacc, D, ACT, RS, jb + jl, ib + il, sl * rows, (sl + 1) * rows, g, sj);
+  float* A = AW + (sl < slices ? sl : 0) * P;
+#pragma unroll
+  for (int jj = 0; jj < 4; ++jj) {
+    const int j = jb + jl + 8 * jj;
+    if (j < nj) {
+#pragma unroll
+      for (int ii = 0; ii < 8; ++ii) {
+        const int i = ib + il + 4 * ii;
+        if (i < ni) A[off_w + j * ni + i] += acc[jj][ii];
+      }
+      if (il == 0 && ib == 0) A[off_b + j] += bacc[jj];
+    }
+  }
+}
+
 // Dynamic shared memory (floats):
 //   [image per pass][AW: 4 slices x P][stage: nstage x RS][XN: KP x RS][H1, H2, DZ1: JP x RS each]
 //   [lg, gv, gp, dv, lpv: R each]
@@ -204,8 +248,6 @@ __global__ void __launch_bounds__(R, 256 / R) k_disc_fwdbwd(const DiscLaunch L, 
                                                       int* __restrict__ meta, int JP, int KP, int img_sz, int aw_off, int st_off, int xn_off,
                                                       int t_off, int v_off, int nsl) {
   // one thread per tile row: R threads, warp w -> column group w % 4 (8 columns) and row half w / 4
-  constexpr int NQ = 1;
-  constexpr int NTK = R;
   constexpr int RS = R + TILE_PAD;
   extern __shared__ __align__(128) float smem[];
   __shared__ __align__(8) uint64_t bar;
@@ -227,7 +269,7 @@ __global__ void __launch_bounds__(R, 256 / R) k_disc_fwdbwd(const DiscLaunch L, 
 
   for (int p = 0; p < L.npass; ++p)
     load_timg(smem + p * img_sz, L.pass[p], JP, params, L.pass[p].has_norm ? L.pass[p].norm : nullptr, L.pass[p].eps);
-  for (int i = tid; i < nsl * P; i += NTK) AW[i] = 0.f;
+  for (int i = tid; i < nsl * P; i += R) AW[i] = 0.f;
   if (tid == 0) {
     mbar_init(&bar, 1);
     mbar_fence_init();
@@ -251,8 +293,7 @@ __global__ void __launch_bounds__(R, 256 / R) k_disc_fwdbwd(const DiscLaunch L, 
   uint32_t phase = 0;
   if (tid == 0 && (int64_t)blockIdx.x < ntiles) issue(blockIdx.x);
 
-  int rq[NQ];
-  rq[0] = grp * 128 + lane * 4;
+  const int r0 = grp * 128 + lane * 4;  // this thread's row quad in the register-tiled GEMMs
   const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
   float s_loss = 0.f, s_ent = 0.f;
   int c_exp = 0, c_gen = 0, c_pred_exp = 0;
@@ -266,7 +307,7 @@ __global__ void __launch_bounds__(R, 256 / R) k_disc_fwdbwd(const DiscLaunch L, 
     const float* mean = img + TImg::mean(din, JP);
     const float* istd = img + TImg::istd(din, JP);
     // normalised inputs, feature-major; rows >= nv and features >= din are zero
-    for (int i = tid; i < KP * (R / 4); i += NTK) {
+    for (int i = tid; i < KP * (R / 4); i += R) {
       const int k = i / (R / 4), r4 = (i - k * (R / 4)) * 4;
       float4 v = zero4;
       if (k < din) {
@@ -282,53 +323,14 @@ __global__ void __launch_bounds__(R, 256 / R) k_disc_fwdbwd(const DiscLaunch L, 
     __syncthreads();
     const float* HL = XN;
     int hl = din;
-    float4 gq[NQ];
-#pragma unroll
-    for (int q = 0; q < NQ; ++q) gq[q] = zero4;
     if (Pd.n_hidden >= 1) {
-      for (int jh = 0; jh < JP / 32; ++jh) {
-        const int j0 = jh * 32 + cg * 8;
-        float acc[NQ * 4][8];
-#pragma unroll
-        for (int a = 0; a < NQ * 4; ++a)
-#pragma unroll
-          for (int t = 0; t < 8; ++t) acc[a][t] = 0.f;
-        gemm_acc<NQ, false>(acc, XN, RS, rq, img + TImg::w1t(din, JP), JP, j0, din, gq, nullptr);
-        const float* b1 = img + TImg::b1(din, JP);
-#pragma unroll
-        for (int t = 0; t < 8; ++t) {
-          const float b = b1[j0 + t];
-#pragma unroll
-          for (int q = 0; q < NQ; ++q)
-            st4(H1 + (j0 + t) * RS + rq[q],
-                make_float4(fmaxf(acc[q * 4 + 0][t] + b, 0.f), fmaxf(acc[q * 4 + 1][t] + b, 0.f),
-                            fmaxf(acc[q * 4 + 2][t] + b, 0.f), fmaxf(acc[q * 4 + 3][t] + b, 0.f)));
-        }
-      }
+      tile_layer<ACT_RELU, 4, R>(XN, din, img + TImg::w1t(din, JP), JP, img + TImg::b1(din, JP), H1, JP);
       __syncthreads();
       HL = H1;
       hl = Pd.h1;
     }
     if (Pd.n_hidden >= 2) {
-      for (int jh = 0; jh < JP / 32; ++jh) {
-        const int j0 = jh * 32 + cg * 8;
-        float acc[NQ * 4][8];
-#pragma unroll
-        for (int a = 0; a < NQ * 4; ++a)
-#pragma unroll
-          for (int t = 0; t < 8; ++t) acc[a][t] = 0.f;
-        gemm_acc<NQ, false>(acc, H1, RS, rq, img + TImg::w2t(din, JP), JP, j0, Pd.h1, gq, nullptr);
-        const float* b2 = img + TImg::b2(din, JP);
-#pragma unroll
-        for (int t = 0; t < 8; ++t) {
-          const float b = b2[j0 + t];
-#pragma unroll
-          for (int q = 0; q < NQ; ++q)
-            st4(H2 + (j0 + t) * RS + rq[q],
-                make_float4(fmaxf(acc[q * 4 + 0][t] + b, 0.f), fmaxf(acc[q * 4 + 1][t] + b, 0.f),
-                            fmaxf(acc[q * 4 + 2][t] + b, 0.f), fmaxf(acc[q * 4 + 3][t] + b, 0.f)));
-        }
-      }
+      tile_layer<ACT_RELU, 4, R>(H1, Pd.h1, img + TImg::w2t(din, JP), JP, img + TImg::b2(din, JP), H2, JP);
       __syncthreads();
       HL = H2;
       hl = Pd.h2;
@@ -336,7 +338,7 @@ __global__ void __launch_bounds__(R, 256 / R) k_disc_fwdbwd(const DiscLaunch L, 
     if (accumulate) {
       const float* wf = img + TImg::wf(din, JP);
       const float bf = img[TImg::bf(din, JP)];
-      for (int r = tid; r < R; r += NTK) {
+      for (int r = tid; r < R; r += R) {
         float o = bf;
         for (int j = 0; j < hl; ++j) o = fmaf(wf[j], HL[j * RS + r], o);
         const float c = pass_coef(Pd.coef_kind, L.gamma, dv[r]);
@@ -350,7 +352,7 @@ __global__ void __launch_bounds__(R, 256 / R) k_disc_fwdbwd(const DiscLaunch L, 
     mbar_wait(&bar, phase);
     phase ^= 1u;
     const int nv = (int)min((int64_t)R, n - tile * R);
-    for (int r = tid; r < R; r += NTK) {
+    for (int r = tid; r < R; r += R) {
       dv[r] = (L.done_slot >= 0 && r < nv) ? xs[L.done_slot * RS + r] : 0.f;
       lpv[r] = (L.logp_slot >= 0 && r < nv) ? xs[L.logp_slot * RS + r] : 0.f;
     }
@@ -362,7 +364,7 @@ __global__ void __launch_bounds__(R, 256 / R) k_disc_fwdbwd(const DiscLaunch L, 
     const int64_t next = tile + gridDim.x;
     if (!recompute && tid == 0 && next < ntiles) issue(next);
     // ---- dL/dlogit per row + statistics -------------------------------------------------------------
-    for (int r = tid; r < R; r += NTK) {
+    for (int r = tid; r < R; r += R) {
       float g = 0.f;
       if (r < nv) {
         const int64_t row = tile * R + r;
@@ -395,9 +397,8 @@ __global__ void __launch_bounds__(R, 256 / R) k_disc_fwdbwd(const DiscLaunch L, 
       const float* img = smem + p * img_sz;
       const int din = Pd.din;
       const float* wf = img + TImg::wf(din, JP);
-      for (int r = tid; r < R; r += NTK) gp[r] = gv[r] * pass_coef(Pd.coef_kind, L.gamma, dv[r]);
+      for (int r = tid; r < R; r += R) gp[r] = gv[r] * pass_coef(Pd.coef_kind, L.gamma, dv[r]);
       __syncthreads();
-      float* A0 = AW;  // slice 0 accumulators
       const int h1w = Pd.h1, h2w = Pd.h2;
       const int off_w1 = Pd.param_off, off_b1 = off_w1 + h1w * din, off_w2 = off_b1 + h1w;
       const int off_b2 = off_w2 + ((Pd.n_hidden == 2) ? h2w * h1w : 0);
@@ -406,29 +407,24 @@ __global__ void __launch_bounds__(R, 256 / R) k_disc_fwdbwd(const DiscLaunch L, 
       const float* HL = (Pd.n_hidden == 2) ? H2 : (Pd.n_hidden == 1 ? H1 : XN);
       // dL/dz1 tile
       if (Pd.n_hidden == 2) {
-        float4 gq[NQ];
-#pragma unroll
-        for (int q = 0; q < NQ; ++q) gq[q] = ld4(gp + rq[q]);
+        const float4 g = ld4(gp + r0);
         for (int jh = 0; jh < JP / 32; ++jh) {
           const int i0 = jh * 32 + cg * 8;
-          float acc[NQ * 4][8];
+          float acc[4][8];
 #pragma unroll
-          for (int a = 0; a < NQ * 4; ++a)
+          for (int x = 0; x < 4; ++x)
 #pragma unroll
-            for (int t = 0; t < 8; ++t) acc[a][t] = 0.f;
-          gemm_acc<NQ, true>(acc, H2, RS, rq, img + TImg::w2(din, JP), JP, i0, h2w, gq, wf);
+            for (int t = 0; t < 8; ++t) acc[x][t] = 0.f;
+          gemm_acc(acc, H2, RS, r0, img + TImg::w2(din, JP), JP, i0, h2w, g, wf);
 #pragma unroll
-          for (int t = 0; t < 8; ++t)
-#pragma unroll
-            for (int q = 0; q < NQ; ++q) {
-              const float4 h = ld4(H1 + (i0 + t) * RS + rq[q]);
-              st4(DZ1 + (i0 + t) * RS + rq[q],
-                  make_float4(h.x > 0.f ? acc[q * 4 + 0][t] : 0.f, h.y > 0.f ? acc[q * 4 + 1][t] : 0.f,
-                              h.z > 0.f ? acc[q * 4 + 2][t] : 0.f, h.w > 0.f ? acc[q * 4 + 3][t] : 0.f));
-            }
+          for (int t = 0; t < 8; ++t) {
+            const float4 h = ld4(H1 + (i0 + t) * RS + r0);
+            st4(DZ1 + (i0 + t) * RS + r0, make_float4(h.x > 0.f ? acc[0][t] : 0.f, h.y > 0.f ? acc[1][t] : 0.f,
+                                                      h.z > 0.f ? acc[2][t] : 0.f, h.w > 0.f ? acc[3][t] : 0.f));
+          }
         }
       } else if (Pd.n_hidden == 1) {
-        for (int i = tid; i < JP * (R / 4); i += NTK) {
+        for (int i = tid; i < JP * (R / 4); i += R) {
           const int j = i / (R / 4), r4 = (i - j * (R / 4)) * 4;
           const float4 h = ld4(H1 + j * RS + r4), g = ld4(gp + r4);
           const float w = wf[j];
@@ -437,7 +433,6 @@ __global__ void __launch_bounds__(R, 256 / R) k_disc_fwdbwd(const DiscLaunch L, 
         }
       }
       __syncthreads();
-      const int jl = lane & 7, il = lane >> 3;
       // weight gradients: a group of 4 warps (128 threads) per contraction; with two groups (R = 256)
       // dW2 and dW1 run concurrently, each split into row slices with private accumulators.
       constexpr int NGRP = R / 128;
@@ -449,70 +444,12 @@ __global__ void __launch_bounds__(R, 256 / R) k_disc_fwdbwd(const DiscLaunch L, 
       const int gthreads = split64 ? 64 : 128;
       const bool do_w2 = Pd.n_hidden == 2 && ((NGRP == 1 && !split64) || wg == 0);
       const bool do_w1 = Pd.n_hidden >= 1 && ((NGRP == 1 && !split64) || wg == (Pd.n_hidden == 2 ? 1 : 0));
-      if (do_w2) {
-        const int nblk = (JP / 32) * (JP / 32), ntl = nblk * 32;
-        const int slices = min(gthreads / ntl, nsl);
-        const int lt = tgw % ntl, sl = tgw / ntl, blk = lt >> 5;
-        const int jb = (blk % (JP / 32)) * 32, ib = (blk / (JP / 32)) * 32;
-        float acc[4][8], bacc[4], sj[4];
-#pragma unroll
-        for (int jj = 0; jj < 4; ++jj) {
-          bacc[jj] = 0.f;
-          sj[jj] = wf[jb + jl + 8 * jj];
-#pragma unroll
-          for (int ii = 0; ii < 8; ++ii) acc[jj][ii] = 0.f;
-        }
-        const int rows = R / slices;
-        if (sl < slices)
-          wgrad_acc<true>(acc, bacc, H2, H1, RS, jb + jl, ib + il, sl * rows, (sl + 1) * rows, gp, sj);
-        float* A = A0 + (sl < slices ? sl : 0) * P;
-#pragma unroll
-        for (int jj = 0; jj < 4; ++jj) {
-          const int j = jb + jl + 8 * jj;
-          if (j < h2w) {
-#pragma unroll
-            for (int ii = 0; ii < 8; ++ii) {
-              const int i = ib + il + 4 * ii;
-              if (i < h1w) A[off_w2 + j * h1w + i] += acc[jj][ii];
-            }
-            if (il == 0 && ib == 0) A[off_b2 + j] += bacc[jj];
-          }
-        }
-      }
-      if (do_w1) {
-        const int nblk = (JP / 32) * (KP / 32), ntl = nblk * 32;
-        const int slices = min(gthreads / ntl, nsl);
-        const int lt = tgw % ntl, sl = tgw / ntl, blk = lt >> 5;
-        const int jb = (blk % (JP / 32)) * 32, ib = (blk / (JP / 32)) * 32;
-        float acc[4][8], bacc[4];
-        const float sj[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-        for (int jj = 0; jj < 4; ++jj) {
-          bacc[jj] = 0.f;
-#pragma unroll
-          for (int ii = 0; ii < 8; ++ii) acc[jj][ii] = 0.f;
-        }
-        const int rows = R / slices;
-        if (sl < slices)
-          wgrad_acc<false>(acc, bacc, DZ1, XN, RS, jb + jl, ib + il, sl * rows, (sl + 1) * rows, nullptr, sj);
-        float* A = A0 + (sl < slices ? sl : 0) * P;
-#pragma unroll
-        for (int jj = 0; jj < 4; ++jj) {
-          const int j = jb + jl + 8 * jj;
-          if (j < h1w) {
-#pragma unroll
-            for (int ii = 0; ii < 8; ++ii) {
-              const int kk = ib + il + 4 * ii;
-              if (kk < din) A[off_w1 + j * din + kk] += acc[jj][ii];
-            }
-            if (il == 0 && ib == 0) A[off_b1 + j] += bacc[jj];
-          }
-        }
-      }
+      if (do_w2) wgrad_tile<R, true>(AW, P, nsl, tgw, gthreads, JP, JP, H2, H1, gp, wf, h2w, h1w, off_w2, off_b2);
+      if (do_w1) wgrad_tile<R, false>(AW, P, nsl, tgw, gthreads, JP, KP, DZ1, XN, nullptr, nullptr, h1w, din, off_w1, off_b1);
       // dwf / dbf: thread j sums its feature row against gp (slice 1 accumulators keep owners unique)
       {
-        float* A = A0 + 1 * P;
-        for (int j = tid; j <= hl; j += NTK) {
+        float* A = AW + 1 * P;
+        for (int j = tid; j <= hl; j += R) {
           float acc = 0.f;
           if (j < hl) {
             for (int r = 0; r < R; r += 4) {
@@ -537,7 +474,7 @@ __global__ void __launch_bounds__(R, 256 / R) k_disc_fwdbwd(const DiscLaunch L, 
 
   // ---- per-CTA partials: gradients (slices summed in fixed order) + statistics ----------------------
   float* my = partial + (int64_t)blockIdx.x * part_stride(P);
-  for (int i = tid; i < P; i += NTK) {
+  for (int i = tid; i < P; i += R) {
     float v = AW[i];
     for (int s2 = 1; s2 < nsl; ++s2) v += AW[s2 * P + i];
     my[i] = v;
@@ -557,7 +494,7 @@ __global__ void __launch_bounds__(R, 256 / R) k_disc_fwdbwd(const DiscLaunch L, 
   __syncthreads();
   if (tid < 5) {
     float v = 0.f;
-    for (int w = 0; w < NTK / 32; ++w) v += red[w * 5 + tid];
+    for (int w = 0; w < R / 32; ++w) v += red[w * 5 + tid];
     my[P + tid] = v;
   }
 }

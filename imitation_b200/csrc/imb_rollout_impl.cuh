@@ -64,95 +64,6 @@ __device__ __forceinline__ int64_t flat_index(int64_t e, int64_t t, int64_t E, i
   return E * start + e * (end - start) + (t - start);
 }
 
-enum { ACT_TANH = 0, ACT_RELU = 1 };
-
-// OUT[j][r] = act(bias[j] + sum_k A[k][r] * Wk[k][j]) for j < JPx (multiple of 32); 128 threads:
-// warp -> 8-column group, lane -> RPL consecutive rows.
-// rows per tile for a rows-per-lane parameter (RPL = 0: the 8-row tile, lane = (row, column pair))
-__host__ __device__ constexpr int rows_of(int rpl) { return rpl == 0 ? 8 : 32 * rpl; }
-
-// 8-row tile: warp -> 8-column group, lane -> (row = lane % 8, columns 2 * (lane / 8), +1): two FMAs per input and
-// lane, so a layer's latency is ~K x 10 cycles and the grid covers all SMs at 1024 envs (128 CTAs)
-template <int ACT>
-__device__ __forceinline__ void tile_layer8(const float* __restrict__ A, int K, const float* __restrict__ Wk, int wld,
-                                            const float* __restrict__ bias, float* __restrict__ OUT, int JPx) {
-  constexpr int RRS = 8 + TILE_PAD;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int r = lane & 7, c2 = 2 * (lane >> 3);
-  for (int jh = 0; jh < JPx / 32; ++jh) {
-    const int j0 = jh * 32 + warp * 8 + c2;
-    float a0 = 0.f, a1 = 0.f, b0 = 0.f, b1 = 0.f;  // two accumulator pairs (even / odd k)
-    int k = 0;
-#pragma unroll 4
-    for (; k + 2 <= K; k += 2) {
-      const float x0 = A[k * RRS + r], x1 = A[(k + 1) * RRS + r];
-      const float2 w0 = *reinterpret_cast<const float2*>(Wk + k * wld + j0);
-      const float2 w1 = *reinterpret_cast<const float2*>(Wk + (k + 1) * wld + j0);
-      a0 = fmaf(x0, w0.x, a0);
-      a1 = fmaf(x0, w0.y, a1);
-      b0 = fmaf(x1, w1.x, b0);
-      b1 = fmaf(x1, w1.y, b1);
-    }
-    if (k < K) {
-      const float x0 = A[k * RRS + r];
-      const float2 w0 = *reinterpret_cast<const float2*>(Wk + k * wld + j0);
-      a0 = fmaf(x0, w0.x, a0);
-      a1 = fmaf(x0, w0.y, a1);
-    }
-    const float z0 = (a0 + b0) + bias[j0], z1 = (a1 + b1) + bias[j0 + 1];
-    OUT[j0 * RRS + r] = ACT == ACT_TANH ? tanh_fast(z0) : fmaxf(z0, 0.f);
-    OUT[(j0 + 1) * RRS + r] = ACT == ACT_TANH ? tanh_fast(z1) : fmaxf(z1, 0.f);
-  }
-}
-
-template <int ACT, int RPL>
-__device__ __forceinline__ void tile_layer(const float* __restrict__ A, int K, const float* __restrict__ Wk, int wld,
-                                           const float* __restrict__ bias, float* __restrict__ OUT, int JPx) {
-  if (RPL == 0) {
-    tile_layer8<ACT>(A, K, Wk, wld, bias, OUT, JPx);
-    return;
-  }
-  constexpr int RRS = 32 * RPL + TILE_PAD;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int r0 = lane * RPL;
-  for (int jh = 0; jh < JPx / 32; ++jh) {
-    const int j0 = jh * 32 + warp * 8;
-    float acc[RPL > 0 ? RPL : 1][8];
-#pragma unroll
-    for (int a = 0; a < RPL; ++a)
-#pragma unroll
-      for (int t = 0; t < 8; ++t) acc[a][t] = 0.f;
-#pragma unroll 4
-    for (int k = 0; k < K; ++k) {
-      float av[RPL > 0 ? RPL : 1];
-      if (RPL == 4) {
-        const float4 a4 = ld4(A + k * RRS + r0);
-        av[0] = a4.x, av[RPL > 1 ? 1 : 0] = a4.y, av[RPL > 2 ? 2 : 0] = a4.z, av[RPL > 3 ? 3 : 0] = a4.w;
-      } else if (RPL == 2) {
-        const float2 a2 = *reinterpret_cast<const float2*>(A + k * RRS + r0);
-        av[0] = a2.x, av[RPL > 1 ? 1 : 0] = a2.y;
-      } else {
-        av[0] = A[k * RRS + r0];
-      }
-      const float4 w0 = ld4(Wk + k * wld + j0), w1 = ld4(Wk + k * wld + j0 + 4);
-      const float w[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
-#pragma unroll
-      for (int x = 0; x < RPL; ++x)
-#pragma unroll
-        for (int t = 0; t < 8; ++t) acc[x][t] = fmaf(av[x], w[t], acc[x][t]);
-    }
-#pragma unroll
-    for (int t = 0; t < 8; ++t) {
-      const float b = bias[j0 + t];
-#pragma unroll
-      for (int x = 0; x < RPL; ++x) {
-        const float z = acc[x][t] + b;
-        OUT[(j0 + t) * RRS + r0 + x] = ACT == ACT_TANH ? tanh_fast(z) : fmaxf(z, 0.f);
-      }
-    }
-  }
-}
-
 // ENS: evaluate the Mb.M ensemble members (raw outputs to Mb.raw) instead of the one net at disc_params (reward to the
 // table's reward column); the single-net variant is compiled without the member loop.
 template <int RPL, bool ENS>

@@ -22,55 +22,122 @@ constexpr int TILE_PAD = 4;
 __device__ __forceinline__ float4 ld4(const float* p) { return *reinterpret_cast<const float4*>(p); }
 __device__ __forceinline__ void st4(float* p, const float4& v) { *reinterpret_cast<float4*>(p) = v; }
 
-// acc[NQ*4][8] += sum_k A[k][rq[q]+0..3] * Wk[k * wld + j0 + 0..7]
-//   A: feature-major tile (row stride RS); Wk: k-major weights (row stride wld, 16-byte aligned).
-// MASK: the A operand is generated on the fly as  (S[k][r] > 0) ? gq[r] * sk[k] : 0
-//   (dL/dz of a ReLU layer: S = post-activation tile, gq = upstream scalar per row, sk = per-k scale).
-template <int NQ, bool MASK>
-__device__ __forceinline__ void gemm_acc(float (&acc)[NQ * 4][8], const float* __restrict__ A, int RS,
-                                         const int (&rq)[NQ], const float* __restrict__ Wk, int wld, int j0,
-                                         int K, const float4 (&gq)[NQ], const float* __restrict__ sk) {
-#pragma unroll 2
-  for (int k = 0; k < K; ++k) {
-    float4 a[NQ];
-#pragma unroll
-    for (int q = 0; q < NQ; ++q) a[q] = ld4(A + k * RS + rq[q]);
-    if (MASK) {
-      const float s = sk[k];
-#pragma unroll
-      for (int q = 0; q < NQ; ++q) {
-        a[q].x = a[q].x > 0.f ? gq[q].x * s : 0.f;
-        a[q].y = a[q].y > 0.f ? gq[q].y * s : 0.f;
-        a[q].z = a[q].z > 0.f ? gq[q].z * s : 0.f;
-        a[q].w = a[q].w > 0.f ? gq[q].w * s : 0.f;
-      }
+enum { ACT_TANH = 0, ACT_RELU = 1 };
+
+// rows per tile for a rows-per-lane parameter (RPL = 0: the 8-row tile, lane = (row, column pair))
+__host__ __device__ constexpr int rows_of(int rpl) { return rpl == 0 ? 8 : 32 * rpl; }
+
+// 8-row tile: warp -> 8-column group, lane -> (row = lane % 8, columns 2 * (lane / 8), +1): two FMAs per input and
+// lane, so a layer's latency is ~K x 10 cycles and the grid covers all SMs at 1024 envs (128 CTAs)
+template <int ACT>
+__device__ __forceinline__ void tile_layer8(const float* __restrict__ A, int K, const float* __restrict__ Wk, int wld,
+                                            const float* __restrict__ bias, float* __restrict__ OUT, int JPx) {
+  constexpr int RRS = 8 + TILE_PAD;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int r = lane & 7, c2 = 2 * (lane >> 3);
+  for (int jh = 0; jh < JPx / 32; ++jh) {
+    const int j0 = jh * 32 + warp * 8 + c2;
+    float a0 = 0.f, a1 = 0.f, b0 = 0.f, b1 = 0.f;  // two accumulator pairs (even / odd k)
+    int k = 0;
+#pragma unroll 4
+    for (; k + 2 <= K; k += 2) {
+      const float x0 = A[k * RRS + r], x1 = A[(k + 1) * RRS + r];
+      const float2 w0 = *reinterpret_cast<const float2*>(Wk + k * wld + j0);
+      const float2 w1 = *reinterpret_cast<const float2*>(Wk + (k + 1) * wld + j0);
+      a0 = fmaf(x0, w0.x, a0);
+      a1 = fmaf(x0, w0.y, a1);
+      b0 = fmaf(x1, w1.x, b0);
+      b1 = fmaf(x1, w1.y, b1);
     }
-    const float4 w0 = ld4(Wk + k * wld + j0), w1 = ld4(Wk + k * wld + j0 + 4);
-    const float w[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
+    if (k < K) {
+      const float x0 = A[k * RRS + r];
+      const float2 w0 = *reinterpret_cast<const float2*>(Wk + k * wld + j0);
+      a0 = fmaf(x0, w0.x, a0);
+      a1 = fmaf(x0, w0.y, a1);
+    }
+    const float z0 = (a0 + b0) + bias[j0], z1 = (a1 + b1) + bias[j0 + 1];
+    OUT[j0 * RRS + r] = ACT == ACT_TANH ? tanh_fast(z0) : fmaxf(z0, 0.f);
+    OUT[(j0 + 1) * RRS + r] = ACT == ACT_TANH ? tanh_fast(z1) : fmaxf(z1, 0.f);
+  }
+}
+
+// One MLP layer over a feature-major tile of ROWS rows (row stride ROWS + TILE_PAD):
+//   OUT[j][r] = act(bias[j] + sum_k A[k][r] * Wk[k * wld + j])     for j < JPx (a multiple of 32)
+// each element an fmaf chain over k in ascending order from 0, then + bias, then the activation.  Groups of 4 warps
+// (ROWS / (32 RPL) groups, one per 128 threads) split the rows: warp -> 8-column group (warp % 4) of its group's
+// 32 RPL rows (warp / 4), lane -> RPL consecutive rows.  RPL = 0 is the 8-row tile of tile_layer8.
+template <int ACT, int RPL, int ROWS = rows_of(RPL)>
+__device__ __forceinline__ void tile_layer(const float* __restrict__ A, int K, const float* __restrict__ Wk, int wld,
+                                           const float* __restrict__ bias, float* __restrict__ OUT, int JPx) {
+  if (RPL == 0) {
+    tile_layer8<ACT>(A, K, Wk, wld, bias, OUT, JPx);
+    return;
+  }
+  constexpr int RRS = ROWS + TILE_PAD;
+  constexpr int NGRP = RPL > 0 ? ROWS / (32 * RPL) : 1;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int cg = NGRP == 1 ? warp : warp & 3;
+  const int r0 = (NGRP == 1 ? 0 : (warp >> 2) * 32 * RPL) + lane * RPL;
+  for (int jh = 0; jh < JPx / 32; ++jh) {
+    const int j0 = jh * 32 + cg * 8;
+    float acc[RPL > 0 ? RPL : 1][8];
 #pragma unroll
-    for (int q = 0; q < NQ; ++q) {
-      const float av[4] = {a[q].x, a[q].y, a[q].z, a[q].w};
+    for (int a = 0; a < RPL; ++a)
 #pragma unroll
-      for (int x = 0; x < 4; ++x)
+      for (int t = 0; t < 8; ++t) acc[a][t] = 0.f;
+#pragma unroll 4
+    for (int k = 0; k < K; ++k) {
+      float av[RPL > 0 ? RPL : 1];
+      if (RPL == 4) {
+        const float4 a4 = ld4(A + k * RRS + r0);
+        av[0] = a4.x, av[RPL > 1 ? 1 : 0] = a4.y, av[RPL > 2 ? 2 : 0] = a4.z, av[RPL > 3 ? 3 : 0] = a4.w;
+      } else if (RPL == 2) {
+        const float2 a2 = *reinterpret_cast<const float2*>(A + k * RRS + r0);
+        av[0] = a2.x, av[RPL > 1 ? 1 : 0] = a2.y;
+      } else {
+        av[0] = A[k * RRS + r0];
+      }
+      const float4 w0 = ld4(Wk + k * wld + j0), w1 = ld4(Wk + k * wld + j0 + 4);
+      const float w[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
 #pragma unroll
-        for (int t = 0; t < 8; ++t) acc[q * 4 + x][t] = fmaf(av[x], w[t], acc[q * 4 + x][t]);
+      for (int x = 0; x < RPL; ++x)
+#pragma unroll
+        for (int t = 0; t < 8; ++t) acc[x][t] = fmaf(av[x], w[t], acc[x][t]);
+    }
+#pragma unroll
+    for (int t = 0; t < 8; ++t) {
+      const float b = bias[j0 + t];
+#pragma unroll
+      for (int x = 0; x < RPL; ++x) {
+        const float z = acc[x][t] + b;
+        OUT[(j0 + t) * RRS + r0 + x] = ACT == ACT_TANH ? tanh_fast(z) : fmaxf(z, 0.f);
+      }
     }
   }
 }
 
-// 4 x 4 variant (PPO: 64-row minibatch tiles, 16 outputs per thread)
-template <bool TANHMASK>
-__device__ __forceinline__ void gemm_acc44(float (&acc)[4][4], const float* __restrict__ A, int RS, int r0,
-                                           const float* __restrict__ Wk, int wld, int j0, int K) {
-#pragma unroll 4
+// dL/dz of a ReLU layer contracted with the next layer's weights, for the 4 rows r0..r0+3 and 8 columns j0..j0+7:
+//   acc[x][t] += sum_k D[k][r0 + x] * Wk[k * wld + j0 + t],   D[k][r] = (S[k][r] > 0) ? g_r * sk[k] : 0
+// S: the layer's post-activation tile (feature-major, row stride RS); g: the upstream scalar of each of the 4 rows;
+// sk: per-k scale; Wk: k-major weights (row stride wld, 16-byte aligned).
+__device__ __forceinline__ void gemm_acc(float (&acc)[4][8], const float* __restrict__ S, int RS, int r0,
+                                         const float* __restrict__ Wk, int wld, int j0, int K, const float4 g,
+                                         const float* __restrict__ sk) {
+#pragma unroll 2
   for (int k = 0; k < K; ++k) {
-    const float4 a = ld4(A + k * RS + r0);
-    const float4 w = ld4(Wk + k * wld + j0);
-    const float av[4] = {a.x, a.y, a.z, a.w}, wv[4] = {w.x, w.y, w.z, w.w};
+    float4 a = ld4(S + k * RS + r0);
+    const float s = sk[k];
+    a.x = a.x > 0.f ? g.x * s : 0.f;
+    a.y = a.y > 0.f ? g.y * s : 0.f;
+    a.z = a.z > 0.f ? g.z * s : 0.f;
+    a.w = a.w > 0.f ? g.w * s : 0.f;
+    const float4 w0 = ld4(Wk + k * wld + j0), w1 = ld4(Wk + k * wld + j0 + 4);
+    const float w[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
+    const float av[4] = {a.x, a.y, a.z, a.w};
 #pragma unroll
     for (int x = 0; x < 4; ++x)
 #pragma unroll
-      for (int t = 0; t < 4; ++t) acc[x][t] = fmaf(av[x], wv[t], acc[x][t]);
+      for (int t = 0; t < 8; ++t) acc[x][t] = fmaf(av[x], w[t], acc[x][t]);
   }
 }
 
