@@ -24,95 +24,131 @@ IMB_RF_DETERMINISTIC = 1  # imb_rollout flags
 ST_RING_IDX, ST_RING_N, ST_EP_STEP, ST_EPISODE, ST_GLOBAL_STEP, ST_REPLAY_DRAW = 0, 1, 2, 3, 4, 5
 ST_EXPERT_POS, ST_EXPERT_EPOCH, ST_PPO_EPOCH, ST_DISC_STEP, ST_PPO_STEP, ST_WORDS = 6, 7, 8, 9, 10, 16
 
+PU_MAX_MEMBERS = 16  # members of an imb_pref_unc_desc / imb_rollout_members
+SYNC_MAX_AVG, SYNC_MAX_NORM = 8, 4  # tensors of an imb_sync_desc
+
 
 class ImbError(RuntimeError):
     pass
 
 
+# the C types of include/imb.h: int / int32_t, int64_t, uint64_t, float, and every data pointer and stream
+_i32, _i64, _u64, _f32, _ptr = C.c_int32, C.c_int64, C.c_uint64, C.c_float, C.c_void_p
+
+
 class Mlp(C.Structure):
-    _fields_ = [("din", C.c_int32), ("n_hidden", C.c_int32), ("h1", C.c_int32), ("h2", C.c_int32),
-                ("n_out", C.c_int32), ("has_norm", C.c_int32), ("param_off", C.c_int32), ("norm_off", C.c_int32),
-                ("count_idx", C.c_int32), ("norm_eps", C.c_float)]
+    _fields_ = [("din", _i32), ("n_hidden", _i32), ("h1", _i32), ("h2", _i32), ("n_out", _i32), ("has_norm", _i32),
+                ("param_off", _i32), ("norm_off", _i32), ("count_idx", _i32), ("norm_eps", _f32)]
 
 
 class DiscDesc(C.Structure):
-    _fields_ = [("d_obs", C.c_int32), ("d_act", C.c_int32), ("use_state", C.c_int32), ("use_action", C.c_int32),
-                ("use_next_state", C.c_int32), ("use_done", C.c_int32), ("base", Mlp), ("shaped", C.c_int32),
-                ("potential", Mlp), ("gamma", C.c_float), ("subtract_logp", C.c_int32), ("n_params", C.c_int32)]
+    _fields_ = [("d_obs", _i32), ("d_act", _i32), ("use_state", _i32), ("use_action", _i32), ("use_next_state", _i32),
+                ("use_done", _i32), ("base", Mlp), ("shaped", _i32), ("potential", Mlp), ("gamma", _f32),
+                ("subtract_logp", _i32), ("n_params", _i32)]
 
 
 class Adam(C.Structure):
-    _fields_ = [("lr", C.c_float), ("beta1", C.c_float), ("beta2", C.c_float), ("eps", C.c_float),
-                ("weight_decay", C.c_float)]  # > 0: torch.optim.AdamW's decoupled decay
+    _fields_ = [("lr", _f32), ("beta1", _f32), ("beta2", _f32), ("eps", _f32),
+                ("weight_decay", _f32)]  # > 0: torch.optim.AdamW's decoupled decay
 
 
 class PolicyDesc(C.Structure):
-    _fields_ = [("d_obs", C.c_int32), ("d_act", C.c_int32), ("discrete", C.c_int32), ("hidden", C.c_int32),
-                ("has_norm", C.c_int32), ("norm_eps", C.c_float),
-                ("off_pi_w1", C.c_int32), ("off_pi_b1", C.c_int32), ("off_pi_w2", C.c_int32), ("off_pi_b2", C.c_int32),
-                ("off_vf_w1", C.c_int32), ("off_vf_b1", C.c_int32), ("off_vf_w2", C.c_int32), ("off_vf_b2", C.c_int32),
-                ("off_act_w", C.c_int32), ("off_act_b", C.c_int32), ("off_val_w", C.c_int32), ("off_val_b", C.c_int32),
-                ("off_log_std", C.c_int32), ("n_params", C.c_int32)]
+    _fields_ = [("d_obs", _i32), ("d_act", _i32), ("discrete", _i32), ("hidden", _i32), ("has_norm", _i32),
+                ("norm_eps", _f32), ("off_pi_w1", _i32), ("off_pi_b1", _i32), ("off_pi_w2", _i32), ("off_pi_b2", _i32),
+                ("off_vf_w1", _i32), ("off_vf_b1", _i32), ("off_vf_w2", _i32), ("off_vf_b2", _i32), ("off_act_w", _i32),
+                ("off_act_b", _i32), ("off_val_w", _i32), ("off_val_b", _i32), ("off_log_std", _i32),
+                ("n_params", _i32)]
 
 
 class EnvDesc(C.Structure):
-    _fields_ = [("d_obs", C.c_int32), ("d_act", C.c_int32), ("discrete", C.c_int32), ("horizon", C.c_int32),
-                ("seed", C.c_uint64), ("env_id_offset", C.c_int64)]
+    _fields_ = [("d_obs", _i32), ("d_act", _i32), ("discrete", _i32), ("horizon", _i32), ("seed", _u64),
+                ("env_id_offset", _i64)]
 
 
 class PpoHparams(C.Structure):
-    _fields_ = [("gamma", C.c_float), ("gae_lambda", C.c_float), ("clip_range", C.c_float), ("ent_coef", C.c_float),
-                ("vf_coef", C.c_float), ("max_grad_norm", C.c_float), ("lr", C.c_float), ("adam_eps", C.c_float),
-                ("n_epochs", C.c_int32), ("batch_size", C.c_int32), ("normalize_advantage", C.c_int32)]
-
-
-PU_MAX_MEMBERS = 16
+    _fields_ = [("gamma", _f32), ("gae_lambda", _f32), ("clip_range", _f32), ("ent_coef", _f32), ("vf_coef", _f32),
+                ("max_grad_norm", _f32), ("lr", _f32), ("adam_eps", _f32), ("n_epochs", _i32), ("batch_size", _i32),
+                ("normalize_advantage", _i32)]
 
 
 class PrefUncDesc(C.Structure):
-    _fields_ = [("n_members", C.c_int32), ("rews", C.c_void_p * PU_MAX_MEMBERS),
-                ("norm_state", C.c_void_p * PU_MAX_MEMBERS), ("norm_count", C.c_void_p * PU_MAX_MEMBERS),
-                ("norm_eps", C.c_float * PU_MAX_MEMBERS), ("norm_kind", C.c_int32 * PU_MAX_MEMBERS),
-                ("norm_decay", C.c_float * PU_MAX_MEMBERS)]
-
-
-PU_MODES = {"logit": 0, "probability": 1, "label": 2}
+    _fields_ = [("n_members", _i32), ("rews", _ptr * PU_MAX_MEMBERS), ("norm_state", _ptr * PU_MAX_MEMBERS),
+                ("norm_count", _ptr * PU_MAX_MEMBERS), ("norm_eps", _f32 * PU_MAX_MEMBERS),
+                ("norm_kind", _i32 * PU_MAX_MEMBERS), ("norm_decay", _f32 * PU_MAX_MEMBERS)]
 
 
 class RolloutMembers(C.Structure):
-    _fields_ = [("n_members", C.c_int32), ("params", C.c_void_p * PU_MAX_MEMBERS),
-                ("norm_state", C.c_void_p * PU_MAX_MEMBERS), ("raw", C.c_void_p)]
-
-SYNC_MAX_AVG, SYNC_MAX_NORM = 8, 4
+    _fields_ = [("n_members", _i32), ("params", _ptr * PU_MAX_MEMBERS), ("norm_state", _ptr * PU_MAX_MEMBERS),
+                ("raw", _ptr)]
 
 
 class SyncDesc(C.Structure):
-    _fields_ = [("n_avg", C.c_int32), ("n_norm", C.c_int32), ("avg", C.c_void_p * SYNC_MAX_AVG),
-                ("avg_n", C.c_int64 * SYNC_MAX_AVG), ("mean", C.c_void_p * SYNC_MAX_NORM),
-                ("var", C.c_void_p * SYNC_MAX_NORM), ("count", C.c_void_p * SYNC_MAX_NORM),
-                ("k", C.c_int32 * SYNC_MAX_NORM)]
+    _fields_ = [("n_avg", _i32), ("n_norm", _i32), ("avg", _ptr * SYNC_MAX_AVG), ("avg_n", _i64 * SYNC_MAX_AVG),
+                ("mean", _ptr * SYNC_MAX_NORM), ("var", _ptr * SYNC_MAX_NORM), ("count", _ptr * SYNC_MAX_NORM),
+                ("k", _i32 * SYNC_MAX_NORM)]
 
-
-_lib: Optional[C.CDLL] = None
-
-# every symbol include/imb.h declares (tests check the library exports each of them)
-SYMBOLS = [
-    "imb_version", "imb_last_error", "imb_disc_workspace_floats", "imb_disc_norm_update", "imb_disc_fwd_bwd",
-    "imb_disc_reduce", "imb_disc_adam", "imb_reward_forward", "imb_reward_norm_scan", "imb_reward_ema_scan",
-    "imb_table_store",
-    "imb_ring_advance", "imb_sample_indices", "imb_gather_rows", "imb_rollout", "imb_rollout_row_width", "imb_gae",
-    "imb_rollout_advance", "imb_env_reset", "imb_ppo_update", "imb_policy_logp", "imb_state_init",
-    "imb_sync_buffer_doubles", "imb_sync_snapshot", "imb_sync_pack", "imb_sync_unpack",
-    "imb_disc_sample_gather", "imb_sample_advance2", "imb_disc_reduce_adam", "imb_norm_batch_stats", "imb_norm_fold",
-    "imb_disc_set_rows", "imb_stats_publish", "imb_pref_loss", "imb_pref_uncertainty_ws_floats", "imb_pref_uncertainty",
-    "imb_rollout_ensemble", "imb_ensemble_relabel_ws_floats", "imb_ensemble_relabel", "imb_disc_plan", "imb_ppo_plan",
-    "imb_ppo_update_variant",
-]
 
 # imb_disc_plan codes: the kernel imb_disc_fwd_bwd runs
 PLAN_TC, PLAN_FFMA128X2, PLAN_FFMA256, PLAN_FFMA128 = 1, 2, 3, 4
 # imb_ppo_plan codes: the kernel imb_ppo_update runs
 PPO_PLAN_UPDATE, PPO_PLAN_GEN1, PPO_PLAN_GEN2 = 1, 2, 3
+# imb_pref_uncertainty modes
+PU_MODES = {"logit": 0, "probability": 1, "label": 2}
+
+_disc, _adam, _pol, _env, _hp, _pu, _members, _sync = map(C.POINTER, (
+    DiscDesc, Adam, PolicyDesc, EnvDesc, PpoHparams, PrefUncDesc, RolloutMembers, SyncDesc))
+
+# every entry point include/imb.h declares, in its order: name -> (restype, argtypes, kernels launched per call; None:
+# the wrapper counts them).  tests/test_cabi_loads.py holds this table to the header.
+SIGNATURES = {
+    "imb_version": (_i32, [], 0),
+    "imb_last_error": (C.c_char_p, [], 0),
+    "imb_disc_workspace_floats": (_i64, [_disc], 0),
+    "imb_disc_norm_update": (_i32, [_disc, _ptr, _i64, _i64, _ptr, _ptr, _ptr, _ptr], None),
+    "imb_norm_batch_stats": (_i32, [_disc, _ptr, _i64, _i64, _i32, _i32, _ptr, _ptr, _ptr, _i32, _ptr, _ptr], 1),
+    "imb_norm_fold": (_i32, [_i32, _ptr, _ptr, _ptr, _i32, _ptr], 1),
+    "imb_stats_publish": (_i32, [_ptr, _i32, _ptr, _ptr, _i32, _ptr], 1),
+    "imb_disc_set_rows": (_i32, [_disc, _ptr, _i64, _i64, _ptr], 1),
+    "imb_disc_fwd_bwd": (_i32, [_disc, _ptr, _ptr, _ptr, _i64, _i64, _i64, _f32, _ptr, _ptr, _i32, _ptr, _ptr], 1),
+    "imb_disc_plan": (_i32, [_disc, _i64], 0),
+    "imb_disc_reduce": (_i32, [_disc, _ptr, _ptr, _ptr], 1),
+    "imb_disc_adam": (_i32, [_disc, _adam, _ptr, _ptr, _ptr, _ptr, _f32, _ptr, _ptr, _ptr, _ptr], 1),
+    "imb_reward_forward": (_i32, [_disc, _ptr, _ptr, _ptr, _i64, _i64, _i32, _ptr, _ptr], 1),
+    "imb_reward_norm_scan": (_i32, [_ptr, _i64, _i64, _i64, _i64, _ptr, _ptr, _f32, _i32, _ptr], 1),
+    "imb_reward_ema_scan": (_i32, [_ptr, _i64, _i64, _i64, _i64, _ptr, _ptr, _f32, _f32, _i32, _ptr], 1),
+    "imb_table_store": (_i32, [_ptr, _i64, _i32, _i32, _ptr, _ptr, _ptr, _ptr, _ptr, _i64, _i32, _ptr, _ptr], 1),
+    "imb_ring_advance": (_i32, [_ptr, _i64, _i64, _ptr], 1),
+    "imb_sample_indices": (_i32, [_i32, _ptr, _i64, _i64, _u64, _ptr, _ptr], 2),
+    "imb_disc_sample_gather": (_i32, [_ptr, _i64, _ptr, _i64, _i32, _i64, _i64, _u64, _ptr, _ptr, _ptr, _i64, _ptr], 1),
+    "imb_sample_advance2": (_i32, [_i64, _i64, _ptr, _ptr, _ptr], 1),
+    "imb_gather_rows": (_i32, [_ptr, _i64, _i32, _ptr, _i64, _ptr, _i64, _i64, _ptr], 1),
+    "imb_rollout": (_i32, [_env, _ptr, _ptr, _pol, _ptr, _ptr, _disc, _ptr, _ptr, _i32, _hp, _i64, _i64, _ptr, _ptr,
+                           _i64, _ptr, _ptr, _ptr, _i32, _ptr, _ptr], 1),
+    "imb_rollout_row_width": (_i32, [_pol], 0),
+    "imb_gae": (_i32, [_ptr, _i32, _i32, _i64, _i64, _ptr, _f32, _f32, _ptr, _i32, _ptr], 1),
+    "imb_rollout_advance": (_i32, [_ptr, _i64, _i64, _i32, _i64, _ptr], 1),
+    "imb_env_reset": (_i32, [_ptr, _i64, _env, _ptr, _ptr], 1),
+    "imb_ppo_update": (_i32, [_pol, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _i64, _hp, _ptr, _u64, _ptr, _ptr, _ptr], 1),
+    "imb_ppo_plan": (_i32, [_pol, _i32], 0),
+    "imb_ppo_update_variant": (_i32, [_pol], 0),
+    "imb_policy_logp": (_i32, [_pol, _ptr, _ptr, _ptr, _i64, _i64, _i32, _ptr], 1),
+    "imb_disc_reduce_adam": (_i32, [_disc, _adam, _ptr, _ptr, _ptr, _f32, _ptr, _ptr, _ptr, _ptr], 1),
+    "imb_pref_loss": (_i32, [_ptr, _i64, _i32, _ptr, _f32, _f32, _f32, _f32, _ptr, _ptr, _ptr, _i32, _ptr], 1),
+    "imb_pref_uncertainty_ws_floats": (_i64, [_i32, _i64], 0),
+    "imb_pref_uncertainty": (_i32, [_pu, _i64, _i32, _i32, _f32, _f32, _f32, _ptr, _ptr, _ptr, _ptr], None),
+    "imb_rollout_ensemble": (_i32, [_env, _ptr, _ptr, _pol, _ptr, _ptr, _disc, _members, _hp, _i64, _i64, _ptr, _ptr,
+                                    _i64, _ptr, _ptr, _ptr, _i32, _ptr, _ptr], 1),
+    "imb_ensemble_relabel_ws_floats": (_i64, [_i32, _i64], 0),
+    "imb_ensemble_relabel": (_i32, [_pu, _f32, _ptr, _i32, _i32, _i64, _i64, _ptr, _ptr], None),
+    "imb_sync_buffer_doubles": (_i64, [_sync], 0),
+    "imb_sync_snapshot": (_i32, [_sync, _ptr, _ptr], None),
+    "imb_sync_pack": (_i32, [_sync, _ptr, _ptr], 1),
+    "imb_sync_unpack": (_i32, [_sync, _ptr, _ptr, _i32, _ptr], 1),
+    "imb_state_init": (_i32, [_ptr, _ptr], 0),
+}
+SYMBOLS = list(SIGNATURES)
+
+_lib: Optional[C.CDLL] = None
 
 
 def lib() -> C.CDLL:
@@ -122,56 +158,43 @@ def lib() -> C.CDLL:
         if not os.path.exists(LIB_PATH):
             raise ImbError(f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
                            "(nvcc, sm_90a). imitation_b200 has no CPU fallback.")
-        _lib = C.CDLL(LIB_PATH)
-        _lib.imb_last_error.restype = C.c_char_p
-        _lib.imb_disc_workspace_floats.restype = C.c_int64
-        _lib.imb_sync_buffer_doubles.restype = C.c_int64
-        _lib.imb_pref_uncertainty_ws_floats.restype = C.c_int64
-        _lib.imb_ensemble_relabel_ws_floats.restype = C.c_int64
-        for name in SYMBOLS:
-            getattr(_lib, name)  # AttributeError if the .so is stale
+        dll = C.CDLL(LIB_PATH)
+        for name, (restype, argtypes, _) in SIGNATURES.items():
+            fn = getattr(dll, name)  # AttributeError if the .so is stale
+            fn.restype, fn.argtypes = restype, argtypes
+        _lib = dll
     return _lib
 
 
 # kernel launches issued through this binding (bench.py reports them as `gpu_launches`)
 LAUNCHES = {"count": 0}
-_KERNELS_PER_CALL = {
-    "imb_state_init": 0, "imb_disc_norm_update": None, "imb_disc_fwd_bwd": 1, "imb_disc_reduce": 1,
-    "imb_disc_adam": 1, "imb_reward_forward": 1, "imb_reward_norm_scan": 1, "imb_reward_ema_scan": 1,
-    "imb_table_store": 1,
-    "imb_ring_advance": 1, "imb_sample_indices": 2, "imb_gather_rows": 1, "imb_rollout": 1, "imb_gae": 1,
-    "imb_rollout_advance": 1, "imb_env_reset": 1, "imb_ppo_update": 1, "imb_policy_logp": 1,
-    "imb_disc_sample_gather": 1, "imb_sample_advance2": 1, "imb_disc_reduce_adam": 1, "imb_norm_batch_stats": 1,
-    "imb_norm_fold": 1, "imb_disc_set_rows": 1, "imb_stats_publish": 1, "imb_pref_loss": 1,
-    "imb_pref_uncertainty": None, "imb_rollout_ensemble": 1, "imb_ensemble_relabel": None,
-}
 
 
 def _check(rc: int, what: str, n_kernels: Optional[int] = None):
-    LAUNCHES["count"] += _KERNELS_PER_CALL.get(what, 1) if n_kernels is None else n_kernels
+    LAUNCHES["count"] += SIGNATURES[what][2] if n_kernels is None else n_kernels
     if rc != 0:
         raise ImbError(f"{what}: {lib().imb_last_error().decode()} (rc={rc})")
 
 
-def _p(t: Optional[th.Tensor], dtype=None):
+def _p(t: Optional[th.Tensor], dtype=None) -> Optional[int]:
     """Device pointer of a contiguous CUDA tensor (None -> NULL)."""
     if t is None:
-        return C.c_void_p(0)
+        return None
     if not t.is_cuda:
         raise ImbError("imitation_b200 kernels need CUDA tensors (no CPU path)")
     if not t.is_contiguous():
         raise ImbError("tensor must be contiguous")
     if dtype is not None and t.dtype != dtype:
         raise ImbError(f"expected dtype {dtype}, got {t.dtype}")
-    return C.c_void_p(t.data_ptr())
+    return t.data_ptr()
 
 
-def _stream():
-    return C.c_void_p(th.cuda.current_stream().cuda_stream)
+def _stream() -> int:
+    return th.cuda.current_stream().cuda_stream
 
 
 def disc_workspace_floats(d: DiscDesc) -> int:
-    return int(lib().imb_disc_workspace_floats(C.byref(d)))
+    return lib().imb_disc_workspace_floats(d)
 
 
 def sync_desc(averaged, norms) -> SyncDesc:
@@ -182,29 +205,27 @@ def sync_desc(averaged, norms) -> SyncDesc:
     d = SyncDesc()
     d.n_avg, d.n_norm = len(averaged), len(norms)
     for i, t in enumerate(averaged):
-        d.avg[i], d.avg_n[i] = _p(t, th.float32).value, t.numel()
+        d.avg[i], d.avg_n[i] = _p(t, th.float32), t.numel()
     for i, (m, v, c) in enumerate(norms):
-        d.mean[i], d.var[i], d.count[i] = _p(m, th.float32).value, _p(v, th.float32).value, _p(c, th.int32).value
+        d.mean[i], d.var[i], d.count[i] = _p(m, th.float32), _p(v, th.float32), _p(c, th.int32)
         d.k[i] = m.numel()
     return d
 
 
 def sync_buffer_doubles(d: SyncDesc) -> int:
-    return int(lib().imb_sync_buffer_doubles(C.byref(d)))
+    return lib().imb_sync_buffer_doubles(d)
 
 
 def sync_snapshot(d: SyncDesc, start):
-    _check(lib().imb_sync_snapshot(C.byref(d), _p(start, th.float64), _stream()), "imb_sync_snapshot",
-           1 if d.n_norm else 0)
+    _check(lib().imb_sync_snapshot(d, _p(start, th.float64), _stream()), "imb_sync_snapshot", 1 if d.n_norm else 0)
 
 
 def sync_pack(d: SyncDesc, buf):
-    _check(lib().imb_sync_pack(C.byref(d), _p(buf, th.float64), _stream()), "imb_sync_pack")
+    _check(lib().imb_sync_pack(d, _p(buf, th.float64), _stream()), "imb_sync_pack")
 
 
 def sync_unpack(d: SyncDesc, buf, start, world: int):
-    _check(lib().imb_sync_unpack(C.byref(d), _p(buf, th.float64), _p(start, th.float64), C.c_int32(world), _stream()),
-           "imb_sync_unpack")
+    _check(lib().imb_sync_unpack(d, _p(buf, th.float64), _p(start, th.float64), world, _stream()), "imb_sync_unpack")
 
 
 def state_init(state):
@@ -212,78 +233,73 @@ def state_init(state):
 
 
 def disc_norm_update(d, batch, ld, n, norm_state, norm_count, ws):
-    _check(lib().imb_disc_norm_update(C.byref(d), _p(batch, th.float32), C.c_int64(ld), C.c_int64(n),
-                                      _p(norm_state, th.float32), _p(norm_count, th.int32), _p(ws, th.float32),
-                                      _stream()), "imb_disc_norm_update",
+    _check(lib().imb_disc_norm_update(d, _p(batch, th.float32), ld, n, _p(norm_state, th.float32),
+                                      _p(norm_count, th.int32), _p(ws, th.float32), _stream()), "imb_disc_norm_update",
            1 if (d.shaped and d.potential.has_norm) else int(d.base.has_norm))  # shaped: one multi-job launch
 
 
 def norm_batch_stats(d, batch, ld, n, row0, din, norm_state, norm_count, defer, defer_cap, ws):
     """RunningNorm update of a foreign normaliser (the policy's feature extractor) from batch rows [row0, row0 + din);
     `defer` = slot list for a later in-order `norm_fold` (None: fold immediately)."""
-    _check(lib().imb_norm_batch_stats(C.byref(d), _p(batch, th.float32), C.c_int64(ld), C.c_int64(n), C.c_int(row0),
-                                      C.c_int(din), _p(norm_state, th.float32), _p(norm_count, th.int32), _p(defer),
-                                      C.c_int(defer_cap), _p(ws, th.float32), _stream()), "imb_norm_batch_stats")
+    _check(lib().imb_norm_batch_stats(d, _p(batch, th.float32), ld, n, row0, din, _p(norm_state, th.float32),
+                                      _p(norm_count, th.int32), _p(defer), defer_cap, _p(ws, th.float32), _stream()),
+           "imb_norm_batch_stats")
 
 
 def norm_fold(din, defer, norm_state, norm_count, n_slots=0):
-    _check(lib().imb_norm_fold(C.c_int(din), _p(defer, th.float32), _p(norm_state, th.float32),
-                               _p(norm_count, th.int32), C.c_int(n_slots), _stream()), "imb_norm_fold")
+    _check(lib().imb_norm_fold(din, _p(defer, th.float32), _p(norm_state, th.float32), _p(norm_count, th.int32),
+                               n_slots, _stream()), "imb_norm_fold")
 
 
 def stats_publish(stats_dev, n, host_pinned, state, state_idx):
     """host_pinned: a pinned (page-locked, hence device-mapped under unified addressing) float32 CPU tensor of 16 elements."""
     if host_pinned.is_cuda or not host_pinned.is_pinned() or host_pinned.numel() < 16:
         raise ImbError("stats_publish needs a pinned CPU tensor of >= 16 floats")
-    _check(lib().imb_stats_publish(_p(stats_dev, th.float32), C.c_int(n), C.c_void_p(host_pinned.data_ptr()),
-                                   _p(state, th.int64), C.c_int(state_idx), _stream()), "imb_stats_publish")
+    _check(lib().imb_stats_publish(_p(stats_dev, th.float32), n, host_pinned.data_ptr(), _p(state, th.int64), state_idx,
+                                   _stream()), "imb_stats_publish")
 
 
 def disc_set_rows(d, ws, n_rows_total, n_expert_total):
-    _check(lib().imb_disc_set_rows(C.byref(d), _p(ws, th.float32), C.c_int64(n_rows_total), C.c_int64(n_expert_total),
-                                   _stream()), "imb_disc_set_rows")
+    _check(lib().imb_disc_set_rows(d, _p(ws, th.float32), n_rows_total, n_expert_total, _stream()), "imb_disc_set_rows")
 
 
 def disc_fwd_bwd(d, params, norm_state, batch, ld, n, n_expert, loss_scale, grad_out, logits_out, flags, ws):
-    _check(lib().imb_disc_fwd_bwd(C.byref(d), _p(params, th.float32), _p(norm_state, th.float32),
-                                  _p(batch, th.float32), C.c_int64(ld), C.c_int64(n), C.c_int64(n_expert),
-                                  C.c_float(loss_scale), _p(grad_out), _p(logits_out), C.c_int(flags),
-                                  _p(ws, th.float32), _stream()), "imb_disc_fwd_bwd")
+    _check(lib().imb_disc_fwd_bwd(d, _p(params, th.float32), _p(norm_state, th.float32), _p(batch, th.float32), ld, n,
+                                  n_expert, loss_scale, _p(grad_out), _p(logits_out), flags, _p(ws, th.float32),
+                                  _stream()), "imb_disc_fwd_bwd")
 
 
 def disc_plan(d: DiscDesc, n: int) -> int:
     """PLAN_* code of the kernel `disc_fwd_bwd` runs for `d` over n rows (host only, no GPU needed); ImbError naming
     the shared-memory limit when the fused kernels cannot run the shape."""
-    rc = int(lib().imb_disc_plan(C.byref(d), C.c_int64(n)))
+    rc = lib().imb_disc_plan(d, n)
     if rc < 0:
         raise ImbError(f"imb_disc_plan: {lib().imb_last_error().decode()} (rc={rc})")
     return rc
 
 
 def disc_reduce(d, ws, grad_out_flat=None):
-    _check(lib().imb_disc_reduce(C.byref(d), _p(ws, th.float32), _p(grad_out_flat), _stream()), "imb_disc_reduce")
+    _check(lib().imb_disc_reduce(d, _p(ws, th.float32), _p(grad_out_flat), _stream()), "imb_disc_reduce")
 
 
 def disc_adam(d, opt: Adam, params, exp_avg, exp_avg_sq, grad_flat, grad_div, ws, state, stats_out):
-    _check(lib().imb_disc_adam(C.byref(d), C.byref(opt), _p(params, th.float32), _p(exp_avg, th.float32),
-                               _p(exp_avg_sq, th.float32), _p(grad_flat), C.c_float(grad_div), _p(ws, th.float32),
-                               _p(state, th.int64), _p(stats_out), _stream()), "imb_disc_adam")
+    _check(lib().imb_disc_adam(d, opt, _p(params, th.float32), _p(exp_avg, th.float32), _p(exp_avg_sq, th.float32),
+                               _p(grad_flat), grad_div, _p(ws, th.float32), _p(state, th.int64), _p(stats_out),
+                               _stream()), "imb_disc_adam")
 
 
 def reward_forward(d, params, norm_state, batch, ld, n, out_mode, out):
-    _check(lib().imb_reward_forward(C.byref(d), _p(params, th.float32), _p(norm_state, th.float32),
-                                    _p(batch, th.float32), C.c_int64(ld), C.c_int64(n), C.c_int(out_mode),
-                                    _p(out, th.float32), _stream()), "imb_reward_forward")
+    _check(lib().imb_reward_forward(d, _p(params, th.float32), _p(norm_state, th.float32), _p(batch, th.float32), ld,
+                                    n, out_mode, _p(out, th.float32), _stream()), "imb_reward_forward")
 
 
 def pref_loss(rews, n_pairs, frag_len, prefs, noise_prob, discount, threshold, grad_scale, grad_rews, probs_out, stats_acc,
               stats_slot=0):
     """Boltzmann preference probabilities + cross entropy (+ d loss / d rews) of one minibatch of fragment pairs;
     stats_acc: float32 [4 * n_slots] accumulators, slot k = (sum of minibatch losses, sum of accuracies, n minibatches, -)."""
-    _check(lib().imb_pref_loss(_p(rews, th.float32), C.c_int64(n_pairs), C.c_int32(frag_len), _p(prefs, th.float32),
-                               C.c_float(noise_prob), C.c_float(discount), C.c_float(threshold), C.c_float(grad_scale),
-                               _p(grad_rews), _p(probs_out), _p(stats_acc), C.c_int32(stats_slot), _stream()),
-           "imb_pref_loss")
+    _check(lib().imb_pref_loss(_p(rews, th.float32), n_pairs, frag_len, _p(prefs, th.float32), noise_prob, discount,
+                               threshold, grad_scale, _p(grad_rews), _p(probs_out), _p(stats_acc), stats_slot,
+                               _stream()), "imb_pref_loss")
 
 
 def pref_uncertainty_desc(rews, norms) -> PrefUncDesc:
@@ -295,9 +311,9 @@ def pref_uncertainty_desc(rews, norms) -> PrefUncDesc:
     d = PrefUncDesc()
     d.n_members = len(rews)
     for m, (r, nm) in enumerate(zip(rews, norms)):
-        d.rews[m] = _p(r, th.float32).value
+        d.rews[m] = _p(r, th.float32)
         if nm is not None:
-            d.norm_state[m], d.norm_count[m] = _p(nm[0], th.float32).value, _p(nm[1], th.int32).value
+            d.norm_state[m], d.norm_count[m] = _p(nm[0], th.float32), _p(nm[1], th.int32)
             d.norm_eps[m] = nm[2]
             if len(nm) > 3:
                 d.norm_kind[m], d.norm_decay[m] = 1, nm[3]
@@ -305,17 +321,16 @@ def pref_uncertainty_desc(rews, norms) -> PrefUncDesc:
 
 
 def pref_uncertainty_ws_floats(n_members: int, n_pairs: int) -> int:
-    return int(lib().imb_pref_uncertainty_ws_floats(C.c_int32(n_members), C.c_int64(n_pairs)))
+    return lib().imb_pref_uncertainty_ws_floats(n_members, n_pairs)
 
 
 def pref_uncertainty(d: PrefUncDesc, n_pairs, frag_len, mode, noise_prob, discount, threshold, ws, scores,
                      member_out=None):
     """Active-selection scores of n_pairs candidate pairs (mode: 0 logit, 1 probability, 2 label; PU_MODES)."""
     norm = any(d.norm_state[m] for m in range(d.n_members))
-    _check(lib().imb_pref_uncertainty(C.byref(d), C.c_int64(n_pairs), C.c_int32(frag_len), C.c_int32(mode),
-                                      C.c_float(noise_prob), C.c_float(discount), C.c_float(threshold),
-                                      _p(ws, th.float32), _p(scores, th.float32), _p(member_out, th.float32),
-                                      _stream()), "imb_pref_uncertainty", (1 + int(norm)) if n_pairs > 0 else 0)
+    _check(lib().imb_pref_uncertainty(d, n_pairs, frag_len, mode, noise_prob, discount, threshold, _p(ws, th.float32),
+                                      _p(scores, th.float32), _p(member_out, th.float32), _stream()),
+           "imb_pref_uncertainty", (1 + int(norm)) if n_pairs > 0 else 0)
 
 
 def reward_norm_scan(rews, n_envs, n_steps, step_stride, env_stride, norm_state2, norm_count, eps, update_stats,
@@ -324,72 +339,62 @@ def reward_norm_scan(rews, n_envs, n_steps, step_stride, env_stride, norm_state2
     [mean, var], norm_count [count]; otherwise EMANorm with that decay, norm_state2 [mean, var, inv_learning_rate],
     norm_count [count, num_batches]."""
     if ema_decay is None:
-        _check(lib().imb_reward_norm_scan(_p(rews, th.float32), C.c_int64(n_envs), C.c_int64(n_steps),
-                                          C.c_int64(step_stride), C.c_int64(env_stride), _p(norm_state2, th.float32),
-                                          _p(norm_count, th.int32), C.c_float(eps), C.c_int(int(update_stats)),
+        _check(lib().imb_reward_norm_scan(_p(rews, th.float32), n_envs, n_steps, step_stride, env_stride,
+                                          _p(norm_state2, th.float32), _p(norm_count, th.int32), eps, int(update_stats),
                                           _stream()), "imb_reward_norm_scan")
     else:
-        _check(lib().imb_reward_ema_scan(_p(rews, th.float32), C.c_int64(n_envs), C.c_int64(n_steps),
-                                         C.c_int64(step_stride), C.c_int64(env_stride), _p(norm_state2, th.float32),
-                                         _p(norm_count, th.int32), C.c_float(ema_decay), C.c_float(eps),
-                                         C.c_int(int(update_stats)), _stream()), "imb_reward_ema_scan")
+        _check(lib().imb_reward_ema_scan(_p(rews, th.float32), n_envs, n_steps, step_stride, env_stride,
+                                         _p(norm_state2, th.float32), _p(norm_count, th.int32), ema_decay, eps,
+                                         int(update_stats), _stream()), "imb_reward_ema_scan")
 
 
 def table_store(table, capacity, d_obs, d_act, obs, acts_f, acts_i, next_obs, dones, n, use_ring, state):
-    _check(lib().imb_table_store(_p(table, th.float32), C.c_int64(capacity), C.c_int32(d_obs), C.c_int32(d_act),
-                                 _p(obs, th.float32), _p(acts_f), _p(acts_i), _p(next_obs, th.float32),
-                                 _p(dones, th.uint8), C.c_int64(n), C.c_int(int(use_ring)), _p(state), _stream()),
-           "imb_table_store")
+    _check(lib().imb_table_store(_p(table, th.float32), capacity, d_obs, d_act, _p(obs, th.float32), _p(acts_f),
+                                 _p(acts_i), _p(next_obs, th.float32), _p(dones, th.uint8), n, int(use_ring), _p(state),
+                                 _stream()), "imb_table_store")
 
 
 def ring_advance(state, capacity, n_stored):
-    _check(lib().imb_ring_advance(_p(state, th.int64), C.c_int64(capacity), C.c_int64(n_stored), _stream()),
-           "imb_ring_advance")
+    _check(lib().imb_ring_advance(_p(state, th.int64), capacity, n_stored, _stream()), "imb_ring_advance")
 
 
 def sample_indices(kind, idx_out, n, size, seed, state):
-    _check(lib().imb_sample_indices(C.c_int(kind), _p(idx_out, th.int64), C.c_int64(n), C.c_int64(size),
-                                    C.c_uint64(seed), _p(state, th.int64), _stream()), "imb_sample_indices")
+    _check(lib().imb_sample_indices(kind, _p(idx_out, th.int64), n, size, seed, _p(state, th.int64), _stream()),
+           "imb_sample_indices")
 
 
 def disc_sample_gather(e_table, e_n, ring, ring_cap, tw, mb, start, seed, e_state, g_state, batch, ld):
-    _check(lib().imb_disc_sample_gather(_p(e_table, th.float32), C.c_int64(e_n), _p(ring, th.float32),
-                                        C.c_int64(ring_cap), C.c_int32(tw), C.c_int64(mb), C.c_int64(start),
-                                        C.c_uint64(seed), _p(e_state, th.int64), _p(g_state, th.int64),
-                                        _p(batch, th.float32), C.c_int64(ld), _stream()), "imb_disc_sample_gather")
+    _check(lib().imb_disc_sample_gather(_p(e_table, th.float32), e_n, _p(ring, th.float32), ring_cap, tw, mb, start,
+                                        seed, _p(e_state, th.int64), _p(g_state, th.int64), _p(batch, th.float32), ld,
+                                        _stream()), "imb_disc_sample_gather")
 
 
 def sample_advance2(n, e_n, e_state, g_state):
-    _check(lib().imb_sample_advance2(C.c_int64(n), C.c_int64(e_n), _p(e_state, th.int64), _p(g_state, th.int64),
-                                     _stream()), "imb_sample_advance2")
+    _check(lib().imb_sample_advance2(n, e_n, _p(e_state, th.int64), _p(g_state, th.int64), _stream()),
+           "imb_sample_advance2")
 
 
 def disc_reduce_adam(d, opt, params, exp_avg, exp_avg_sq, grad_div, ws, state, stats_out):
-    _check(lib().imb_disc_reduce_adam(C.byref(d), C.byref(opt), _p(params, th.float32), _p(exp_avg, th.float32),
-                                      _p(exp_avg_sq, th.float32), C.c_float(grad_div), _p(ws, th.float32),
-                                      _p(state, th.int64), _p(stats_out, th.float32), _stream()),
-           "imb_disc_reduce_adam")
+    _check(lib().imb_disc_reduce_adam(d, opt, _p(params, th.float32), _p(exp_avg, th.float32),
+                                      _p(exp_avg_sq, th.float32), grad_div, _p(ws, th.float32), _p(state, th.int64),
+                                      _p(stats_out, th.float32), _stream()), "imb_disc_reduce_adam")
 
 
 def gather_rows(table, capacity, tw, idx, n, batch, ld, col0):
-    _check(lib().imb_gather_rows(_p(table, th.float32), C.c_int64(capacity), C.c_int32(tw), _p(idx), C.c_int64(n),
-                                 _p(batch, th.float32), C.c_int64(ld), C.c_int64(col0), _stream()),
-           "imb_gather_rows")
+    _check(lib().imb_gather_rows(_p(table, th.float32), capacity, tw, _p(idx), n, _p(batch, th.float32), ld, col0,
+                                 _stream()), "imb_gather_rows")
 
 
 def rollout_row_width(pol: PolicyDesc) -> int:
-    return int(lib().imb_rollout_row_width(C.byref(pol)))
+    return lib().imb_rollout_row_width(pol)
 
 
 def rollout(env, env_params, env_obs, pol, pol_params, pol_norm, disc, disc_params, disc_norm, reward_mode, hp,
             n_envs, n_steps, rollout_tbl, ring, ring_capacity, flat_out, aux, noise, state, flags=0):
-    _check(lib().imb_rollout(C.byref(env), _p(env_params, th.float32), _p(env_obs, th.float32), C.byref(pol),
-                             _p(pol_params, th.float32), _p(pol_norm), C.byref(disc) if disc is not None else None,
-                             _p(disc_params), _p(disc_norm), C.c_int(reward_mode), C.byref(hp), C.c_int64(n_envs),
-                             C.c_int64(n_steps), _p(rollout_tbl, th.float32), _p(ring), C.c_int64(ring_capacity),
-                             _p(flat_out), _p(aux, th.float32), _p(noise), C.c_int(flags), _p(state, th.int64),
-                             _stream()),
-           "imb_rollout")
+    _check(lib().imb_rollout(env, _p(env_params, th.float32), _p(env_obs, th.float32), pol, _p(pol_params, th.float32),
+                             _p(pol_norm), disc, _p(disc_params), _p(disc_norm), reward_mode, hp, n_envs, n_steps,
+                             _p(rollout_tbl, th.float32), _p(ring), ring_capacity, _p(flat_out), _p(aux, th.float32),
+                             _p(noise), flags, _p(state, th.int64), _stream()), "imb_rollout")
 
 
 def rollout_members(params, norm_states, raw) -> RolloutMembers:
@@ -400,64 +405,58 @@ def rollout_members(params, norm_states, raw) -> RolloutMembers:
     d = RolloutMembers()
     d.n_members = len(params)
     for m, (pm, nm) in enumerate(zip(params, norm_states)):
-        d.params[m] = _p(pm, th.float32).value
-        d.norm_state[m] = _p(nm, th.float32).value if nm is not None else None
-    d.raw = _p(raw, th.float32).value
+        d.params[m], d.norm_state[m] = _p(pm, th.float32), _p(nm, th.float32)
+    d.raw = _p(raw, th.float32)
     return d
 
 
 def rollout_ensemble(env, env_params, env_obs, pol, pol_params, pol_norm, disc, members: RolloutMembers, hp, n_envs,
                      n_steps, rollout_tbl, ring, ring_capacity, flat_out, aux, noise, state, flags=0):
     """`rollout` with every member's raw reward written to members.raw ([M][T][E]) instead of the reward column."""
-    _check(lib().imb_rollout_ensemble(C.byref(env), _p(env_params, th.float32), _p(env_obs, th.float32), C.byref(pol),
-                                      _p(pol_params, th.float32), _p(pol_norm), C.byref(disc), C.byref(members),
-                                      C.byref(hp), C.c_int64(n_envs), C.c_int64(n_steps), _p(rollout_tbl, th.float32),
-                                      _p(ring), C.c_int64(ring_capacity), _p(flat_out), _p(aux, th.float32), _p(noise),
-                                      C.c_int(flags), _p(state, th.int64), _stream()),
+    _check(lib().imb_rollout_ensemble(env, _p(env_params, th.float32), _p(env_obs, th.float32), pol,
+                                      _p(pol_params, th.float32), _p(pol_norm), disc, members, hp, n_envs, n_steps,
+                                      _p(rollout_tbl, th.float32), _p(ring), ring_capacity, _p(flat_out),
+                                      _p(aux, th.float32), _p(noise), flags, _p(state, th.int64), _stream()),
            "imb_rollout_ensemble")
 
 
 def ensemble_relabel_ws_floats(n_members: int, n_steps: int) -> int:
-    return int(lib().imb_ensemble_relabel_ws_floats(C.c_int32(n_members), C.c_int64(n_steps)))
+    return lib().imb_ensemble_relabel_ws_floats(n_members, n_steps)
 
 
 def ensemble_relabel(d: PrefUncDesc, alpha, rollout_tbl, rw, col_rew, n_envs, n_steps, ws):
     """Per-step output normalisation of the members (d.rews[m] = member m's raw [T][E]) and mean + alpha * std into the
     rollout table's reward column."""
     norm = any(d.norm_state[m] for m in range(d.n_members))
-    _check(lib().imb_ensemble_relabel(C.byref(d), C.c_float(alpha), _p(rollout_tbl, th.float32), C.c_int32(rw),
-                                      C.c_int32(col_rew), C.c_int64(n_envs), C.c_int64(n_steps), _p(ws, th.float32),
-                                      _stream()), "imb_ensemble_relabel", 1 + int(norm))
+    _check(lib().imb_ensemble_relabel(d, alpha, _p(rollout_tbl, th.float32), rw, col_rew, n_envs, n_steps,
+                                      _p(ws, th.float32), _stream()), "imb_ensemble_relabel", 1 + int(norm))
 
 
 def gae(rollout_tbl, rw, col_value, n_envs, n_steps, aux, gamma, gae_lambda, state, horizon):
-    _check(lib().imb_gae(_p(rollout_tbl, th.float32), C.c_int32(rw), C.c_int32(col_value), C.c_int64(n_envs),
-                         C.c_int64(n_steps), _p(aux, th.float32), C.c_float(gamma), C.c_float(gae_lambda),
-                         _p(state, th.int64), C.c_int32(horizon), _stream()), "imb_gae")
+    _check(lib().imb_gae(_p(rollout_tbl, th.float32), rw, col_value, n_envs, n_steps, _p(aux, th.float32), gamma,
+                         gae_lambda, _p(state, th.int64), horizon, _stream()), "imb_gae")
 
 
 def rollout_advance(state, n_envs, n_steps, horizon, ring_capacity):
-    _check(lib().imb_rollout_advance(_p(state, th.int64), C.c_int64(n_envs), C.c_int64(n_steps), C.c_int32(horizon),
-                                     C.c_int64(ring_capacity), _stream()), "imb_rollout_advance")
+    _check(lib().imb_rollout_advance(_p(state, th.int64), n_envs, n_steps, horizon, ring_capacity, _stream()),
+           "imb_rollout_advance")
 
 
 def env_reset(env_obs, n_envs, env, state):
-    _check(lib().imb_env_reset(_p(env_obs, th.float32), C.c_int64(n_envs), C.byref(env), _p(state, th.int64),
-                               _stream()), "imb_env_reset")
+    _check(lib().imb_env_reset(_p(env_obs, th.float32), n_envs, env, _p(state, th.int64), _stream()), "imb_env_reset")
 
 
 def ppo_update(pol, params, norm, norm_count, exp_avg, exp_avg_sq, rollout_tbl, n_rows, hp, perm, seed, loss_log,
                state):
-    _check(lib().imb_ppo_update(C.byref(pol), _p(params, th.float32), _p(norm), _p(norm_count),
-                                _p(exp_avg, th.float32), _p(exp_avg_sq, th.float32), _p(rollout_tbl, th.float32),
-                                C.c_int64(n_rows), C.byref(hp), _p(perm), C.c_uint64(seed), _p(loss_log),
-                                _p(state, th.int64), _stream()), "imb_ppo_update")
+    _check(lib().imb_ppo_update(pol, _p(params, th.float32), _p(norm), _p(norm_count), _p(exp_avg, th.float32),
+                                _p(exp_avg_sq, th.float32), _p(rollout_tbl, th.float32), n_rows, hp, _p(perm), seed,
+                                _p(loss_log), _p(state, th.int64), _stream()), "imb_ppo_update")
 
 
 def ppo_plan(pol: PolicyDesc, batch_size: int) -> int:
     """PPO_PLAN_* code of the kernel `ppo_update` runs for `pol` at minibatch size batch_size (host only, no GPU
     needed); ImbError naming the shared-memory need and limit when no PPO kernel can run the shape."""
-    rc = int(lib().imb_ppo_plan(C.byref(pol), C.c_int32(batch_size)))
+    rc = lib().imb_ppo_plan(pol, batch_size)
     if rc < 0:
         raise ImbError(f"imb_ppo_plan: {lib().imb_last_error().decode()} (rc={rc})")
     return rc
@@ -466,9 +465,9 @@ def ppo_plan(pol: PolicyDesc, batch_size: int) -> int:
 def ppo_update_variant(pol: PolicyDesc) -> int:
     """Instantiation of k_ppo_update that `ppo_update` runs for `pol` when `ppo_plan` gives PPO_PLAN_UPDATE (host only):
     0 = the runtime-shape one, 1-3 = the shape-specialised ones (include/imb.h); IMB_PPO_FORCE_RUNTIME_SHAPE=1 forces 0."""
-    return int(lib().imb_ppo_update_variant(C.byref(pol)))
+    return lib().imb_ppo_update_variant(pol)
 
 
 def policy_logp(pol, params, norm, batch, ld, n, row_logp):
-    _check(lib().imb_policy_logp(C.byref(pol), _p(params, th.float32), _p(norm), _p(batch, th.float32),
-                                 C.c_int64(ld), C.c_int64(n), C.c_int32(row_logp), _stream()), "imb_policy_logp")
+    _check(lib().imb_policy_logp(pol, _p(params, th.float32), _p(norm), _p(batch, th.float32), ld, n, row_logp,
+                                 _stream()), "imb_policy_logp")
