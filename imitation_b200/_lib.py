@@ -19,6 +19,7 @@ IMB_F_ZERO_GRAD = 1
 IMB_F_TRAIN_NORM = 2
 IMB_F_NO_TENSOR = 4   # force the fp32-FFMA discriminator kernel (A/B measurements)
 IMB_RF_DETERMINISTIC = 1  # imb_rollout flags
+ACT_TANH, ACT_RELU = 0, 1  # pol_act: the policy towers' activation (imb_rollout, imb_ppo_update, imb_policy_logp, ...)
 
 # device-resident counter block (include/imb.h enum)
 ST_RING_IDX, ST_RING_N, ST_EP_STEP, ST_EPISODE, ST_GLOBAL_STEP, ST_REPLAY_DRAW = 0, 1, 2, 3, 4, 5
@@ -122,22 +123,23 @@ SIGNATURES = {
     "imb_disc_sample_gather": (_i32, [_ptr, _i64, _ptr, _i64, _i32, _i64, _i64, _u64, _ptr, _ptr, _ptr, _i64, _ptr], 1),
     "imb_sample_advance2": (_i32, [_i64, _i64, _ptr, _ptr, _ptr], 1),
     "imb_gather_rows": (_i32, [_ptr, _i64, _i32, _ptr, _i64, _ptr, _i64, _i64, _ptr], 1),
-    "imb_rollout": (_i32, [_env, _ptr, _ptr, _pol, _ptr, _ptr, _disc, _ptr, _ptr, _i32, _hp, _i64, _i64, _ptr, _ptr,
-                           _i64, _ptr, _ptr, _ptr, _i32, _ptr, _ptr], 1),
+    "imb_rollout": (_i32, [_env, _ptr, _ptr, _pol, _i32, _ptr, _ptr, _disc, _ptr, _ptr, _i32, _hp, _i64, _i64, _ptr,
+                           _ptr, _i64, _ptr, _ptr, _ptr, _i32, _ptr, _ptr], 1),
     "imb_rollout_row_width": (_i32, [_pol], 0),
     "imb_gae": (_i32, [_ptr, _i32, _i32, _i64, _i64, _ptr, _f32, _f32, _ptr, _i32, _ptr], 1),
     "imb_rollout_advance": (_i32, [_ptr, _i64, _i64, _i32, _i64, _ptr], 1),
     "imb_env_reset": (_i32, [_ptr, _i64, _env, _ptr, _ptr], 1),
-    "imb_ppo_update": (_i32, [_pol, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _i64, _hp, _ptr, _u64, _ptr, _ptr, _ptr], 1),
-    "imb_ppo_plan": (_i32, [_pol, _i32], 0),
+    "imb_ppo_update": (_i32, [_pol, _i32, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _i64, _hp, _ptr, _u64, _ptr, _ptr, _ptr],
+                       1),
+    "imb_ppo_plan": (_i32, [_pol, _i32, _i32], 0),
     "imb_ppo_update_variant": (_i32, [_pol], 0),
-    "imb_policy_logp": (_i32, [_pol, _ptr, _ptr, _ptr, _i64, _i64, _i32, _ptr], 1),
+    "imb_policy_logp": (_i32, [_pol, _i32, _ptr, _ptr, _ptr, _i64, _i64, _i32, _ptr], 1),
     "imb_disc_reduce_adam": (_i32, [_disc, _adam, _ptr, _ptr, _ptr, _f32, _ptr, _ptr, _ptr, _ptr], 1),
     "imb_pref_loss": (_i32, [_ptr, _i64, _i32, _ptr, _f32, _f32, _f32, _f32, _ptr, _ptr, _ptr, _i32, _ptr], 1),
     "imb_pref_uncertainty_ws_floats": (_i64, [_i32, _i64], 0),
     "imb_pref_uncertainty": (_i32, [_pu, _i64, _i32, _i32, _f32, _f32, _f32, _ptr, _ptr, _ptr, _ptr], None),
-    "imb_rollout_ensemble": (_i32, [_env, _ptr, _ptr, _pol, _ptr, _ptr, _disc, _members, _hp, _i64, _i64, _ptr, _ptr,
-                                    _i64, _ptr, _ptr, _ptr, _i32, _ptr, _ptr], 1),
+    "imb_rollout_ensemble": (_i32, [_env, _ptr, _ptr, _pol, _i32, _ptr, _ptr, _disc, _members, _hp, _i64, _i64, _ptr,
+                                    _ptr, _i64, _ptr, _ptr, _ptr, _i32, _ptr, _ptr], 1),
     "imb_ensemble_relabel_ws_floats": (_i64, [_i32, _i64], 0),
     "imb_ensemble_relabel": (_i32, [_pu, _f32, _ptr, _i32, _i32, _i64, _i64, _ptr, _ptr], None),
     "imb_sync_buffer_doubles": (_i64, [_sync], 0),
@@ -390,9 +392,10 @@ def rollout_row_width(pol: PolicyDesc) -> int:
 
 
 def rollout(env, env_params, env_obs, pol, pol_params, pol_norm, disc, disc_params, disc_norm, reward_mode, hp,
-            n_envs, n_steps, rollout_tbl, ring, ring_capacity, flat_out, aux, noise, state, flags=0):
-    _check(lib().imb_rollout(env, _p(env_params, th.float32), _p(env_obs, th.float32), pol, _p(pol_params, th.float32),
-                             _p(pol_norm), disc, _p(disc_params), _p(disc_norm), reward_mode, hp, n_envs, n_steps,
+            n_envs, n_steps, rollout_tbl, ring, ring_capacity, flat_out, aux, noise, state, flags=0, act=ACT_TANH):
+    """act: the policy towers' activation, ACT_TANH or ACT_RELU (the same for every policy entry point below)."""
+    _check(lib().imb_rollout(env, _p(env_params, th.float32), _p(env_obs, th.float32), pol, act,
+                             _p(pol_params, th.float32), _p(pol_norm), disc, _p(disc_params), _p(disc_norm), reward_mode, hp, n_envs, n_steps,
                              _p(rollout_tbl, th.float32), _p(ring), ring_capacity, _p(flat_out), _p(aux, th.float32),
                              _p(noise), flags, _p(state, th.int64), _stream()), "imb_rollout")
 
@@ -411,9 +414,9 @@ def rollout_members(params, norm_states, raw) -> RolloutMembers:
 
 
 def rollout_ensemble(env, env_params, env_obs, pol, pol_params, pol_norm, disc, members: RolloutMembers, hp, n_envs,
-                     n_steps, rollout_tbl, ring, ring_capacity, flat_out, aux, noise, state, flags=0):
+                     n_steps, rollout_tbl, ring, ring_capacity, flat_out, aux, noise, state, flags=0, act=ACT_TANH):
     """`rollout` with every member's raw reward written to members.raw ([M][T][E]) instead of the reward column."""
-    _check(lib().imb_rollout_ensemble(env, _p(env_params, th.float32), _p(env_obs, th.float32), pol,
+    _check(lib().imb_rollout_ensemble(env, _p(env_params, th.float32), _p(env_obs, th.float32), pol, act,
                                       _p(pol_params, th.float32), _p(pol_norm), disc, members, hp, n_envs, n_steps,
                                       _p(rollout_tbl, th.float32), _p(ring), ring_capacity, _p(flat_out),
                                       _p(aux, th.float32), _p(noise), flags, _p(state, th.int64), _stream()),
@@ -447,16 +450,16 @@ def env_reset(env_obs, n_envs, env, state):
 
 
 def ppo_update(pol, params, norm, norm_count, exp_avg, exp_avg_sq, rollout_tbl, n_rows, hp, perm, seed, loss_log,
-               state):
-    _check(lib().imb_ppo_update(pol, _p(params, th.float32), _p(norm), _p(norm_count), _p(exp_avg, th.float32),
+               state, act=ACT_TANH):
+    _check(lib().imb_ppo_update(pol, act, _p(params, th.float32), _p(norm), _p(norm_count), _p(exp_avg, th.float32),
                                 _p(exp_avg_sq, th.float32), _p(rollout_tbl, th.float32), n_rows, hp, _p(perm), seed,
                                 _p(loss_log), _p(state, th.int64), _stream()), "imb_ppo_update")
 
 
-def ppo_plan(pol: PolicyDesc, batch_size: int) -> int:
-    """PPO_PLAN_* code of the kernel `ppo_update` runs for `pol` at minibatch size batch_size (host only, no GPU
-    needed); ImbError naming the shared-memory need and limit when no PPO kernel can run the shape."""
-    rc = lib().imb_ppo_plan(pol, batch_size)
+def ppo_plan(pol: PolicyDesc, batch_size: int, act: int = ACT_TANH) -> int:
+    """PPO_PLAN_* code of the kernel `ppo_update` runs for `pol` with activation `act` at minibatch size batch_size
+    (host only, no GPU needed); ImbError naming the shared-memory need and limit when no PPO kernel can run the shape."""
+    rc = lib().imb_ppo_plan(pol, act, batch_size)
     if rc < 0:
         raise ImbError(f"imb_ppo_plan: {lib().imb_last_error().decode()} (rc={rc})")
     return rc
@@ -468,6 +471,6 @@ def ppo_update_variant(pol: PolicyDesc) -> int:
     return lib().imb_ppo_update_variant(pol)
 
 
-def policy_logp(pol, params, norm, batch, ld, n, row_logp):
-    _check(lib().imb_policy_logp(pol, _p(params, th.float32), _p(norm), _p(batch, th.float32), ld, n, row_logp,
+def policy_logp(pol, params, norm, batch, ld, n, row_logp, act=ACT_TANH):
+    _check(lib().imb_policy_logp(pol, act, _p(params, th.float32), _p(norm), _p(batch, th.float32), ld, n, row_logp,
                                  _stream()), "imb_policy_logp")

@@ -472,7 +472,8 @@ class AdversarialTrainer(base.DemonstrationAlgorithm):
             self._policy_norm_side_effect(eng, n)
             if self._needs_logp:
                 pp, pn, _ = self.policy.flat_vectors()
-                _lib.policy_logp(self.policy.desc, pp, pn, self._batch, self._ld, n, self._bw - 1)
+                _lib.policy_logp(self.policy.desc, pp, pn, self._batch, self._ld, n, self._bw - 1,
+                                 act=self.policy.act)
             tn = train_mode and eng.has_norm
             W = self._dist_world
             if tn and W > 1:

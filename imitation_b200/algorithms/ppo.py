@@ -51,7 +51,7 @@ class DevicePPO:
                 th.manual_seed(self._user_seed)
             self.policy = cls(self._base_env.observation_space, self._base_env.action_space, **kw).to(self.device)
         try:  # refuse a policy / minibatch no PPO kernel can run now, not at the first train()
-            _lib.ppo_plan(self.policy.desc, self.batch_size)
+            _lib.ppo_plan(self.policy.desc, self.batch_size, act=self.policy.act)
         except _lib.ImbError as e:
             raise NotImplementedError(f"policy / minibatch not supported by the PPO update kernels: {e}") from None
         n = self.policy.desc.n_params
@@ -123,11 +123,12 @@ class DevicePPO:
         ring_args = (ring.table if ring is not None else None, ring.capacity if ring is not None else 0)
         if ens is None:
             _lib.rollout(env.desc, env.params, env.obs, pol.desc, pp, pn, disc, dparams, dnorm, mode, self.hp, E, T,
-                         self._tbl, *ring_args, flat, self._aux, self.noise, env.state)
+                         self._tbl, *ring_args, flat, self._aux, self.noise, env.state, act=pol.act)
         else:
             members, relabel = self._ensemble_tables(ens, E, T)
             _lib.rollout_ensemble(env.desc, env.params, env.obs, pol.desc, pp, pn, ens.nets[0].engine().desc, members,
-                                  self.hp, E, T, self._tbl, *ring_args, flat, self._aux, self.noise, env.state)
+                                  self.hp, E, T, self._tbl, *ring_args, flat, self._aux, self.noise, env.state,
+                                  act=pol.act)
         da = 1 if pol.discrete else pol.d_act
         col_val = pol.d_obs + da + 1
         if ens is not None:
@@ -171,7 +172,7 @@ class DevicePPO:
         pp, pn, pc = pol.flat_vectors()
         N = self._tbl.shape[0]
         _lib.ppo_update(pol.desc, pp, pn, pc, self.exp_avg, self.exp_avg_sq, self._tbl, N, self.hp, self.perm,
-                        self.seed, self.loss_log, self._base_env.state)
+                        self.seed, self.loss_log, self._base_env.state, act=pol.act)
 
     def _pointer_key(self):
         """Everything a captured graph bakes in: device pointers of the vectors the kernels touch."""

@@ -973,8 +973,9 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
 
 // ---- log pi(a|s) for the AIRL discriminator batch --------------------------------------------------------------
 // thread per batch column; obs rows [0,Do), act rows [Do, Do+Da_onehot) of the feature-major batch.  The pi tower, the
-// action head and log_std come from the policy's PolImg; then xn_ld >= Do inputs per thread.
-template <int HP>
+// action head and log_std come from the policy's PolImg; then xn_ld >= Do inputs per thread.  ACT: the towers'
+// activation (ACT_TANH: tanhf, ACT_RELU: fmaxf(z, 0)).
+template <int HP, int ACT>
 __global__ void __launch_bounds__(128) k_policy_logp(const imb_policy_desc pd, const float* __restrict__ params,
                                                     const float* __restrict__ norm, float* __restrict__ batch,
                                                     int64_t ld, int64_t n, int row_logp, int xn_off, int xn_ld) {
@@ -1004,7 +1005,7 @@ __global__ void __launch_bounds__(128) k_policy_logp(const imb_policy_desc pd, c
     }
 #pragma unroll
     for (int j = 0; j < HP; ++j) {
-      h1[j] = tanhf(h1[j]);
+      h1[j] = ACT == ACT_TANH ? tanhf(h1[j]) : fmaxf(h1[j], 0.f);
       lat[j] = smem[S.b2p + j];
     }
 #pragma unroll
@@ -1014,7 +1015,7 @@ __global__ void __launch_bounds__(128) k_policy_logp(const imb_policy_desc pd, c
       for (int j = 0; j < HP; ++j) lat[j] = fmaf(w2t[i * HP + j], hv, lat[j]);
     }
 #pragma unroll
-    for (int j = 0; j < HP; ++j) lat[j] = tanhf(lat[j]);
+    for (int j = 0; j < HP; ++j) lat[j] = ACT == ACT_TANH ? tanhf(lat[j]) : fmaxf(lat[j], 0.f);
     float logp = 0.f;
     if (!pd.discrete) {
       for (int a = 0; a < Da; ++a) {
@@ -1094,9 +1095,12 @@ extern "C" int imb_rollout_row_width(const imb_policy_desc* pol);
 // Which PPO kernel runs the policy A.pol at minibatch A.hp.batch_size (the IMB_PPO_PLAN_* codes of imb_ppo_plan), with
 // the launch geometry (rw, KP, S, RS2, HP) filled into A and the dynamic shared memory into *bytes.  k_ppo_update
 // (64-row minibatch resident in shared memory, one lane per hidden unit) for tower width <= 32 and minibatches <= 64
-// rows when its shared memory and slice fit; else k_ppo_update_gen with U = 1 or 2 hidden units per lane.
-static int ppo_plan(PpoArgs& A, size_t* bytes) {
+// rows when its shared memory and slice fit; else k_ppo_update_gen with U = 1 or 2 hidden units per lane.  ReLU towers
+// (act = IMB_ACT_RELU) always run k_ppo_update_gen: k_ppo_update is built for the tanh policies bench.py trains.
+static int ppo_plan(PpoArgs& A, int act, size_t* bytes) {
   const imb_policy_desc& pd = A.pol;
+  IMB_REQUIRE(act == IMB_ACT_TANH || act == IMB_ACT_RELU,
+              "pol_act must be IMB_ACT_TANH (0) or IMB_ACT_RELU (1), got %d", act);
   IMB_REQUIRE(pd.hidden >= 1 && pd.hidden <= 64, "policy tower width must be <= 64");
   IMB_REQUIRE(pd.d_obs >= 1 && pd.d_obs <= IMB_MAX_DIN && pd.d_act >= 1 && pd.d_act <= IMB_MAX_DIN,
               "d_obs/d_act must be in [1, %d]", IMB_MAX_DIN);
@@ -1108,7 +1112,7 @@ static int ppo_plan(PpoArgs& A, size_t* bytes) {
   A.RS2 = ppo_row_stride(A.rw);
   // IMB_PPO_FORCE_GENERAL=1 (tests): run the general kernel on shapes the specialised one covers
   const char* force = getenv("IMB_PPO_FORCE_GENERAL");
-  if (pd.hidden <= 32 && A.hp.batch_size <= PR && !(force && force[0] == '1')) {
+  if (act == IMB_ACT_TANH && pd.hidden <= 32 && A.hp.batch_size <= PR && !(force && force[0] == '1')) {
     A.HP = 32;
     *bytes = ppo_smem_floats(A) * 4;
     if (A.S / 4 <= PT && *bytes <= IMB_SMEM_MAX) return IMB_PPO_PLAN_UPDATE;
@@ -1120,12 +1124,12 @@ static int ppo_plan(PpoArgs& A, size_t* bytes) {
   return A.HP == 32 ? IMB_PPO_PLAN_GEN1 : IMB_PPO_PLAN_GEN2;
 }
 
-extern "C" int imb_ppo_plan(const imb_policy_desc* pol, int32_t batch_size) {
+extern "C" int imb_ppo_plan(const imb_policy_desc* pol, int32_t pol_act, int32_t batch_size) {
   PpoArgs A = {};
   A.pol = *pol;
   A.hp.batch_size = batch_size;
   size_t bytes;
-  return ppo_plan(A, &bytes);
+  return ppo_plan(A, pol_act, &bytes);
 }
 
 // The policy shapes with their own instantiation of k_ppo_update (tower width 32): the policies bench.py trains.
@@ -1163,31 +1167,33 @@ static int ppo_variant(const imb_policy_desc& pd) {
 
 extern "C" int imb_ppo_update_variant(const imb_policy_desc* pol) { return ppo_variant(*pol); }
 
-static int launch_ppo(const PpoArgs& A0, float* params, float* norm, int32_t* norm_count, float* m, float* v,
+static int launch_ppo(const PpoArgs& A0, int act, float* params, float* norm, int32_t* norm_count, float* m, float* v,
                       const float* rollout, const int64_t* perm, float* loss_log, int64_t* state, cudaStream_t st) {
   PpoArgs A = A0;
   size_t bytes;
-  const int plan = ppo_plan(A, &bytes);
+  const int plan = ppo_plan(A, act, &bytes);
   if (plan == IMB_PPO_PLAN_UPDATE) {
     static size_t attr_bytes[kNumPpoVariants] = {};
     const int var = ppo_variant(A.pol);
     return launch_cluster(kPpoUpdateKernels[var], kPpoUpdateNames[var], bytes, &attr_bytes[var], st, A, params, norm,
                           norm_count, m, v, rollout, perm, loss_log, state);
   }
-  if (plan == IMB_PPO_PLAN_GEN1) {
-    static size_t attr_bytes = 0;
-    return launch_cluster(k_ppo_update_gen<1>, "k_ppo_update_gen<1>", bytes, &attr_bytes, st, A, params, norm, norm_count, m,
+  if (plan == IMB_PPO_PLAN_GEN1 || plan == IMB_PPO_PLAN_GEN2) {
+    // [U - 1][act]: k_ppo_update_gen<U, act>
+    static size_t attr_bytes[2][2] = {};
+    constexpr decltype(&k_ppo_update_gen<1, ACT_TANH>) kernels[2][2] = {
+        {k_ppo_update_gen<1, ACT_TANH>, k_ppo_update_gen<1, ACT_RELU>},
+        {k_ppo_update_gen<2, ACT_TANH>, k_ppo_update_gen<2, ACT_RELU>}};
+    constexpr const char* names[2][2] = {{"k_ppo_update_gen<1>", "k_ppo_update_gen<1, relu>"},
+                                         {"k_ppo_update_gen<2>", "k_ppo_update_gen<2, relu>"}};
+    const int u = plan == IMB_PPO_PLAN_GEN1 ? 0 : 1;
+    return launch_cluster(kernels[u][act], names[u][act], bytes, &attr_bytes[u][act], st, A, params, norm, norm_count, m,
                           v, rollout, perm, loss_log, state);
-  }
-  if (plan == IMB_PPO_PLAN_GEN2) {
-    static size_t attr_bytes2 = 0;
-    return launch_cluster(k_ppo_update_gen<2>, "k_ppo_update_gen<2>", bytes, &attr_bytes2, st, A, params, norm, norm_count,
-                          m, v, rollout, perm, loss_log, state);
   }
   return plan;
 }
 
-extern "C" int imb_ppo_update(const imb_policy_desc* pol, float* pol_params, float* pol_norm,
+extern "C" int imb_ppo_update(const imb_policy_desc* pol, int32_t pol_act, float* pol_params, float* pol_norm,
                               int32_t* pol_norm_count, float* exp_avg, float* exp_avg_sq, const float* rollout,
                               int64_t n_rows, const imb_ppo_hparams* hp, const int64_t* perm, uint64_t seed,
                               float* loss_log, int64_t* state, void* stream) {
@@ -1197,11 +1203,11 @@ extern "C" int imb_ppo_update(const imb_policy_desc* pol, float* pol_params, flo
   A.hp = *hp;
   A.n_rows = n_rows;
   A.seed = seed;
-  return launch_ppo(A, pol_params, pol_norm, pol_norm_count, exp_avg, exp_avg_sq, rollout, perm, loss_log, state,
+  return launch_ppo(A, pol_act, pol_params, pol_norm, pol_norm_count, exp_avg, exp_avg_sq, rollout, perm, loss_log, state,
                     (cudaStream_t)stream);
 }
 
-template <int HP>
+template <int HP, int ACT>
 static int launch_logp(const imb_policy_desc* pol, const float* params, const float* norm, float* batch, int64_t ld,
                        int64_t n, int row_logp, cudaStream_t st) {
   auto al = [](int x) { return (x + 31) / 32 * 32; };
@@ -1210,24 +1216,31 @@ static int launch_logp(const imb_policy_desc* pol, const float* params, const fl
   IMB_REQUIRE(bytes <= IMB_SMEM_MAX, "policy too large");
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(k_policy_logp<HP>, cudaFuncAttributeMaxDynamicSharedMemorySize, IMB_SMEM_MAX);
+    cudaError_t e = cudaFuncSetAttribute(k_policy_logp<HP, ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, IMB_SMEM_MAX);
     if (e != cudaSuccess) IMB_FAIL(-2, "cudaFuncSetAttribute(k_policy_logp): %s", cudaGetErrorString(e));
     attr_set = true;
   }
   int64_t blocks = (n + 127) / 128;
   const int64_t cap = (int64_t)imb_num_sms() * 2;
   if (blocks > cap) blocks = cap;
-  k_policy_logp<HP><<<(int)blocks, 128, bytes, st>>>(*pol, params, norm, batch, ld, n, row_logp, xn_off, xn_ld);
+  k_policy_logp<HP, ACT><<<(int)blocks, 128, bytes, st>>>(*pol, params, norm, batch, ld, n, row_logp, xn_off, xn_ld);
   IMB_CHECK_LAUNCH("k_policy_logp");
   return 0;
 }
 
-extern "C" int imb_policy_logp(const imb_policy_desc* pol, const float* pol_params, const float* pol_norm,
-                               float* batch, int64_t ld, int64_t n, int32_t row_logp, void* stream) {
+extern "C" int imb_policy_logp(const imb_policy_desc* pol, int32_t pol_act, const float* pol_params,
+                               const float* pol_norm, float* batch, int64_t ld, int64_t n, int32_t row_logp,
+                               void* stream) {
+  IMB_REQUIRE(pol_act == IMB_ACT_TANH || pol_act == IMB_ACT_RELU,
+              "pol_act must be IMB_ACT_TANH (0) or IMB_ACT_RELU (1), got %d", pol_act);
   if (n <= 0) return 0;
   IMB_REQUIRE(pol->hidden >= 1 && pol->hidden <= 64, "policy tower width must be <= 64");
-  if (pol->hidden <= 32) return launch_logp<32>(pol, pol_params, pol_norm, batch, ld, n, row_logp, (cudaStream_t)stream);
-  return launch_logp<64>(pol, pol_params, pol_norm, batch, ld, n, row_logp, (cudaStream_t)stream);
+  const cudaStream_t st = (cudaStream_t)stream;
+  if (pol_act == IMB_ACT_TANH)
+    return pol->hidden <= 32 ? launch_logp<32, ACT_TANH>(pol, pol_params, pol_norm, batch, ld, n, row_logp, st)
+                             : launch_logp<64, ACT_TANH>(pol, pol_params, pol_norm, batch, ld, n, row_logp, st);
+  return pol->hidden <= 32 ? launch_logp<32, ACT_RELU>(pol, pol_params, pol_norm, batch, ld, n, row_logp, st)
+                           : launch_logp<64, ACT_RELU>(pol, pol_params, pol_norm, batch, ld, n, row_logp, st);
 }
 
 #ifdef IMB_PPO_TIMING

@@ -15,6 +15,7 @@
 //     squared slice norms, run clip_grad_norm_ + Adam on their slice and store the new parameters into every CTA.
 // Three cluster barriers per optimiser step instead of the mbarrier-signalled exchange of k_ppo_update: simpler, and
 // the barriers' cost is small against steps that carry 2-32x the arithmetic.
+// ACT is the towers' activation: every ReLU policy runs here whatever its shape (k_ppo_update is tanh only).
 constexpr int RG = 16;             // minibatch rows per CTA and pass
 constexpr int GEN_MAX_MB = 4096;   // index list of one minibatch in shared memory
 
@@ -81,7 +82,18 @@ __device__ __forceinline__ float sum16(const float (&d)[16]) {
   return s0 + s1;
 }
 
-template <int U>
+// Activation of the policy towers (ACT_TANH / ACT_RELU) and its backward through the post-activation a: tanh's
+// g (1 - a^2); ReLU's g where a > 0, else 0 (torch's threshold_backward: the derivative at exactly 0 is 0).
+template <int ACT>
+__device__ __forceinline__ float ppo_act(float z) {
+  return ACT == ACT_TANH ? PPO_TANH(z) : fmaxf(z, 0.f);
+}
+template <int ACT>
+__device__ __forceinline__ float ppo_act_grad(float g, float a) {
+  return ACT == ACT_TANH ? g * (1.0f - a * a) : (a > 0.f ? g : 0.f);
+}
+
+template <int U, int PACT>  // PACT: the towers' activation (ACT names the shared-memory action tile below)
 __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float* __restrict__ g_params,
                                                           float* __restrict__ g_norm, int32_t* __restrict__ g_norm_count,
                                                           float* __restrict__ g_m, float* __restrict__ g_v,
@@ -289,7 +301,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
         for (int u = 0; u < U; ++u) {
           const float b = Pm[c_b1 + jc[u]];
 #pragma unroll
-          for (int r = 0; r < 4; ++r) h1[u][r] = jl[u] ? PPO_TANH(acc[u][r] + b) : 0.f;
+          for (int r = 0; r < 4; ++r) h1[u][r] = jl[u] ? ppo_act<PACT>(acc[u][r] + b) : 0.f;
           st4(cH1 + (lane + 32 * u) * RG + r0, make_float4(h1[u][0], h1[u][1], h1[u][2], h1[u][3]));
         }
         __syncwarp();
@@ -313,7 +325,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
           const float b = Pm[c_b2 + jc[u]];
 #pragma unroll
           for (int r = 0; r < 4; ++r) {
-            lat[u][r] = jl[u] ? PPO_TANH(acc[u][r] + b) : 0.f;
+            lat[u][r] = jl[u] ? ppo_act<PACT>(acc[u][r] + b) : 0.f;
             dl[u][r] = 0.f;
           }
           st4(cLAT + (lane + 32 * u) * RG + r0, make_float4(lat[u][0], lat[u][1], lat[u][2], lat[u][3]));
@@ -459,10 +471,10 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
 #pragma unroll
         for (int u = 0; u < U; ++u)
           st4(cDZ2 + (lane + 32 * u) * RG + r0,
-              make_float4(jl[u] ? dl[u][0] * (1.0f - lat[u][0] * lat[u][0]) : 0.f,
-                          jl[u] ? dl[u][1] * (1.0f - lat[u][1] * lat[u][1]) : 0.f,
-                          jl[u] ? dl[u][2] * (1.0f - lat[u][2] * lat[u][2]) : 0.f,
-                          jl[u] ? dl[u][3] * (1.0f - lat[u][3] * lat[u][3]) : 0.f));
+              make_float4(jl[u] ? ppo_act_grad<PACT>(dl[u][0], lat[u][0]) : 0.f,
+                          jl[u] ? ppo_act_grad<PACT>(dl[u][1], lat[u][1]) : 0.f,
+                          jl[u] ? ppo_act_grad<PACT>(dl[u][2], lat[u][2]) : 0.f,
+                          jl[u] ? ppo_act_grad<PACT>(dl[u][3], lat[u][3]) : 0.f));
         __syncwarp();
 #pragma unroll
         for (int u = 0; u < U; ++u) acc[u][0] = acc[u][1] = acc[u][2] = acc[u][3] = 0.f;
@@ -481,10 +493,10 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
 #pragma unroll
         for (int u = 0; u < U; ++u)
           st4(cDZ1 + (lane + 32 * u) * RG + r0,
-              make_float4(jl[u] ? acc[u][0] * (1.f - h1[u][0] * h1[u][0]) : 0.f,
-                          jl[u] ? acc[u][1] * (1.f - h1[u][1] * h1[u][1]) : 0.f,
-                          jl[u] ? acc[u][2] * (1.f - h1[u][2] * h1[u][2]) : 0.f,
-                          jl[u] ? acc[u][3] * (1.f - h1[u][3] * h1[u][3]) : 0.f));
+              make_float4(jl[u] ? ppo_act_grad<PACT>(acc[u][0], h1[u][0]) : 0.f,
+                          jl[u] ? ppo_act_grad<PACT>(acc[u][1], h1[u][1]) : 0.f,
+                          jl[u] ? ppo_act_grad<PACT>(acc[u][2], h1[u][2]) : 0.f,
+                          jl[u] ? ppo_act_grad<PACT>(acc[u][3], h1[u][3]) : 0.f));
       }
       __syncthreads();
       // weight gradients of the pass's RG rows, accumulated into GP (P-layout): thread = (tower, unit gj, every

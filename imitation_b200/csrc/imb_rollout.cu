@@ -1,13 +1,15 @@
 // imb_rollout.cu -- C-ABI entry points of stage 1 (kernels: imb_rollout_impl.cuh).
 #include "imb_rollout_impl.cuh"
 
+static_assert(IMB_ACT_TANH == ACT_TANH && IMB_ACT_RELU == ACT_RELU, "imb.h activation codes = the kernels' ACT_*");
+
 extern "C" int imb_rollout_row_width(const imb_policy_desc* pol) {
   return imb_row_width(pol->d_obs, pol->d_act, pol->discrete != 0);
 }
 
 // members == nullptr: imb_rollout; otherwise imb_rollout_ensemble (reward_mode 2, member m's vectors from the table)
 static int rollout_common(const imb_env_desc* env, const float* env_params, float* env_obs, const imb_policy_desc* pol,
-                          const float* pol_params, const float* pol_norm, const imb_disc_desc* disc,
+                          int pol_act, const float* pol_params, const float* pol_norm, const imb_disc_desc* disc,
                           const float* disc_params, const float* disc_norm, const imb_rollout_members* members,
                           int reward_mode, const imb_ppo_hparams* hp, int64_t n_envs, int64_t n_steps, float* rollout,
                           float* ring, int64_t ring_capacity, float* flat_out, float* aux, const float* noise, int flags,
@@ -16,6 +18,8 @@ static int rollout_common(const imb_env_desc* env, const float* env_params, floa
   IMB_REQUIRE(env->d_obs == pol->d_obs && env->d_act == pol->d_act && env->discrete == pol->discrete,
               "env / policy space mismatch");
   IMB_REQUIRE(pol->hidden >= 1 && pol->hidden <= 64, "policy tower width must be <= 64");
+  IMB_REQUIRE(pol_act == IMB_ACT_TANH || pol_act == IMB_ACT_RELU,
+              "pol_act must be IMB_ACT_TANH (0) or IMB_ACT_RELU (1), got %d", pol_act);
   IMB_REQUIRE(env->d_obs <= IMB_MAX_DIN && env->d_act <= IMB_MAX_DIN, "d_obs/d_act must be <= %d", IMB_MAX_DIN);
   RolloutArgs A;
   A.env = *env;
@@ -39,7 +43,7 @@ static int rollout_common(const imb_env_desc* env, const float* env_params, floa
   }
   cudaStream_t st = (cudaStream_t)stream;
   if (!members)
-    return launch_rollout(A, L, nullptr, env_params, env_obs, pol_params, pol_norm, disc_params, rollout, ring,
+    return launch_rollout(A, pol_act, L, nullptr, env_params, env_obs, pol_params, pol_norm, disc_params, rollout, ring,
                           flat_out, aux, noise, state, st);
   const int M = members->n_members;
   IMB_REQUIRE(M >= 2 && M <= IMB_PU_MAX_MEMBERS, "imb_rollout_ensemble: %d members (2 to %d)", M, IMB_PU_MAX_MEMBERS);
@@ -58,30 +62,30 @@ static int rollout_common(const imb_env_desc* env, const float* env_params, floa
       Mb.norm[m][p] = mlp.has_norm ? members->norm_state[m] + mlp.norm_off : nullptr;
     }
   }
-  return launch_rollout(A, L, &Mb, env_params, env_obs, pol_params, pol_norm, nullptr, rollout, ring, flat_out, aux,
-                        noise, state, st);
+  return launch_rollout(A, pol_act, L, &Mb, env_params, env_obs, pol_params, pol_norm, nullptr, rollout, ring, flat_out,
+                        aux, noise, state, st);
 }
 
 extern "C" int imb_rollout(const imb_env_desc* env, const float* env_params, float* env_obs,
-                           const imb_policy_desc* pol, const float* pol_params, const float* pol_norm,
+                           const imb_policy_desc* pol, int32_t pol_act, const float* pol_params, const float* pol_norm,
                            const imb_disc_desc* disc, const float* disc_params, const float* disc_norm,
                            int reward_mode, const imb_ppo_hparams* hp, int64_t n_envs, int64_t n_steps,
                            float* rollout, float* ring, int64_t ring_capacity, float* flat_out, float* aux,
                            const float* noise, int flags, const int64_t* state, void* stream) {
-  return rollout_common(env, env_params, env_obs, pol, pol_params, pol_norm, disc, disc_params, disc_norm, nullptr,
-                        reward_mode, hp, n_envs, n_steps, rollout, ring, ring_capacity, flat_out, aux, noise, flags,
-                        state, stream);
+  return rollout_common(env, env_params, env_obs, pol, pol_act, pol_params, pol_norm, disc, disc_params, disc_norm,
+                        nullptr, reward_mode, hp, n_envs, n_steps, rollout, ring, ring_capacity, flat_out, aux, noise,
+                        flags, state, stream);
 }
 
 extern "C" int imb_rollout_ensemble(const imb_env_desc* env, const float* env_params, float* env_obs,
-                                    const imb_policy_desc* pol, const float* pol_params, const float* pol_norm,
-                                    const imb_disc_desc* disc, const imb_rollout_members* members,
+                                    const imb_policy_desc* pol, int32_t pol_act, const float* pol_params,
+                                    const float* pol_norm, const imb_disc_desc* disc, const imb_rollout_members* members,
                                     const imb_ppo_hparams* hp, int64_t n_envs, int64_t n_steps, float* rollout,
                                     float* ring, int64_t ring_capacity, float* flat_out, float* aux, const float* noise,
                                     int flags, const int64_t* state, void* stream) {
   IMB_REQUIRE(disc && members, "imb_rollout_ensemble needs a member architecture and a member table");
-  return rollout_common(env, env_params, env_obs, pol, pol_params, pol_norm, disc, nullptr, nullptr, members, 2, hp,
-                        n_envs, n_steps, rollout, ring, ring_capacity, flat_out, aux, noise, flags, state, stream);
+  return rollout_common(env, env_params, env_obs, pol, pol_act, pol_params, pol_norm, disc, nullptr, nullptr, members, 2,
+                        hp, n_envs, n_steps, rollout, ring, ring_capacity, flat_out, aux, noise, flags, state, stream);
 }
 
 extern "C" int imb_rollout_advance(int64_t* state, int64_t n_envs, int64_t n_steps, int32_t horizon,

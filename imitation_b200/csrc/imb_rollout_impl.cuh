@@ -64,9 +64,9 @@ __device__ __forceinline__ int64_t flat_index(int64_t e, int64_t t, int64_t E, i
   return E * start + e * (end - start) + (t - start);
 }
 
-// ENS: evaluate the Mb.M ensemble members (raw outputs to Mb.raw) instead of the one net at disc_params (reward to the
-// table's reward column); the single-net variant is compiled without the member loop.
-template <int RPL, bool ENS>
+// ENS: evaluate the Mb.M ensemble members (raw outputs to Mb.raw) instead of the one net at disc_params (reward column);
+// the single-net variant has no member loop.  ACT: the policy towers' activation (env and reward net keep their own).
+template <int RPL, bool ENS, int ACT>
 __global__ void __launch_bounds__(RT, 1) k_rollout(const RolloutArgs A, const DiscLaunch L, const RolloutMembers Mb,
                                                    const float* __restrict__ env_params, float* __restrict__ env_obs,
                                                    const float* __restrict__ pol_params,
@@ -185,9 +185,9 @@ __global__ void __launch_bounds__(RT, 1) k_rollout(const RolloutArgs A, const Di
   };
   auto value_of_obs = [&](const float* __restrict__ SRC) {
     norm_obs(SRC);
-    tile_layer<ACT_TANH, RPL>(XN, Do, psm + S.w1v, HP, psm + S.b1v, H1, HP);
+    tile_layer<ACT, RPL>(XN, Do, psm + S.w1v, HP, psm + S.b1v, H1, HP);
     __syncthreads();
-    tile_layer<ACT_TANH, RPL>(H1, h, psm + S.w2v, HP, psm + S.b2v, H2, HP);
+    tile_layer<ACT, RPL>(H1, h, psm + S.w2v, HP, psm + S.b2v, H2, HP);
     __syncthreads();
     const float v = value_row();
     __syncthreads();
@@ -199,9 +199,9 @@ __global__ void __launch_bounds__(RT, 1) k_rollout(const RolloutArgs A, const Di
     float* row = rollout + (e * T + t) * rw;
     // ---- policy: value tower, then pi tower (H2 ends up holding the pi latent) ------------------------------
     const float value = value_of_obs(OBSU);
-    tile_layer<ACT_TANH, RPL>(XN, Do, psm + S.w1p, HP, psm + S.b1p, H1, HP);
+    tile_layer<ACT, RPL>(XN, Do, psm + S.w1p, HP, psm + S.b1p, H1, HP);
     __syncthreads();
-    tile_layer<ACT_TANH, RPL>(H1, h, psm + S.w2p, HP, psm + S.b2p, H2, HP);
+    tile_layer<ACT, RPL>(H1, h, psm + S.w2p, HP, psm + S.b2p, H2, HP);
     __syncthreads();
     // ---- action head + sampling, thread per env ----------------------------------------------------------------
     float logp = 0.f;
@@ -453,7 +453,7 @@ __global__ void k_env_reset(float* __restrict__ env_obs, int64_t E, int d_obs, u
 
 }  // namespace
 
-template <int RPL, bool ENS>
+template <int RPL, bool ENS, int ACT>
 static int launch_rollout_t(RolloutArgs A, const DiscLaunch& L, const RolloutMembers& Mb, const float* env_params,
                             float* env_obs, const float* pol_params, const float* pol_norm, const float* disc_params,
                             float* rollout, float* ring, float* flat_out, float* aux, const float* noise,
@@ -498,33 +498,44 @@ static int launch_rollout_t(RolloutArgs A, const DiscLaunch& L, const RolloutMem
   IMB_REQUIRE(bytes <= IMB_SMEM_MAX, "rollout kernel needs %zu B of shared memory", bytes);
   static size_t attr_bytes = 0;
   if (bytes > attr_bytes) {
-    cudaError_t e = cudaFuncSetAttribute(k_rollout<RPL, ENS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    cudaError_t e = cudaFuncSetAttribute(k_rollout<RPL, ENS, ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)bytes);
     if (e != cudaSuccess) IMB_FAIL(-2, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
     attr_bytes = bytes;
   }
   const int blocks = (int)((A.E + RR - 1) / RR);
-  k_rollout<RPL, ENS><<<blocks, RT, bytes, st>>>(A, L, Mb, env_params, env_obs, pol_params, pol_norm, disc_params,
-                                                 rollout, ring, flat_out, aux, noise, state);
+  k_rollout<RPL, ENS, ACT><<<blocks, RT, bytes, st>>>(A, L, Mb, env_params, env_obs, pol_params, pol_norm, disc_params,
+                                                      rollout, ring, flat_out, aux, noise, state);
   IMB_CHECK_LAUNCH("k_rollout");
   return 0;
 }
 
-// Mb == nullptr: the single-net rollout
-static int launch_rollout(const RolloutArgs& A, const DiscLaunch& L, const RolloutMembers* Mb, const float* env_params,
-                          float* env_obs, const float* pol_params, const float* pol_norm, const float* disc_params,
-                          float* rollout, float* ring, float* flat_out, float* aux, const float* noise,
-                          const int64_t* state, cudaStream_t st) {
+// Mb == nullptr: the single-net rollout; act: the policy towers' activation (ACT_TANH / ACT_RELU)
+template <int ACT>
+static int launch_rollout_act(const RolloutArgs& A, const DiscLaunch& L, const RolloutMembers* Mb,
+                              const float* env_params, float* env_obs, const float* pol_params, const float* pol_norm,
+                              const float* disc_params, float* rollout, float* ring, float* flat_out, float* aux,
+                              const float* noise, const int64_t* state, cudaStream_t st) {
   // smallest tile that still covers the SMs: the kernel's duration is one CTA's latency
   const int64_t sms = imb_num_sms();
   static const RolloutMembers no_members = {};
-#define IMB_RL(R)                                                                                                     \
-  return Mb ? launch_rollout_t<R, true>(A, L, *Mb, env_params, env_obs, pol_params, pol_norm, disc_params, rollout, \
-                                        ring, flat_out, aux, noise, state, st)                                      \
-            : launch_rollout_t<R, false>(A, L, no_members, env_params, env_obs, pol_params, pol_norm, disc_params,   \
-                                         rollout, ring, flat_out, aux, noise, state, st)
+#define IMB_RL(R)                                                                                                      \
+  return Mb ? launch_rollout_t<R, true, ACT>(A, L, *Mb, env_params, env_obs, pol_params, pol_norm, disc_params,       \
+                                             rollout, ring, flat_out, aux, noise, state, st)                           \
+            : launch_rollout_t<R, false, ACT>(A, L, no_members, env_params, env_obs, pol_params, pol_norm, disc_params, \
+                                              rollout, ring, flat_out, aux, noise, state, st)
   if (A.E <= sms * 8 * 2) IMB_RL(0);
   if (A.E <= sms * 32) IMB_RL(1);
   if (A.E <= sms * 64 * 2) IMB_RL(2);
   IMB_RL(4);
 #undef IMB_RL
+}
+
+static int launch_rollout(const RolloutArgs& A, int act, const DiscLaunch& L, const RolloutMembers* Mb,
+                          const float* env_params, float* env_obs, const float* pol_params, const float* pol_norm,
+                          const float* disc_params, float* rollout, float* ring, float* flat_out, float* aux,
+                          const float* noise, const int64_t* state, cudaStream_t st) {
+  auto go = act == ACT_TANH ? launch_rollout_act<ACT_TANH> : launch_rollout_act<ACT_RELU>;
+  return go(A, L, Mb, env_params, env_obs, pol_params, pol_norm, disc_params, rollout, ring, flat_out, aux, noise,
+            state, st);
 }

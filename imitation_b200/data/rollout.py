@@ -85,7 +85,8 @@ def generate_trajectories(policy, venv, sample_until: GenTrajTerminationFn, rng:
     trajectories = []
     while True:
         _lib.rollout(base.desc, base.params, base.obs, pol.desc, pp, pn, None, None, None, 0, hp, E, H, tbl, None, 0,
-                     flat, aux, None, base.state, flags=_lib.IMB_RF_DETERMINISTIC if deterministic_policy else 0)
+                     flat, aux, None, base.state, flags=_lib.IMB_RF_DETERMINISTIC if deterministic_policy else 0,
+                     act=pol.act)
         _lib.rollout_advance(base.state, E, H, H, 0)
         base.host_ep_step = 0
         rows = tbl.cpu().numpy().reshape(E, H, rw)

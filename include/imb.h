@@ -45,6 +45,9 @@ extern "C" {
 #define IMB_F_TRAIN_NORM 2   /* imb_disc_fwd_bwd: Phi(s') uses the mid-update norm snapshot */
 #define IMB_F_NO_TENSOR 4    /* imb_disc_fwd_bwd: force the fp32-FFMA kernel (A/B measurements; default = wgmma when the shape fits) */
 #define IMB_RF_DETERMINISTIC 1 /* imb_rollout flags: act = mean / argmax (policy.predict(deterministic=True)) */
+/* pol_act of the entry points that evaluate or plan a policy: the activation of both towers' hidden layers */
+#define IMB_ACT_TANH 0       /* nn.Tanh (SB3's default, imitation's FeedForward32Policy) */
+#define IMB_ACT_RELU 1       /* nn.ReLU (the reference's seals_hopper / walker / swimmer configurations) */
 
 /* One MLP: [RunningNorm?] -> Linear(din,h1) -> act -> [Linear(h1,h2) -> act] -> Linear(h_last,n_out).
  * util/networks.py:204-283 (build_mlp).  Parameter block (at `param_off` floats into the
@@ -234,14 +237,16 @@ int imb_gather_rows(const float* table, int64_t capacity, int32_t tw, const int6
 
 /* ---- stage 1: generator rollouts (GPU-resident VecEnv + policy + reward relabel) ---------- */
 
-/* Actor-critic policy (SB3 ActorCriticPolicy with separate pi / vf towers, tanh;
+/* Actor-critic policy (SB3 ActorCriticPolicy with separate pi / vf towers;
  * imitation policies/base.py:92-104 FeedForward32Policy; optional feature RunningNorm,
  * policies/base.py:123-149).  Flat parameter vector: pi tower | vf tower | action head
- * (imb_mlp with n_hidden = 0 semantics: Linear(h, d_act)) | value head | log_std[d_act]. */
+ * (imb_mlp with n_hidden = 0 semantics: Linear(h, d_act)) | value head | log_std[d_act].
+ * The towers' activation is not part of the descriptor: every entry point that evaluates or
+ * plans the policy takes it as `pol_act` (IMB_ACT_TANH or IMB_ACT_RELU; any other value is an error). */
 typedef struct imb_policy_desc {
   int32_t d_obs, d_act;     /* d_act: action dim (Box) or number of actions (Discrete) */
   int32_t discrete;
-  int32_t hidden;           /* tower width (two tanh layers of this width) */
+  int32_t hidden;           /* tower width (two layers of this width, activation pol_act) */
   int32_t has_norm;         /* NormalizeFeaturesExtractor */
   float norm_eps;
   int32_t off_pi_w1, off_pi_b1, off_pi_w2, off_pi_b2;
@@ -276,7 +281,7 @@ typedef struct imb_ppo_hparams {
  * noise (optional, [T][E][d_act] normals or [T][E] uniforms) pins sampling for parity;
  * flags: IMB_RF_DETERMINISTIC for evaluation rollouts (data/rollout.py:382-506). */
 int imb_rollout(const imb_env_desc* env, const float* env_params, float* env_obs,
-                const imb_policy_desc* pol, const float* pol_params, const float* pol_norm,
+                const imb_policy_desc* pol, int32_t pol_act, const float* pol_params, const float* pol_norm,
                 const imb_disc_desc* disc, const float* disc_params, const float* disc_norm,
                 int reward_mode, const imb_ppo_hparams* hp, int64_t n_envs, int64_t n_steps,
                 float* rollout, float* ring, int64_t ring_capacity, float* flat_out, float* aux,
@@ -303,9 +308,10 @@ int imb_env_reset(float* env_obs, int64_t n_envs, const imb_env_desc* env, const
  * entropy loss, backward, clip_grad_norm_, Adam).  Two kernels behind this entry point: k_ppo_update for tower width <= 32
  * and batch_size <= 64 (the reference's FeedForward32Policy with SB3's default minibatch: the minibatch is resident in
  * shared memory, one lane per hidden unit), k_ppo_update_gen for tower widths up to 64 (SB3 MlpPolicy 64x64) and
- * minibatches up to 4096 rows (tuned_hps airl_seals_walker: 128, airl_seals_hopper: 512).  perm == NULL -> device Feistel
+ * minibatches up to 4096 rows (tuned_hps airl_seals_walker: 128, airl_seals_hopper: 512), and for every ReLU policy
+ * (pol_act = IMB_ACT_RELU; k_ppo_update is tanh only).  perm == NULL -> device Feistel
  * permutations.  loss_log (optional) [n_steps_total][4] = pg_loss, value_loss, entropy_loss, total. */
-int imb_ppo_update(const imb_policy_desc* pol, float* pol_params, float* pol_norm,
+int imb_ppo_update(const imb_policy_desc* pol, int32_t pol_act, float* pol_params, float* pol_norm,
                    int32_t* pol_norm_count, float* exp_avg, float* exp_avg_sq,
                    const float* rollout, int64_t n_rows, const imb_ppo_hparams* hp,
                    const int64_t* perm, uint64_t seed, float* loss_log, int64_t* state,
@@ -315,10 +321,10 @@ int imb_ppo_update(const imb_policy_desc* pol, float* pol_params, float* pol_nor
  * Honours IMB_PPO_FORCE_GENERAL.  <0 (imb_last_error() names the shared-memory need and limit) when no kernel can run
  * the shape.  Shapes within k_ppo_update's width and minibatch whose shared memory or parameter slice does not fit it
  * run on k_ppo_update_gen<1>. */
-#define IMB_PPO_PLAN_UPDATE 1  /* k_ppo_update: tower width <= 32, minibatch <= 64 rows */
-#define IMB_PPO_PLAN_GEN1 2    /* k_ppo_update_gen<1>: tower width <= 32 */
+#define IMB_PPO_PLAN_UPDATE 1  /* k_ppo_update: tanh, tower width <= 32, minibatch <= 64 rows */
+#define IMB_PPO_PLAN_GEN1 2    /* k_ppo_update_gen<1>: tower width <= 32 (every ReLU policy of that width) */
 #define IMB_PPO_PLAN_GEN2 3    /* k_ppo_update_gen<2>: tower width 33 to 64 */
-int imb_ppo_plan(const imb_policy_desc* pol, int32_t batch_size);
+int imb_ppo_plan(const imb_policy_desc* pol, int32_t pol_act, int32_t batch_size);
 
 /* Which instantiation of k_ppo_update imb_ppo_update runs for `pol` when imb_ppo_plan returns IMB_PPO_PLAN_UPDATE; host
  * only.  0: the one that reads the shape at run time (every shape without its own); 1: 17 obs / 6 actions Box with a
@@ -329,7 +335,7 @@ int imb_ppo_update_variant(const imb_policy_desc* pol);
 
 /* log pi(a|s) of the generator policy for the disc batch (common.py:476-519 ->
  * ActorCriticPolicy.evaluate_actions), written into the batch's last feature row. */
-int imb_policy_logp(const imb_policy_desc* pol, const float* pol_params, const float* pol_norm,
+int imb_policy_logp(const imb_policy_desc* pol, int32_t pol_act, const float* pol_params, const float* pol_norm,
                     float* batch, int64_t ld, int64_t n, int32_t row_logp, void* stream);
 
 /* imb_disc_reduce + imb_disc_adam in one launch (last minibatch of an update; gradient taken from
@@ -403,7 +409,7 @@ typedef struct imb_rollout_members {
   float* raw;                                   /* [M][T][E] raw member outputs */
 } imb_rollout_members;
 int imb_rollout_ensemble(const imb_env_desc* env, const float* env_params, float* env_obs,
-                         const imb_policy_desc* pol, const float* pol_params, const float* pol_norm,
+                         const imb_policy_desc* pol, int32_t pol_act, const float* pol_params, const float* pol_norm,
                          const imb_disc_desc* disc, const imb_rollout_members* members,
                          const imb_ppo_hparams* hp, int64_t n_envs, int64_t n_steps, float* rollout, float* ring,
                          int64_t ring_capacity, float* flat_out, float* aux, const float* noise, int flags,
