@@ -126,6 +126,7 @@ SIGNATURES = {
     "imb_rollout": (_i32, [_env, _ptr, _ptr, _pol, _i32, _ptr, _ptr, _disc, _ptr, _ptr, _i32, _hp, _i64, _i64, _ptr,
                            _ptr, _i64, _ptr, _ptr, _ptr, _i32, _ptr, _ptr], 1),
     "imb_rollout_row_width": (_i32, [_pol], 0),
+    "imb_rollout_plan": (_i32, [_pol, _disc, _i32, _i64, _i32], 0),
     "imb_gae": (_i32, [_ptr, _i32, _i32, _i64, _i64, _ptr, _f32, _f32, _ptr, _i32, _ptr], 1),
     "imb_rollout_advance": (_i32, [_ptr, _i64, _i64, _i32, _i64, _ptr], 1),
     "imb_env_reset": (_i32, [_ptr, _i64, _env, _ptr, _ptr], 1),
@@ -389,6 +390,16 @@ def gather_rows(table, capacity, tw, idx, n, batch, ld, col0):
 
 def rollout_row_width(pol: PolicyDesc) -> int:
     return lib().imb_rollout_row_width(pol)
+
+
+def rollout_plan(pol: PolicyDesc, disc: Optional[DiscDesc], n_members: int, n_envs: int, n_sms: int = 0) -> int:
+    """Rows per CTA (8, 32, 64 or 128) `rollout` (n_members 1) or `rollout_ensemble` (2 to 16) runs for these shapes
+    over n_envs envs on n_sms SMs (<= 0: the current device's); disc None: reward_mode 0.  Host only, no GPU needed;
+    ImbError naming the shared-memory need and limit when not even the 8-row tile fits."""
+    rc = lib().imb_rollout_plan(pol, disc, n_members, n_envs, n_sms)
+    if rc < 0:
+        raise ImbError(f"imb_rollout_plan: {lib().imb_last_error().decode()} (rc={rc})")
+    return rc
 
 
 def rollout(env, env_params, env_obs, pol, pol_params, pol_norm, disc, disc_params, disc_norm, reward_mode, hp,

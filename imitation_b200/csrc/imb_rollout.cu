@@ -7,6 +7,36 @@ extern "C" int imb_rollout_row_width(const imb_policy_desc* pol) {
   return imb_row_width(pol->d_obs, pol->d_act, pol->discrete != 0);
 }
 
+// the policy and reward-net shapes k_rollout accepts
+static int check_shapes(const imb_policy_desc* pol, const imb_disc_desc* disc) {
+  IMB_REQUIRE(pol->hidden >= 1 && pol->hidden <= 64, "policy tower width must be <= 64");
+  IMB_REQUIRE(pol->d_obs >= 1 && pol->d_act >= 1 && pol->d_obs <= IMB_MAX_DIN && pol->d_act <= IMB_MAX_DIN,
+              "d_obs/d_act must be in [1, %d]", IMB_MAX_DIN);
+  IMB_REQUIRE(!disc || (disc->d_obs == pol->d_obs && disc->d_act == pol->d_act), "reward net / env space mismatch");
+  return 0;
+}
+
+extern "C" int imb_rollout_plan(const imb_policy_desc* pol, const imb_disc_desc* disc, int32_t n_members,
+                                int64_t n_envs, int32_t n_sms) {
+  IMB_REQUIRE(pol && n_envs >= 1, "rollout plan needs a policy and n_envs >= 1");
+  IMB_REQUIRE(n_members == 1 || (disc && n_members >= 2 && n_members <= IMB_PU_MAX_MEMBERS),
+              "rollout plan: %d members (1, or 2 to %d with a reward net)", n_members, IMB_PU_MAX_MEMBERS);
+  if (int rc = check_shapes(pol, disc)) return rc;
+  RolloutArgs A;
+  memset(&A, 0, sizeof(A));
+  A.env.d_obs = pol->d_obs;
+  A.env.d_act = pol->d_act;
+  A.pol = *pol;
+  A.reward_mode = disc ? 1 : 0;
+  A.E = n_envs;
+  DiscLaunch L;
+  memset(&L, 0, sizeof(L));
+  if (disc)
+    if (int rc = build_launch(disc, nullptr, nullptr, L)) return rc;
+  const int rpl = rollout_plan(A, L, n_members, n_sms > 0 ? n_sms : imb_num_sms());
+  return rpl < 0 ? rpl : rows_of(rpl);
+}
+
 // members == nullptr: imb_rollout; otherwise imb_rollout_ensemble (reward_mode 2, member m's vectors from the table)
 static int rollout_common(const imb_env_desc* env, const float* env_params, float* env_obs, const imb_policy_desc* pol,
                           int pol_act, const float* pol_params, const float* pol_norm, const imb_disc_desc* disc,
@@ -17,10 +47,9 @@ static int rollout_common(const imb_env_desc* env, const float* env_params, floa
   IMB_REQUIRE(n_envs >= 1 && n_steps >= 1, "rollout needs n_envs, n_steps >= 1");
   IMB_REQUIRE(env->d_obs == pol->d_obs && env->d_act == pol->d_act && env->discrete == pol->discrete,
               "env / policy space mismatch");
-  IMB_REQUIRE(pol->hidden >= 1 && pol->hidden <= 64, "policy tower width must be <= 64");
   IMB_REQUIRE(pol_act == IMB_ACT_TANH || pol_act == IMB_ACT_RELU,
               "pol_act must be IMB_ACT_TANH (0) or IMB_ACT_RELU (1), got %d", pol_act);
-  IMB_REQUIRE(env->d_obs <= IMB_MAX_DIN && env->d_act <= IMB_MAX_DIN, "d_obs/d_act must be <= %d", IMB_MAX_DIN);
+  if (int rc = check_shapes(pol, reward_mode != 0 ? disc : nullptr)) return rc;
   RolloutArgs A;
   A.env = *env;
   A.pol = *pol;
@@ -35,8 +64,6 @@ static int rollout_common(const imb_env_desc* env, const float* env_params, floa
   memset(&L, 0, sizeof(L));
   if (reward_mode != 0) {
     IMB_REQUIRE(disc && (disc_params || members), "reward_mode != 0 needs a reward net");
-    const int onehot = env->discrete ? env->d_act : env->d_act;
-    IMB_REQUIRE(disc->d_obs == env->d_obs && disc->d_act == onehot, "reward net / env space mismatch");
     imb_disc_desc dd = *disc;
     dd.subtract_logp = 0;  // reward_train.predict_processed never subtracts log pi (airl.py:121-124)
     if (int rc = build_launch(&dd, members ? members->norm_state[0] : disc_norm, nullptr, L)) return rc;

@@ -1,6 +1,6 @@
 // imb_rollout_impl.cuh -- stage 1 of the GAIL/AIRL round: generator rollouts, GPU resident.
 //
-// One launch runs T environment steps for E environments; a CTA owns 128 environments (= tile rows)
+// One launch runs T environment steps for E environments; a CTA owns 8 to 128 environments (= tile rows)
 // and every per-step network evaluation is a shared-memory tiled GEMM over that tile
 // (imb_tile.cuh), with the environment state, the policy, the reward network and the synthetic
 // dynamics all resident in shared memory for the whole rollout:
@@ -27,9 +27,10 @@
 namespace {
 
 constexpr int RT = 128;              // threads per CTA
-// envs (tile rows) per CTA: RR = 32 * RPL with RPL = 1, 2 or 4 rows per lane in the tiled layers; the launch picks
-// the smallest tile that still fills the GPU (1024 envs -> 32 CTAs of 32 envs: the kernel's time is one CTA's
-// latency, so smaller tiles are faster until the SMs run out); tile row stride RRS = RR + 4.
+// envs (tile rows) per CTA: RR = rows_of(RPL) = 8, 32, 64 or 128 (RPL = 0: the 8-row tile, else RPL rows per lane in
+// the tiled layers); rollout_plan picks the smallest tile that still fills the GPU (the kernel's time is one CTA's
+// latency, so smaller tiles are faster until the SMs run out), or a smaller one when that tile's shared memory does not
+// fit; tile row stride RRS = RR + 4.
 
 struct RolloutArgs {
   imb_env_desc env;
@@ -453,12 +454,11 @@ __global__ void k_env_reset(float* __restrict__ env_obs, int64_t E, int d_obs, u
 
 }  // namespace
 
-template <int RPL, bool ENS, int ACT>
-static int launch_rollout_t(RolloutArgs A, const DiscLaunch& L, const RolloutMembers& Mb, const float* env_params,
-                            float* env_obs, const float* pol_params, const float* pol_norm, const float* disc_params,
-                            float* rollout, float* ring, float* flat_out, float* aux, const float* noise,
-                            const int64_t* state, cudaStream_t st) {
-  constexpr int RR = rows_of(RPL), RRS = RR + TILE_PAD;
+// Shared-memory layout of k_rollout for a tile of rows_of(rpl) envs and n_members reward nets (A.reward_mode, A.env and
+// A.pol set): fills A's widths and offsets (floats) and returns the bytes; n_img_floats receives the reward-net images'
+// share.
+static size_t rollout_layout(RolloutArgs& A, const DiscLaunch& L, int n_members, int rpl, size_t* n_img_floats) {
+  const int RRS = rows_of(rpl) + TILE_PAD;
   auto al = [](int x) { return (x + 31) / 32 * 32; };
   const int Do = A.env.d_obs, Da = A.env.d_act;
   A.HP = A.pol.hidden <= 32 ? 32 : 64;
@@ -475,7 +475,7 @@ static int launch_rollout_t(RolloutArgs A, const DiscLaunch& L, const RolloutMem
   o += al((A.KU + 2) * A.IP);
   A.img_off = o;
   A.img_sz = al(TImg::size(dmax, A.JP));
-  const int n_img = A.reward_mode != 0 ? (ENS ? Mb.M : 1) * L.npass : 0;  // every member's images stay resident
+  const int n_img = A.reward_mode != 0 ? n_members * L.npass : 0;  // every member's images stay resident
   o += n_img * A.img_sz;
   A.obsu_off = o;
   o += al(A.KU * RRS);
@@ -490,12 +490,38 @@ static int launch_rollout_t(RolloutArgs A, const DiscLaunch& L, const RolloutMem
   A.vec_off = o;
   o += al(RT);
   A.total = o;
-  const size_t bytes = (size_t)o * 4;
-  IMB_REQUIRE(!ENS || bytes <= IMB_SMEM_MAX,
-              "rollout of a %d-member ensemble needs %zu B of shared memory (%zu B for the member images), more than "
-              "the %d B a CTA can hold: use fewer or narrower members", Mb.M, bytes, (size_t)n_img * A.img_sz * 4,
-              (int)IMB_SMEM_MAX);
-  IMB_REQUIRE(bytes <= IMB_SMEM_MAX, "rollout kernel needs %zu B of shared memory", bytes);
+  if (n_img_floats) *n_img_floats = (size_t)n_img * A.img_sz;
+  return (size_t)o * 4;
+}
+
+// The tile (rows-per-lane parameter RPL: 0, 1, 2 or 4) k_rollout runs for A.E envs on n_sms SMs, with A laid out for it.
+// Preferred: the smallest tile that still covers the SMs (the kernel's duration is one CTA's latency): <= 16 envs per
+// SM -> 8 rows, <= 32 -> 32 rows, <= 128 -> 64 rows, else 128 rows.  When the preferred tile's shared memory exceeds
+// IMB_SMEM_MAX, the next smaller tile that fits runs instead (more CTAs, each as fast); <0 when not even the 8-row tile
+// fits.
+static int rollout_plan(RolloutArgs& A, const DiscLaunch& L, int n_members, int64_t n_sms) {
+  static const int order[4] = {0, 1, 2, 4};
+  int i = A.E <= n_sms * 16 ? 0 : A.E <= n_sms * 32 ? 1 : A.E <= n_sms * 128 ? 2 : 3;
+  size_t n_img = 0, bytes = 0;
+  for (; i >= 0; --i) {
+    bytes = rollout_layout(A, L, n_members, order[i], &n_img);
+    if (bytes <= IMB_SMEM_MAX) return order[i];
+  }
+  IMB_REQUIRE(n_members <= 1,
+              "rollout of a %d-member ensemble needs %zu B of shared memory at its smallest (8-row) tile (%zu B for "
+              "the member images), more than the %d B limit of a CTA: use fewer or narrower members", n_members, bytes,
+              n_img * 4, (int)IMB_SMEM_MAX);
+  IMB_FAIL(-1, "rollout kernel needs %zu B of shared memory at its smallest (8-row) tile (%zu B for the reward-net "
+           "images), more than the %d B limit of a CTA", bytes, n_img * 4, (int)IMB_SMEM_MAX);
+}
+
+template <int RPL, bool ENS, int ACT>
+static int launch_rollout_t(const RolloutArgs& A, const DiscLaunch& L, const RolloutMembers& Mb,
+                            const float* env_params, float* env_obs, const float* pol_params, const float* pol_norm,
+                            const float* disc_params, float* rollout, float* ring, float* flat_out, float* aux,
+                            const float* noise, const int64_t* state, cudaStream_t st) {
+  constexpr int RR = rows_of(RPL);
+  const size_t bytes = (size_t)A.total * 4;
   static size_t attr_bytes = 0;
   if (bytes > attr_bytes) {
     cudaError_t e = cudaFuncSetAttribute(k_rollout<RPL, ENS, ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -512,21 +538,21 @@ static int launch_rollout_t(RolloutArgs A, const DiscLaunch& L, const RolloutMem
 
 // Mb == nullptr: the single-net rollout; act: the policy towers' activation (ACT_TANH / ACT_RELU)
 template <int ACT>
-static int launch_rollout_act(const RolloutArgs& A, const DiscLaunch& L, const RolloutMembers* Mb,
+static int launch_rollout_act(RolloutArgs A, const DiscLaunch& L, const RolloutMembers* Mb,
                               const float* env_params, float* env_obs, const float* pol_params, const float* pol_norm,
                               const float* disc_params, float* rollout, float* ring, float* flat_out, float* aux,
                               const float* noise, const int64_t* state, cudaStream_t st) {
-  // smallest tile that still covers the SMs: the kernel's duration is one CTA's latency
-  const int64_t sms = imb_num_sms();
+  const int rpl = rollout_plan(A, L, Mb ? Mb->M : 1, imb_num_sms());
+  if (rpl < 0) return rpl;
   static const RolloutMembers no_members = {};
 #define IMB_RL(R)                                                                                                      \
   return Mb ? launch_rollout_t<R, true, ACT>(A, L, *Mb, env_params, env_obs, pol_params, pol_norm, disc_params,       \
                                              rollout, ring, flat_out, aux, noise, state, st)                           \
             : launch_rollout_t<R, false, ACT>(A, L, no_members, env_params, env_obs, pol_params, pol_norm, disc_params, \
                                               rollout, ring, flat_out, aux, noise, state, st)
-  if (A.E <= sms * 8 * 2) IMB_RL(0);
-  if (A.E <= sms * 32) IMB_RL(1);
-  if (A.E <= sms * 64 * 2) IMB_RL(2);
+  if (rpl == 0) IMB_RL(0);
+  if (rpl == 1) IMB_RL(1);
+  if (rpl == 2) IMB_RL(2);
   IMB_RL(4);
 #undef IMB_RL
 }

@@ -291,6 +291,13 @@ int imb_rollout(const imb_env_desc* env, const float* env_params, float* env_obs
  * aux needs 2*E + 2*E*T floats (V(last obs), last done, per-step time-limit bootstrap,
  * per-step ground-truth env reward). */
 int imb_rollout_row_width(const imb_policy_desc* pol);
+/* Rows per CTA (8, 32, 64 or 128) imb_rollout / imb_rollout_ensemble run for these shapes; host only, no GPU needed.
+ * disc == NULL: reward_mode 0; n_members 1: imb_rollout, 2..16: imb_rollout_ensemble; n_sms <= 0: the current device's
+ * SM count.  The preferred tile is the smallest that covers the SMs (<= 16 envs per SM: 8 rows, <= 32: 32, <= 128: 64,
+ * else 128); when its shared memory exceeds what a CTA can hold, the next smaller tile that fits runs instead.  <0
+ * (imb_last_error() names the shared-memory need and the limit) when not even the 8-row tile fits. */
+int imb_rollout_plan(const imb_policy_desc* pol, const imb_disc_desc* disc, int32_t n_members, int64_t n_envs,
+                     int32_t n_sms);
 /* GAE over the rollout table once rewards are final (SB3 RolloutBuffer.compute_returns_and_
  * advantage); call BEFORE imb_rollout_advance (it needs the pre-rollout episode step). */
 int imb_gae(float* rollout, int32_t rw, int32_t col_value, int64_t n_envs, int64_t n_steps,
