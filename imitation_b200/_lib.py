@@ -93,6 +93,11 @@ class SyncDesc(C.Structure):
 PLAN_TC, PLAN_FFMA128X2, PLAN_FFMA256, PLAN_FFMA128 = 1, 2, 3, 4
 # imb_ppo_plan codes: the kernel imb_ppo_update runs
 PPO_PLAN_UPDATE, PPO_PLAN_GEN1, PPO_PLAN_GEN2 = 1, 2, 3
+# imb_ppo_update_ex: indices of the training statistics vector (PPO_STAT_FLOATS floats)
+PPO_STAT_ENTROPY_LOSS, PPO_STAT_PG_LOSS, PPO_STAT_VALUE_LOSS, PPO_STAT_APPROX_KL = 0, 1, 2, 3
+PPO_STAT_CLIP_FRACTION, PPO_STAT_LOSS, PPO_STAT_EXPLAINED_VARIANCE, PPO_STAT_STD = 4, 5, 6, 7
+PPO_STAT_N_UPDATES, PPO_STAT_N_STEPS, PPO_STAT_N_EPOCHS, PPO_STAT_STOPPED = 8, 9, 10, 11
+PPO_STAT_FLOATS = 16
 # imb_pref_uncertainty modes
 PU_MODES = {"logit": 0, "probability": 1, "label": 2}
 
@@ -132,6 +137,8 @@ SIGNATURES = {
     "imb_env_reset": (_i32, [_ptr, _i64, _env, _ptr, _ptr], 1),
     "imb_ppo_update": (_i32, [_pol, _i32, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _i64, _hp, _ptr, _u64, _ptr, _ptr, _ptr],
                        1),
+    "imb_ppo_update_ex": (_i32, [_pol, _i32, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _i64, _hp, _f32, _f32, _ptr, _u64, _ptr,
+                                 _ptr, _ptr, _ptr], 1),
     "imb_ppo_plan": (_i32, [_pol, _i32, _i32], 0),
     "imb_ppo_update_variant": (_i32, [_pol], 0),
     "imb_policy_logp": (_i32, [_pol, _i32, _ptr, _ptr, _ptr, _i64, _i64, _i32, _ptr], 1),
@@ -465,6 +472,20 @@ def ppo_update(pol, params, norm, norm_count, exp_avg, exp_avg_sq, rollout_tbl, 
     _check(lib().imb_ppo_update(pol, act, _p(params, th.float32), _p(norm), _p(norm_count), _p(exp_avg, th.float32),
                                 _p(exp_avg_sq, th.float32), _p(rollout_tbl, th.float32), n_rows, hp, _p(perm), seed,
                                 _p(loss_log), _p(state, th.int64), _stream()), "imb_ppo_update")
+
+
+def ppo_update_ex(pol, params, norm, norm_count, exp_avg, exp_avg_sq, rollout_tbl, n_rows, hp, perm, seed, loss_log,
+                  state, target_kl=None, clip_range_vf=None, stats=None, act=ACT_TANH):
+    """`ppo_update` with SB3's target_kl / clip_range_vf (None: off) and the training statistics written to `stats`
+    (float32 [PPO_STAT_FLOATS] CUDA tensor, indices PPO_STAT_*; None: not computed)."""
+    if stats is not None and stats.numel() < PPO_STAT_FLOATS:
+        raise ImbError(f"the PPO statistics vector needs {PPO_STAT_FLOATS} floats")
+    _check(lib().imb_ppo_update_ex(pol, act, _p(params, th.float32), _p(norm), _p(norm_count), _p(exp_avg, th.float32),
+                                   _p(exp_avg_sq, th.float32), _p(rollout_tbl, th.float32), n_rows, hp,
+                                   0.0 if target_kl is None else float(target_kl),
+                                   0.0 if clip_range_vf is None else float(clip_range_vf), _p(perm), seed,
+                                   _p(loss_log), _p(stats, th.float32), _p(state, th.int64), _stream()),
+           "imb_ppo_update_ex")
 
 
 def ppo_plan(pol: PolicyDesc, batch_size: int, act: int = ACT_TANH) -> int:

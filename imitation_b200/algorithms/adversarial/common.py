@@ -170,6 +170,12 @@ class AdversarialTrainer(base.DemonstrationAlgorithm):
         self.venv_train = self.venv_wrapped
         self.gen_algo.set_env(self.venv_train)
         self.gen_algo.set_logger(self.logger)
+        # The generator's PPO statistics (train/approx_kl, ...) are read back at the end of the round in `train()`,
+        # not inside `gen_algo.learn`: the read waits for the PPO update, which train_gen() / train_disc() never do
+        # (GAIL's discriminator updates run beside it).  They land under the "gen" prefix of the round's dump.
+        if hasattr(self.gen_algo, "record_in_learn"):
+            self.gen_algo.record_in_learn = False
+        self._gen_stats_pending = False
 
         if gen_train_timesteps is None:
             env = self.gen_algo.get_env()
@@ -751,6 +757,7 @@ class AdversarialTrainer(base.DemonstrationAlgorithm):
             self.gen_algo.learn(total_timesteps=total_timesteps, reset_num_timesteps=False,
                                 callback=self.gen_callback, **(learn_kwargs or {}))
             self._global_step += 1
+        self._gen_stats_pending = hasattr(self.gen_algo, "record_train_stats")
         ep_lens = list(self.venv_buffering._ep_lens)
         self.venv_buffering.discard()  # the samples were consumed by the fused ring store
         self._check_fixed_horizon(ep_lens)
@@ -767,6 +774,16 @@ class AdversarialTrainer(base.DemonstrationAlgorithm):
                     self.train_disc()
             if self._pn_pending:
                 self.join()
+            self._record_gen_stats()
             if callback:
                 callback(r)
             self.logger.dump(self._global_step)
+
+    def _record_gen_stats(self) -> None:
+        """The last train_gen()'s PPO statistics under the "gen" prefix (raw/gen/train/*, mean/gen/train/*), as
+        SB3's PPO.train records them inside `accumulate_means("gen")`.  Waits for that PPO update."""
+        if not self._gen_stats_pending:
+            return
+        self._gen_stats_pending = False
+        with self.logger.accumulate_means("gen"):
+            self.gen_algo.record_train_stats(self.logger)

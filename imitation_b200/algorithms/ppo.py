@@ -7,7 +7,15 @@ constructor arguments and the attributes the trainers read (`policy`, `n_steps`,
 `set_env`, `get_env`, `set_logger`, `logger`, `num_timesteps`) and runs both halves of `learn`
 as kernels: one rollout launch (csrc/imb_rollout.cu) and one persistent PPO-update launch
 (csrc/imb_ppo.cu).  Arithmetic follows SB3 2.2.x (oracle/ppo_port.py).
+
+SB3's `target_kl` (early stop of `train()` on the approximate KL) and `clip_range_vf` (clipped value loss) run inside
+the PPO kernel, and so do the statistics `PPO.train` records (`train/entropy_loss`, `policy_gradient_loss`,
+`value_loss`, `approx_kl`, `clip_fraction`, `loss`, `explained_variance`, `std`, `n_updates`, `clip_range`,
+`learning_rate`, `clip_range_vf`).  Their semantics restate SB3 2.2.1 `PPO.train` as oracle/ppo_port.py does; SB3 is not
+installed here, so this parity is unpinned, like the rest of the PPO port.
 """
+import math
+
 from typing import Optional
 
 import torch as th
@@ -24,7 +32,15 @@ class DevicePPO:
                  n_epochs: int = 10, gamma: float = 0.99, gae_lambda: float = 0.95, clip_range: float = 0.2,
                  normalize_advantage: bool = True, ent_coef: float = 0.0, vf_coef: float = 0.5,
                  max_grad_norm: float = 0.5, policy_kwargs: Optional[dict] = None, seed: Optional[int] = None,
-                 device="cuda", sampling: str = "device", **unused):
+                 device="cuda", sampling: str = "device", target_kl: Optional[float] = None,
+                 clip_range_vf: Optional[float] = None, **unused):
+        if clip_range_vf is not None and not float(clip_range_vf) > 0:  # SB3 PPO._setup_model asserts the same
+            raise ValueError("`clip_range_vf` must be positive, pass `None` to deactivate vf clipping")
+        if target_kl is not None and not float(target_kl) > 0:
+            raise ValueError("`target_kl` must be positive, pass `None` to train every epoch")
+        self.target_kl = None if target_kl is None else float(target_kl)
+        self.clip_range_vf = None if clip_range_vf is None else float(clip_range_vf)
+        self.learning_rate, self.clip_range = learning_rate, clip_range
         self.device = th.device(device)
         self.n_steps, self.batch_size, self.n_epochs = int(n_steps), int(batch_size), int(n_epochs)
         self._user_seed = None if seed is None else int(seed)  # SB3: the global RNGs are seeded only when a seed is given
@@ -57,6 +73,11 @@ class DevicePPO:
         n = self.policy.desc.n_params
         self.exp_avg = th.zeros(n, device=self.device)
         self.exp_avg_sq = th.zeros(n, device=self.device)
+        # training statistics of the last train() (_lib.PPO_STAT_* order), written by the PPO kernel itself
+        self.train_stats = th.full((_lib.PPO_STAT_FLOATS,), math.nan, device=self.device)
+        # learn() records them after its last train(), like SB3; AdversarialTrainer turns this off and records them
+        # at the end of its round, so that train_gen() never waits for the PPO update
+        self.record_in_learn = True
         self._tbl = None
         self._aux = None
         self._ens_raw = None      # ensemble reward: the members' raw rewards [M][T][E]
@@ -171,14 +192,42 @@ class DevicePPO:
         pol = self.policy
         pp, pn, pc = pol.flat_vectors()
         N = self._tbl.shape[0]
-        _lib.ppo_update(pol.desc, pp, pn, pc, self.exp_avg, self.exp_avg_sq, self._tbl, N, self.hp, self.perm,
-                        self.seed, self.loss_log, self._base_env.state, act=pol.act)
+        _lib.ppo_update_ex(pol.desc, pp, pn, pc, self.exp_avg, self.exp_avg_sq, self._tbl, N, self.hp, self.perm,
+                           self.seed, self.loss_log, self._base_env.state, target_kl=self.target_kl,
+                           clip_range_vf=self.clip_range_vf, stats=self.train_stats, act=pol.act)
+
+    def read_train_stats(self) -> dict:
+        """The statistics of the last train() as SB3's PPO.train records them (key -> float; waits for that update)."""
+        s = self.train_stats.cpu().tolist()
+        out = {"train/entropy_loss": s[_lib.PPO_STAT_ENTROPY_LOSS],
+               "train/policy_gradient_loss": s[_lib.PPO_STAT_PG_LOSS],
+               "train/value_loss": s[_lib.PPO_STAT_VALUE_LOSS],
+               "train/approx_kl": s[_lib.PPO_STAT_APPROX_KL],
+               "train/clip_fraction": s[_lib.PPO_STAT_CLIP_FRACTION],
+               "train/loss": s[_lib.PPO_STAT_LOSS],
+               "train/explained_variance": s[_lib.PPO_STAT_EXPLAINED_VARIANCE]}
+        if not self.policy.discrete:
+            out["train/std"] = s[_lib.PPO_STAT_STD]
+        out["train/n_updates"] = int(s[_lib.PPO_STAT_N_UPDATES])
+        out["train/clip_range"] = float(self.clip_range)
+        if self.clip_range_vf is not None:
+            out["train/clip_range_vf"] = self.clip_range_vf
+        out["train/learning_rate"] = float(self.learning_rate)
+        return out
+
+    def record_train_stats(self, logger=None) -> None:
+        """Record the last train()'s statistics (read_train_stats) on `logger` (default: this algorithm's)."""
+        lg = self._logger if logger is None else logger
+        for k, v in self.read_train_stats().items():
+            lg.record(k, v, exclude="tensorboard" if k == "train/n_updates" else None)
 
     def _pointer_key(self):
         """Everything a captured graph bakes in: device pointers of the vectors the kernels touch."""
         pp, pn, pc = self.policy.flat_vectors()
         key = [pp.data_ptr(), pn.data_ptr(), pc.data_ptr(), self._tbl.data_ptr() if self._tbl is not None else 0,
-               self.n_steps, id(self._rw_wrapper), id(self._buffering)]
+               self.n_steps, id(self._rw_wrapper), id(self._buffering),
+               # launch arguments of the PPO update
+               self.target_kl, self.clip_range_vf, self.train_stats.data_ptr()]
         if self._rw_wrapper is not None:
             net, mode, out_norm = self._rw_wrapper.resolve()
             if isinstance(net, reward_wrapper.EnsembleRelabel):
@@ -249,6 +298,8 @@ class DevicePPO:
                 callback.on_rollout_start()
             self._iteration()
             done += per
+        if self.record_in_learn and done > 0:
+            self.record_train_stats()
         return self
 
     def predict(self, observation, state=None, episode_start=None, deterministic=False):

@@ -56,6 +56,8 @@ struct PpoArgs {
   uint64_t seed;
   int HP, KP, S;  // tower width / obs width padded to 32; padded-layout parameters per slice (multiple of 4)
   int RS2;        // staged row stride in shared memory: >= rw, = 4 (mod 8)
+  float target_kl, clip_vf;  // SB3 PPO target_kl / clip_range_vf; <= 0: off
+  float* stats;              // IMB_PPO_STAT_* of the launch, or NULL
 };
 
 // Padded parameter layout used inside the kernel ("P-layout"): W1 rows have stride ldo = d_obs|1 and W2 rows
@@ -160,6 +162,146 @@ __device__ __forceinline__ void load8(float (&d)[8], const float* __restrict__ p
 }
 __device__ __forceinline__ float sum8(const float (&d)[8]) {
   return ((d[0] + d[1]) + (d[2] + d[3])) + ((d[4] + d[5]) + (d[6] + d[7]));
+}
+
+// ---- training statistics of PPO.train (imb_ppo_update_ex: stats_out, target_kl) -----------------------------------
+// Both kernels keep them in shared memory, out of the chain warps' registers.  Per step, the lanes that own a row's loss
+// terms write them into per-row slots RSL[term][row] of their CTA; ONE thread per CTA folds the slots of the step, in
+// row order and scaled by the step's 1 / nb, into the CTA's accumulators ACC; at the end of the launch CTA 0 sums the
+// CL accumulators in rank order.  Per-row terms (dead rows 0):
+enum { RS_PG = 0, RS_V, RS_ENT, RS_CLIP, RS_KL, RS_N };  // -min(surrogates), value error^2, -entropy, |r - 1| > clip, KL
+// CTA accumulators: sums over the steps evaluated; the KL over the steps of the current epoch; the last step's losses
+enum { AC_PG = 0, AC_V, AC_ENT, AC_CLIP, AC_KL_EPOCH, AC_LAST_PG, AC_LAST_V, AC_LAST_ENT, AC_N };
+
+template <int NR>
+__device__ __forceinline__ void ppo_stats_fold(float* __restrict__ acc, const float* __restrict__ rsl, const float inv_nb,
+                                               const bool epoch_start) {
+  // (one term at a time; RS_PG .. RS_CLIP share their indices with AC_PG .. AC_CLIP)
+#pragma unroll 1
+  for (int k = 0; k < RS_N; ++k) {
+    float t = 0.f;
+#pragma unroll
+    for (int r = 0; r < NR; ++r) t += rsl[k * NR + r];
+    t *= inv_nb;
+    if (k == RS_KL) {
+      acc[AC_KL_EPOCH] = epoch_start ? t : acc[AC_KL_EPOCH] + t;
+    } else {
+      acc[k] += t;
+      if (k < RS_CLIP) acc[AC_LAST_PG + k] = t;  // the last step's losses
+    }
+  }
+}
+
+// k_ppo_update's fold, by one whole warp (the chain's RL = 8 rows): lane = (term lane / 8, row lane % 8) for the first
+// four terms, the KL term's rows on every 8-lane group again; 8-lane butterfly sums, lane 0 updates the accumulators.
+__device__ __forceinline__ void ppo_stats_fold_warp(float* __restrict__ acc, const float* __restrict__ rsl,
+                                                    const float inv_nb, const bool epoch_start, const int lane) {
+  static_assert(RS_CLIP == 3 && RS_KL == 4 && RL == 8, "fold layout");
+  const float a = group8_sum(rsl[lane]), kl = group8_sum(rsl[RS_KL * RL + (lane & 7)]) * inv_nb;
+  const float s_v = __shfl_sync(0xffffffffu, a, 8), s_ent = __shfl_sync(0xffffffffu, a, 16);
+  const float s_clip = __shfl_sync(0xffffffffu, a, 24);
+  if (lane == 0) {
+    const float pg = a * inv_nb, v = s_v * inv_nb, ent = s_ent * inv_nb;
+    acc[AC_PG] += pg;
+    acc[AC_V] += v;
+    acc[AC_ENT] += ent;
+    acc[AC_CLIP] += s_clip * inv_nb;
+    acc[AC_KL_EPOCH] = epoch_start ? kl : acc[AC_KL_EPOCH] + kl;
+    acc[AC_LAST_PG] = pg;
+    acc[AC_LAST_V] = v;
+    acc[AC_LAST_ENT] = ent;
+  }
+}
+
+// This CTA's share of the step's approx-KL (the target_kl test): its rows' KL terms in row order, times 1 / nb.
+template <int NR>
+__device__ __forceinline__ float ppo_kl_part(const float* __restrict__ rsl, const float inv_nb) {
+  float t = 0.f;
+#pragma unroll
+  for (int r = 0; r < NR; ++r) t += rsl[RS_KL * NR + r];
+  return t * inv_nb;
+}
+
+// Explained variance of the rollout (SB3 explained_variance(values, returns)): this CTA's sums over rows crank * PT + tid
+// (stride CL * PT) of y = ret and e = ret - value (e rounded in fp32 like SB3's), both shifted by row 0's value so that a
+// constant column gives a variance of exactly 0, in double; ev[4] = sum dy, sum dy^2, sum de, sum de^2 (thread 0 stores
+// it).  All PT threads call it.  wred: PT / 32 doubles of shared memory.
+__device__ __noinline__ void ppo_ev_partial(const float* __restrict__ rollout, const int64_t N, const int rw,
+                                            const int col_val, const int col_ret, const int crank, double* ev,
+                                            double* wred) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const double y0 = rollout[col_ret], e0 = rollout[col_ret] - rollout[col_val];
+  double s[4] = {0.0, 0.0, 0.0, 0.0};
+  for (int64_t i = (int64_t)crank * PT + tid; i < N; i += (int64_t)CL * PT) {
+    const float y = rollout[i * rw + col_ret], e = y - rollout[i * rw + col_val];
+    const double dy = (double)y - y0, de = (double)e - e0;
+    s[0] += dy;
+    s[1] += dy * dy;
+    s[2] += de;
+    s[3] += de * de;
+  }
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    double v = s[k];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    __syncthreads();
+    if (lane == 0) wred[warp] = v;
+    __syncthreads();
+    if (tid == 0) {
+      double t = 0.0;
+#pragma unroll
+      for (int w = 0; w < PT / 32; ++w) t += wred[w];
+      ev[k] = t;
+    }
+  }
+}
+
+// End of the launch, thread 0 of every CTA: its accumulators and explained-variance partials go to CTA 0's `box`
+// ([CL][16] floats of shared memory no longer in use, 8-byte aligned) with remote stores; a cluster barrier follows.
+template <typename Cluster>
+__device__ __forceinline__ void ppo_stats_push(Cluster& cluster, float* box, const float* acc, const double* ev,
+                                               const int crank) {
+  float* dst = cluster.map_shared_rank(box, 0) + crank * 16;
+#pragma unroll
+  for (int k = 0; k < AC_N; ++k) dst[k] = acc[k];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) reinterpret_cast<double*>(dst + 8)[k] = ev[k];
+}
+
+// CTA 0, one thread, after that barrier: the CL accumulators and explained-variance partials summed in rank order ->
+// stats[IMB_PPO_STAT_*].  n_eval: optimiser steps evaluated (a target_kl stop included); n_epochs: epochs begun; spe:
+// steps per epoch; std: mean exp(log_std) of the final policy (NaN: Discrete).
+__device__ __noinline__ void ppo_stats_finish(const float* box, float* __restrict__ stats, const PpoArgs& A,
+                                              const int64_t n_eval, const int64_t n_epochs, const int64_t spe,
+                                              const float std, const int64_t n_updates, const bool stopped) {
+  float acc[AC_N];
+  double ev[4] = {0.0, 0.0, 0.0, 0.0};
+#pragma unroll
+  for (int k = 0; k < AC_N; ++k) acc[k] = 0.f;
+  for (int c = 0; c < CL; ++c) {  // fixed order: deterministic
+    const float* a = box + c * 16;
+    const double* e = reinterpret_cast<const double*>(box + c * 16 + 8);
+#pragma unroll
+    for (int k = 0; k < AC_N; ++k) acc[k] += a[k];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) ev[k] += e[k];
+  }
+  const float ne = (float)n_eval;
+  stats[IMB_PPO_STAT_ENTROPY_LOSS] = acc[AC_ENT] / ne;
+  stats[IMB_PPO_STAT_PG_LOSS] = acc[AC_PG] / ne;
+  stats[IMB_PPO_STAT_VALUE_LOSS] = acc[AC_V] / ne;
+  stats[IMB_PPO_STAT_APPROX_KL] = acc[AC_KL_EPOCH] / (float)((n_eval - 1) % spe + 1);
+  stats[IMB_PPO_STAT_CLIP_FRACTION] = acc[AC_CLIP] / ne;
+  stats[IMB_PPO_STAT_LOSS] = acc[AC_LAST_PG] + A.hp.ent_coef * acc[AC_LAST_ENT] + A.hp.vf_coef * acc[AC_LAST_V];
+  const double n = (double)A.n_rows;
+  const double var_y = ev[1] / n - (ev[0] / n) * (ev[0] / n), var_e = ev[3] / n - (ev[2] / n) * (ev[2] / n);
+  stats[IMB_PPO_STAT_EXPLAINED_VARIANCE] = var_y == 0.0 ? __int_as_float(0x7fc00000) : (float)(1.0 - var_e / var_y);
+  stats[IMB_PPO_STAT_STD] = std;
+  stats[IMB_PPO_STAT_N_UPDATES] = (float)n_updates;
+  stats[IMB_PPO_STAT_N_STEPS] = (float)n_eval;
+  stats[IMB_PPO_STAT_N_EPOCHS] = (float)n_epochs;
+  stats[IMB_PPO_STAT_STOPPED] = stopped ? 1.f : 0.f;
 }
 
 // Weight gradients of ONE tower over the CTA's RL = 8 rows -> GP (P-layout, local shared memory), by NQ warps: thread =
@@ -276,8 +418,9 @@ __device__ __forceinline__ void tower_wgrad(const int tnet, const int gj, const 
 // HP), whose loop bounds, layout offsets and slice geometry are compile-time constants -- the loops of the step unroll
 // completely and every shared-memory address is an immediate offset, instead of unrolled blocks plus guarded remainder
 // iterations that expose a shared-memory latency on the dependent FMA chain at every block boundary.  The arithmetic and
-// its order are the same in every instantiation.  DO = 0: the shape is read from A.pol (every other shape).
-template <int HP, int DO = 0, int DA = 0, int DISC = 0, int NORM = 0>
+// its order are the same in every instantiation.  DO = 0: the shape is read from A.pol (every other shape).  OPT = 0:
+// target_kl and clip_range_vf are off, and their code is not compiled in (the step is the one without them).
+template <int HP, int DO = 0, int DA = 0, int DISC = 0, int NORM = 0, int OPT = 0>
 __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __restrict__ g_params,
                                                       float* __restrict__ g_norm, int32_t* __restrict__ g_norm_count,
                                                       float* __restrict__ g_m, float* __restrict__ g_v,
@@ -295,6 +438,14 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
   __shared__ __align__(8) uint64_t xbar[3];  // [0]: partial gradients of the owned slice arrived; [1]: all new parameter slices; [2]: all slice norms
   __shared__ float SSQ[CL];                  // squared gradient norms of the 8 slices (each written by its owner)
   __shared__ float nred[PT / 32];            // per-warp partial sums of the owned slice's squared norm
+  // training statistics (see ppo_stats_fold) and target_kl: per-row slots of the step, accumulators, the CTAs' KL shares
+  // of the step (they travel with SSQ), the stopping step + 1 (0: none), explained-variance partials
+  __shared__ float RSL[RS_N * RL];
+  __shared__ float ACC[AC_N];
+  __shared__ float KLS[CL];
+  __shared__ int KSTOP;
+  __shared__ double EVP[4];
+  __shared__ double EVW[PT / 32];
   const imb_policy_desc& pd = A.pol;
   constexpr bool SPEC = DO != 0;
   const int Do = SPEC ? DO : pd.d_obs, Da = SPEC ? DA : pd.d_act, h = SPEC ? HP : pd.hidden, NP = pd.n_params;
@@ -318,6 +469,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
   // rollout row width (multiple of 4) / staged row stride (= 4 mod 8)
   const int rw = SPEC ? imb_row_width(Do, Da, discrete) : A.rw, RS2 = SPEC ? ppo_row_stride(rw) : A.RS2;
   auto al = [](int x) { return (x + 31) / 32 * 32; };
+  const bool kl_on = OPT && A.target_kl > 0.f, vf_on = OPT && A.clip_vf > 0.f;  // (uniform)
 
   // ---- shared-memory carve-up (identical in every CTA: DSMEM addresses are rank + offset) ---------------
   int o = 0;
@@ -351,7 +503,10 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
     rstat[64 + tid] = (has_norm && tid < Do) ? g_norm[Do + tid] : 1.f;
     LOSS[tid & 31] = 0.f;
   }
+  if (tid < RS_N * RL) RSL[tid] = 0.f;
+  if (tid < AC_N) ACC[tid] = 0.f;
   if (tid == 0) {
+    KSTOP = 0;
     mbar_init(&mbar[0], nst);
     mbar_init(&mbar[1], nst);
     mbar_init(&mbar[2], nst);
@@ -459,6 +614,12 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
           var *= itot;
           istd = rsqrtf(var + pd.norm_eps);
           if (gl == 0) {
+            if (kl_on && crank == 0 && gs2 > 0) {
+              // target_kl: the statistics of step gs2 - 1 go out now -- if that step stops the training, they are the
+              // result, and these are computed before the decision (the write-back skips rstat then)
+              g_norm[task] = rstat[task];
+              g_norm[Do + task] = rstat[64 + task];
+            }
             rstat[task] = mean;
             rstat[64 + task] = var;
           }
@@ -479,6 +640,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
   __syncthreads();
   issue_gather(0, 0, 0);
   if (n_steps > 1) issue_gather(mb >= Ni ? 1 : 0, mb >= Ni ? 0 : mb, 1);
+  if (A.stats) ppo_ev_partial(rollout, N, rw, col_logp + 1, col_ret, crank, EVP, EVW);  // (while the first rows land)
   minibatch_stats(0, min(mb, Ni), tid >> 3, PT / 8);
   if (has_norm) run_count += min(mb, Ni);  // (every thread keeps the count; the statistics' owners use it)
   // The gradient exchange is synchronised by the data itself: every 16-byte DSMEM store (st.async) completes
@@ -492,10 +654,11 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
   const unsigned qmagic = (unsigned)(0x100000000ull / (unsigned)(S / 4)) + 1u;  // exact quotient; S / 4 >= 2 (host)
   const uint32_t recv_sa = smem_u32(RECV), pm_sa = smem_u32(Pm), ssq_sa = smem_u32(SSQ);
   const uint32_t xbar0_sa = smem_u32(&xbar[0]), xbar1_sa = smem_u32(&xbar[1]), xbar2_sa = smem_u32(&xbar[2]);
+  const uint32_t nbytes = (uint32_t)(CL * 4 * (kl_on ? 2 : 1));  // slice norms (+ the KL shares with target_kl)
   if (tid == 0) {
     mbar_expect_tx(&xbar[0], xbytes);
     mbar_expect_tx(&xbar[1], xbytes);
-    mbar_expect_tx(&xbar[2], (uint32_t)(CL * 4));
+    mbar_expect_tx(&xbar[2], nbytes);
   }
   cluster.sync();
 
@@ -523,6 +686,13 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
       bc[2 * cur + 1] = (float)sqrt(1.0 - b2pow);
     }
     __syncthreads();  // the parameters written by the previous step's Adam (and XNo, the statistics) are visible
+    if (kl_on && KSTOP) {
+      // target_kl stopped the previous step: drain the row prefetch it issued for this step's successor, take back the
+      // count this step's statistics (computed ahead) added, and leave together
+      if (tid >= st0 && gs + 1 < n_steps) mbar_wait(&mbar[(int)((gs + 1) % 3)], (uint32_t)(((gs + 1) / 3) & 1));
+      if (has_norm) run_count -= min(mb, Ni - start);
+      break;
+    }
     PPO_TICK(0);
 #ifdef IMB_PPO_TIMING
     const long long wclk0 = clock64();
@@ -638,11 +808,20 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
         float kk = up8 ? k1 : k0;
         kk += __shfl_xor_sync(0xffffffffu, up8 ? k0 : k1, 8);
         const float val = oct_sum(kk) + Pm[PL.bv];
-        const float dv = val - row[col_ret];
-        const float dval = live ? A.hp.vf_coef * 2.0f * dv * inv_nb : 0.f;
+        float dv;
+        bool vin = true;  // clip_range_vf: the clamp passes the gradient (torch's clamp backward: edges included)
+        if (vf_on) {
+          const float vold = row[col_logp + 1], dvo = val - vold;
+          dv = (vold + fminf(fmaxf(dvo, -A.clip_vf), A.clip_vf)) - row[col_ret];
+          vin = dvo >= -A.clip_vf && dvo <= A.clip_vf;
+        } else {
+          dv = val - row[col_ret];
+        }
+        const float dval = (live && vin) ? A.hp.vf_coef * 2.0f * dv * inv_nb : 0.f;
         if (la == 0) {
           if (live) l_v = dv * dv;
           DVAL[r0 + rr] = dval;
+          RSL[RS_V * RL + r0 + rr] = live ? dv * dv : 0.f;
         }
         dl0 = __shfl_sync(0xffffffffu, dval, 0) * wvj;
         dl1 = __shfl_sync(0xffffffffu, dval, 8) * wvj;
@@ -727,7 +906,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
         }
         logp = oct_sum(logp);
         PPO_WCLK(6);
-        if (discrete || loss_log) ent = oct_sum(ent);  // (Gaussian: the entropy only feeds the loss log)
+        ent = oct_sum(ent);  // (Gaussian: the entropy only feeds the loss log and the statistics)
         const float ratio = __expf(logp - logp_old);
         const float lo = 1.0f - A.hp.clip_range, hi = 1.0f + A.hp.clip_range;
         const float pl1 = adv * ratio, pl2 = adv * fminf(fmaxf(ratio, lo), hi);
@@ -742,6 +921,13 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
         } else {
           dl_dlogp = 0.f;
           dent = 0.f;
+        }
+        if (la == 0) {  // the row's statistics terms (written always: a condition here costs the chain a register)
+          const int sr = r0 + rr;
+          RSL[RS_PG * RL + sr] = live ? -fminf(pl1, pl2) : 0.f;
+          RSL[RS_ENT * RL + sr] = live ? -ent : 0.f;
+          RSL[RS_CLIP * RL + sr] = (live && fabsf(ratio - 1.0f) > A.hp.clip_range) ? 1.f : 0.f;
+          RSL[RS_KL * RL + sr] = live ? (ratio - 1.0f) - (logp - logp_old) : 0.f;
         }
         if (gfast) {
           if (la < Da) {
@@ -852,6 +1038,11 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
       loss_log[gs * 4 + 3] = pg + A.hp.ent_coef * el + A.hp.vf_coef * vl;
     }
     PPO_TICK(8);
+    // the statistics fold: on warp 3 when it idles through the tail (neither slice owner nor statistics warp: small
+    // policies, whose short tail the statistics warps' work nearly fills), else on the last warp
+    if (A.stats && warp == ((tail_stats && n_own_w < 4) ? 3 : PT / 32 - 1))
+      ppo_stats_fold_warp(ACC, RSL, rcp_fast((float)min(mb, Ni - start)), start == 0, threadIdx.x & 31);
+    // (1 / nb recomputed here: keeping the step's live through the chain until the tail costs the chain a spill)
     if (tail_stats && tid >= st0) {
       // ---- 4a. the statistics threads own no slice quad: they run the next step's statistics while the owners finish
       //          the step.  They skip the exchange waits (they read none of RECV, SSQ or the new parameters before the
@@ -890,11 +1081,27 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
   #pragma unroll
         for (int w = 0; w < PT / 32; ++w) my_ssq += w < n_own_w ? nred[w] : 0.f;
       }
-      if (tid < CL) st_async_f32(mapa_u32(ssq_sa + (uint32_t)crank * 4u, tid), my_ssq, mapa_u32(xbar2_sa, tid));
+      if (tid < CL) {
+        st_async_f32(mapa_u32(ssq_sa + (uint32_t)crank * 4u, tid), my_ssq, mapa_u32(xbar2_sa, tid));
+        if (kl_on)
+          st_async_f32(mapa_u32(smem_u32(KLS) + (uint32_t)crank * 4u, tid), ppo_kl_part<RL>(RSL, inv_nb),
+                       mapa_u32(xbar2_sa, tid));
+      }
       PPO_TICK(10);
       mbar_wait(&xbar[2], (uint32_t)(gs & 1));
-      if (tid == 0) mbar_expect_tx(&xbar[2], (uint32_t)(CL * 4));  // re-arm for the next step
+      if (tid == 0) mbar_expect_tx(&xbar[2], nbytes);  // re-arm for the next step
       PPO_TICK(11);
+      bool stop = false;
+      if (kl_on) {
+        // target_kl (SB3: approx_kl > 1.5 target_kl): the CL shares summed in the same order everywhere, so every CTA
+        // reaches the same decision; a stopping step takes no Adam step (nothing is all-gathered, nobody waits for
+        // it), and all CTAs leave at the next step's top barrier
+        float kl = 0.f;
+#pragma unroll
+        for (int c = 0; c < CL; ++c) kl += KLS[c];
+        stop = kl > 1.5f * A.target_kl;
+        if (stop && tid == 0) KSTOP = (int)gs + 1;
+      }
 
       // ---- 5. clip_grad_norm_ + Adam on the OWNED slice (moments never leave their owner); the new parameters are
       //         all-gathered into every CTA's parameter vector ----------------------------------------------------------
@@ -904,7 +1111,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
       total = sqrtf(total);
       float clip = A.hp.max_grad_norm / (total + 1e-6f);
       clip = clip > 1.0f ? 1.0f : clip;
-      if (own) {
+      if (own && !stop) {
         const float step_size = bc[2 * cur], inv_bc2s = rcp_fast(bc[2 * cur + 1]);
         const int q0 = crank * S + i0;
         const float4 m4 = ld4(Ms + q0), v4 = ld4(Vs + q0), p4 = ld4(Pm + q0);
@@ -929,8 +1136,10 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
           st_async_v4(mapa_u32(pm_sa + (uint32_t)q0 * 4u, dstc), pw, mapa_u32(xbar1_sa, dstc));
         }
       }
-      mbar_wait(&xbar[1], (uint32_t)(gs & 1));  // every CTA's new parameter slice has landed in Pm
-      if (tid == 0) mbar_expect_tx(&xbar[1], xbytes);  // re-arm for the next step
+      if (!stop) {
+        mbar_wait(&xbar[1], (uint32_t)(gs & 1));  // every CTA's new parameter slice has landed in Pm
+        if (tid == 0) mbar_expect_tx(&xbar[1], xbytes);  // re-arm for the next step
+      }
       PPO_TICK(12);
     }
     if (has_norm && gs + 1 < n_steps) run_count += min(mb, Ni - start_next);  // (after the statistics that read it)
@@ -954,18 +1163,36 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
       g_v[p] = Vs[q];
     }
   }
+  // target_kl stop at step KSTOP - 1: Adam steps taken = KSTOP - 1, epochs begun = the stopped step's epoch + 1; when a
+  // later step's statistics were computed ahead, rstat has moved on and g_norm already holds the stopped step's
+  const int kstop = kl_on ? KSTOP : 0;
   if (crank == 0) {
     for (int p = tid; p < NP; p += PT) g_params[p] = Pm[flat_to_play(pd, PL, p)];
     if (has_norm) {
-      if (tid < Do) {
+      if (tid < Do && !(kstop && kstop < n_steps)) {
         g_norm[tid] = rstat[tid];
         g_norm[Do + tid] = rstat[64 + tid];
       }
       if (tid == 0) *g_norm_count = run_count;
     }
     if (tid == 0) {
-      state[IMB_ST_PPO_STEP] = adam_step;
-      state[IMB_ST_PPO_EPOCH] = perm_draw0 + A.hp.n_epochs;
+      state[IMB_ST_PPO_STEP] = kstop ? state[IMB_ST_PPO_STEP] + (kstop - 1) : adam_step;
+      state[IMB_ST_PPO_EPOCH] = perm_draw0 + (kstop ? (kstop - 1) / steps_per_epoch + 1 : A.hp.n_epochs);
+    }
+  }
+  if (A.stats) {
+    if (tid == 0) ppo_stats_push(cluster, TH1, ACC, EVP, crank);  // (the chain's tiles are free now)
+    cluster.sync();
+    if (crank == 0 && tid == 0) {
+      float sd = __int_as_float(0x7fc00000);
+      if (!discrete) {
+        sd = 0.f;
+        for (int a = 0; a < Da; ++a) sd += expf(Pm[PL.ls + a]);
+        sd /= (float)Da;
+      }
+      const int64_t n_eval = kstop ? kstop : n_steps;
+      ppo_stats_finish(TH1, A.stats, A, n_eval, (n_eval - 1) / steps_per_epoch + 1, steps_per_epoch, sd,
+                       state[IMB_ST_PPO_EPOCH], kstop != 0);
     }
   }
   cluster.sync();  // no CTA may exit while peers can still address its shared memory
@@ -1142,11 +1369,15 @@ constexpr PpoShape kPpoShapes[] = {
     {27, 8, 0, 1},  // Ant-shaped Box with NormalizeFeaturesExtractor
     {4, 2, 1, 0},   // CartPole-shaped Discrete
 };
-template <int I>
+template <int I, int OPT>
 constexpr auto k_ppo_update_spec =
-    k_ppo_update<32, kPpoShapes[I].d_obs, kPpoShapes[I].d_act, kPpoShapes[I].discrete, kPpoShapes[I].has_norm>;
-constexpr decltype(&k_ppo_update<32>) kPpoUpdateKernels[] = {k_ppo_update<32>, k_ppo_update_spec<0>, k_ppo_update_spec<1>,
-                                                            k_ppo_update_spec<2>};
+    k_ppo_update<32, kPpoShapes[I].d_obs, kPpoShapes[I].d_act, kPpoShapes[I].discrete, kPpoShapes[I].has_norm, OPT>;
+constexpr decltype(&k_ppo_update<32>) kPpoUpdateKernels[] = {k_ppo_update<32>, k_ppo_update_spec<0, 0>,
+                                                            k_ppo_update_spec<1, 0>, k_ppo_update_spec<2, 0>};
+// With target_kl or clip_range_vf on, every shape runs the runtime-shape instantiation with their code compiled in
+// (OPT = 1): the shape-specialised ones sit at 254-255 registers, and the options' code makes the Ant-shaped one spill.
+// The arithmetic is the same bit for bit in every instantiation.
+constexpr auto kPpoUpdateOptKernel = k_ppo_update<32, 0, 0, 0, 0, 1>;
 constexpr const char* kPpoUpdateNames[] = {"k_ppo_update", "k_ppo_update<17x6 Box, norm>", "k_ppo_update<27x8 Box, norm>",
                                            "k_ppo_update<4x2 Discrete>"};
 constexpr int kNumPpoVariants = sizeof(kPpoUpdateKernels) / sizeof(kPpoUpdateKernels[0]);
@@ -1173,7 +1404,11 @@ static int launch_ppo(const PpoArgs& A0, int act, float* params, float* norm, in
   size_t bytes;
   const int plan = ppo_plan(A, act, &bytes);
   if (plan == IMB_PPO_PLAN_UPDATE) {
-    static size_t attr_bytes[kNumPpoVariants] = {};
+    static size_t attr_bytes[kNumPpoVariants + 1] = {};
+    if (A.target_kl > 0.f || A.clip_vf > 0.f)
+      return launch_cluster(kPpoUpdateOptKernel, "k_ppo_update<target_kl / clip_range_vf>", bytes,
+                            &attr_bytes[kNumPpoVariants], st, A, params, norm, norm_count, m, v, rollout, perm, loss_log,
+                            state);
     const int var = ppo_variant(A.pol);
     return launch_cluster(kPpoUpdateKernels[var], kPpoUpdateNames[var], bytes, &attr_bytes[var], st, A, params, norm,
                           norm_count, m, v, rollout, perm, loss_log, state);
@@ -1193,18 +1428,30 @@ static int launch_ppo(const PpoArgs& A0, int act, float* params, float* norm, in
   return plan;
 }
 
-extern "C" int imb_ppo_update(const imb_policy_desc* pol, int32_t pol_act, float* pol_params, float* pol_norm,
-                              int32_t* pol_norm_count, float* exp_avg, float* exp_avg_sq, const float* rollout,
-                              int64_t n_rows, const imb_ppo_hparams* hp, const int64_t* perm, uint64_t seed,
-                              float* loss_log, int64_t* state, void* stream) {
+extern "C" int imb_ppo_update_ex(const imb_policy_desc* pol, int32_t pol_act, float* pol_params, float* pol_norm,
+                                 int32_t* pol_norm_count, float* exp_avg, float* exp_avg_sq, const float* rollout,
+                                 int64_t n_rows, const imb_ppo_hparams* hp, float target_kl, float clip_range_vf,
+                                 const int64_t* perm, uint64_t seed, float* loss_log, float* stats_out, int64_t* state,
+                                 void* stream) {
   IMB_REQUIRE(n_rows >= 1 && n_rows < (1ll << 31), "bad n_rows");
   PpoArgs A;
   A.pol = *pol;
   A.hp = *hp;
   A.n_rows = n_rows;
   A.seed = seed;
+  A.target_kl = target_kl > 0.f ? target_kl : 0.f;
+  A.clip_vf = clip_range_vf > 0.f ? clip_range_vf : 0.f;
+  A.stats = stats_out;
   return launch_ppo(A, pol_act, pol_params, pol_norm, pol_norm_count, exp_avg, exp_avg_sq, rollout, perm, loss_log, state,
                     (cudaStream_t)stream);
+}
+
+extern "C" int imb_ppo_update(const imb_policy_desc* pol, int32_t pol_act, float* pol_params, float* pol_norm,
+                              int32_t* pol_norm_count, float* exp_avg, float* exp_avg_sq, const float* rollout,
+                              int64_t n_rows, const imb_ppo_hparams* hp, const int64_t* perm, uint64_t seed,
+                              float* loss_log, int64_t* state, void* stream) {
+  return imb_ppo_update_ex(pol, pol_act, pol_params, pol_norm, pol_norm_count, exp_avg, exp_avg_sq, rollout, n_rows, hp,
+                           0.f, 0.f, perm, seed, loss_log, nullptr, state, stream);
 }
 
 template <int HP, int ACT>

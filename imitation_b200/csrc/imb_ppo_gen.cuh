@@ -109,6 +109,13 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
   __shared__ float bc[2];
   __shared__ float SSQ[CL];   // squared gradient norms of the CL slices (each written by its owner into every CTA)
   __shared__ float LOSS[32];  // [CL][3] partial loss sums (read by CTA 0)
+  // training statistics (ppo_stats_fold): per-row slots of the step (summed over its passes), accumulators, the CTAs'
+  // KL shares of the step (target_kl; written beside SSQ), explained-variance partials
+  __shared__ float RSL[RS_N * RG];
+  __shared__ float ACC[AC_N];
+  __shared__ float KLS[CL];
+  __shared__ double EVP[4];
+  __shared__ double EVW[PT / 32];
   const imb_policy_desc& pd = A.pol;
   const int Do = pd.d_obs, Da = pd.d_act, h = pd.hidden, NP = pd.n_params, S = A.S;
   const PLay PL = make_play(pd);
@@ -118,6 +125,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int rw = A.rw;
   const int mb = A.hp.batch_size;
+  const bool kl_on = A.target_kl > 0.f, rec = kl_on || A.stats != nullptr;  // (uniform)
   const GenLayout G = gen_layout(S, HP, A.KP, Da, mb);
   float* Pm = smem + G.Pm;
   float* GP = smem + G.GP;
@@ -145,6 +153,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
   for (int i = tid; i < G.total; i += PT) smem[i] = 0.f;
   if (tid < 32) LOSS[tid] = 0.f;
   if (tid < CL) SSQ[tid] = 0.f;
+  if (tid < AC_N) ACC[tid] = 0.f;
   __syncthreads();
   if (tid < 64) {
     rstat[tid] = (pd.has_norm && tid < Do) ? g_norm[tid] : 0.f;
@@ -167,9 +176,11 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
   int64_t adam_step = state[IMB_ST_PPO_STEP];
   const int64_t perm_draw0 = state[IMB_ST_PPO_EPOCH];
   double b1pow = pow(0.9, (double)adam_step), b2pow = pow(0.999, (double)adam_step);
+  if (A.stats) ppo_ev_partial(rollout, N, rw, col_logp + 1, col_ret, crank, EVP, EVW);
   cluster.sync();  // every CTA's shared memory is initialised before any peer touches it
 
   int ep_now = 0, start = 0;
+  int64_t kstop = 0;  // target_kl: the stopping step + 1
   for (int64_t gs = 0; gs < n_steps; ++gs) {
     const int nb = min(mb, Ni - start);
     const float inv_nb = 1.0f / (float)nb;
@@ -186,6 +197,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
       IDX[r] = (int)idx;
     }
     for (int i = tid; i < CL * S; i += PT) GP[i] = 0.f;
+    if (rec && tid < RS_N * RG) RSL[tid] = 0.f;
     if (tid == PT - 1) {
       b1pow *= 0.9;
       b2pow *= 0.999;
@@ -355,11 +367,20 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
           float kk = up8 ? k1 : k0;
           kk += __shfl_xor_sync(0xffffffffu, up8 ? k0 : k1, 8);
           const float val = oct_sum(kk) + Pm[PL.bv];
-          const float dv = val - RET[lrow];
-          const float dval = live ? A.hp.vf_coef * 2.0f * dv * inv_nb : 0.f;
+          float dv;
+          bool vin = true;  // clip_range_vf: the clamp passes the gradient (torch's clamp backward: edges included)
+          if (A.clip_vf > 0.f) {
+            const float vold = live ? rollout[(int64_t)IDX[base + lrow] * rw + col_logp + 1] : 0.f, dvo = val - vold;
+            dv = (vold + fminf(fmaxf(dvo, -A.clip_vf), A.clip_vf)) - RET[lrow];
+            vin = dvo >= -A.clip_vf && dvo <= A.clip_vf;
+          } else {
+            dv = val - RET[lrow];
+          }
+          const float dval = (live && vin) ? A.hp.vf_coef * 2.0f * dv * inv_nb : 0.f;
           if (la == 0) {
             if (live) l_v += dv * dv;
             DVAL[lrow] = dval;
+            if (rec && live) RSL[RS_V * RG + lrow] += dv * dv;
           }
           const float d0 = __shfl_sync(0xffffffffu, dval, 0), d1 = __shfl_sync(0xffffffffu, dval, 8);
           const float d2 = __shfl_sync(0xffffffffu, dval, 16), d3 = __shfl_sync(0xffffffffu, dval, 24);
@@ -436,6 +457,12 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
             if (la == 0) {
               l_pg += -fminf(pl1, pl2);
               l_ent += -ent;
+              if (rec) {  // the row's statistics terms
+                RSL[RS_PG * RG + lrow] += -fminf(pl1, pl2);
+                RSL[RS_ENT * RG + lrow] += -ent;
+                RSL[RS_CLIP * RG + lrow] += fabsf(ratio - 1.0f) > A.hp.clip_range ? 1.f : 0.f;
+                RSL[RS_KL * RG + lrow] += (ratio - 1.0f) - (logp - logp_old);
+              }
             }
           } else {
             dl_dlogp = 0.f;
@@ -558,6 +585,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
         L0[crank * 3 + 2] = s_ent;
       }
     }
+    if (A.stats && tid == PT - 1) ppo_stats_fold<RG>(ACC, RSL, inv_nb, start == 0);
     cluster.sync();
     if (crank == 0 && tid == 0 && loss_log) {
       float pg = 0.f, vl = 0.f, el = 0.f;
@@ -587,8 +615,22 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
       ss += (g.x * g.x + g.y * g.y) + (g.z * g.z + g.w * g.w);
     }
     const float my_ssq = block_sum(ss, red);
-    if (tid < CL) cluster.map_shared_rank(SSQ, tid)[crank] = my_ssq;
+    if (tid < CL) {
+      cluster.map_shared_rank(SSQ, tid)[crank] = my_ssq;
+      if (kl_on) cluster.map_shared_rank(KLS, tid)[crank] = ppo_kl_part<RG>(RSL, inv_nb);
+    }
     cluster.sync();  // all slice norms are in place everywhere; nobody reads a peer's GP any more
+    if (kl_on) {
+      // target_kl (SB3: approx_kl > 1.5 target_kl): the CL shares summed in the same order everywhere, so every CTA
+      // reaches the same decision; a stopping step takes no Adam step and all CTAs leave the loop here
+      float kl = 0.f;
+#pragma unroll
+      for (int c = 0; c < CL; ++c) kl += KLS[c];
+      if (kl > 1.5f * A.target_kl) {
+        kstop = gs + 1;
+        break;
+      }
+    }
     // ---- 5. clip_grad_norm_ + Adam on the OWNED slice; the new parameters go into every CTA's parameter vector ---------
     float total = 0.f;
 #pragma unroll
@@ -646,8 +688,23 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
       if (tid == 0) *g_norm_count = run_count;
     }
     if (tid == 0) {
-      state[IMB_ST_PPO_STEP] = adam_step;
-      state[IMB_ST_PPO_EPOCH] = perm_draw0 + A.hp.n_epochs;
+      state[IMB_ST_PPO_STEP] = kstop ? adam_step - 1 : adam_step;  // (the stopping step took no Adam step)
+      state[IMB_ST_PPO_EPOCH] = perm_draw0 + (kstop ? ep_now + 1 : A.hp.n_epochs);
+    }
+  }
+  if (A.stats) {
+    if (tid == 0) ppo_stats_push(cluster, TH1, ACC, EVP, crank);  // (the pass tiles are free now)
+    cluster.sync();
+    if (crank == 0 && tid == 0) {
+      float sd = __int_as_float(0x7fc00000);
+      if (!pd.discrete) {
+        sd = 0.f;
+        for (int a = 0; a < Da; ++a) sd += expf(Pm[PL.ls + a]);
+        sd /= (float)Da;
+      }
+      const int64_t n_eval = kstop ? kstop : n_steps;
+      ppo_stats_finish(TH1, A.stats, A, n_eval, (n_eval - 1) / steps_per_epoch + 1, steps_per_epoch, sd,
+                       state[IMB_ST_PPO_EPOCH], kstop != 0);
     }
   }
   cluster.sync();  // no CTA may exit while peers can still address its shared memory

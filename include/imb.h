@@ -323,6 +323,37 @@ int imb_ppo_update(const imb_policy_desc* pol, int32_t pol_act, float* pol_param
                    const float* rollout, int64_t n_rows, const imb_ppo_hparams* hp,
                    const int64_t* perm, uint64_t seed, float* loss_log, int64_t* state,
                    void* stream);
+/* imb_ppo_update with two more SB3 PPO options and the training statistics PPO.train records (SB3 2.2.1 PPO.train as
+ * restated by oracle/ppo_port.py; unpinned, like the rest of the PPO port).  imb_ppo_update is this call with
+ * target_kl = clip_range_vf = 0 and stats_out = NULL, and computes the same bits as it with any stats_out.
+ *  - clip_range_vf > 0: value_loss = mse(ret, old + clamp(value - old, -c, c)), old = the rollout table's value column;
+ *    the gradient flows where |value - old| <= c (torch's clamp backward).  <= 0: off.
+ *  - target_kl > 0: a step whose approx_kl = mean(exp(lr) - 1 - lr), lr = logp - logp_old, exceeds 1.5 target_kl takes
+ *    no optimiser step and ends the call.  Its statistics are recorded and its feature RunningNorm update stays;
+ *    state[IMB_ST_PPO_STEP] advances by the optimiser steps taken, state[IMB_ST_PPO_EPOCH] by the epochs begun.  <= 0: off.
+ *  - stats_out (optional) [IMB_PPO_STAT_FLOATS]: entropy / policy-gradient / value loss and clip fraction = means over
+ *    the steps evaluated (each step weighted equally); approx_kl = mean over the steps of the last epoch begun; loss = the
+ *    total loss of the last step evaluated; explained variance 1 - var(ret - value) / var(ret) over the rollout (NaN when
+ *    var(ret) = 0); std = mean exp(log_std) after the call (NaN: Discrete); n_updates = state[IMB_ST_PPO_EPOCH] after
+ *    the call; the steps evaluated and epochs begun by this call; 1 when target_kl stopped it. */
+#define IMB_PPO_STAT_ENTROPY_LOSS 0
+#define IMB_PPO_STAT_PG_LOSS 1
+#define IMB_PPO_STAT_VALUE_LOSS 2
+#define IMB_PPO_STAT_APPROX_KL 3
+#define IMB_PPO_STAT_CLIP_FRACTION 4
+#define IMB_PPO_STAT_LOSS 5
+#define IMB_PPO_STAT_EXPLAINED_VARIANCE 6
+#define IMB_PPO_STAT_STD 7
+#define IMB_PPO_STAT_N_UPDATES 8
+#define IMB_PPO_STAT_N_STEPS 9
+#define IMB_PPO_STAT_N_EPOCHS 10
+#define IMB_PPO_STAT_STOPPED 11
+#define IMB_PPO_STAT_FLOATS 16
+int imb_ppo_update_ex(const imb_policy_desc* pol, int32_t pol_act, float* pol_params, float* pol_norm,
+                      int32_t* pol_norm_count, float* exp_avg, float* exp_avg_sq,
+                      const float* rollout, int64_t n_rows, const imb_ppo_hparams* hp,
+                      float target_kl, float clip_range_vf, const int64_t* perm, uint64_t seed,
+                      float* loss_log, float* stats_out, int64_t* state, void* stream);
 
 /* Which kernel imb_ppo_update runs for the policy `pol` at minibatch size batch_size; host only, no GPU needed.
  * Honours IMB_PPO_FORCE_GENERAL.  <0 (imb_last_error() names the shared-memory need and limit) when no kernel can run
