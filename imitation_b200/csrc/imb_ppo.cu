@@ -304,94 +304,128 @@ __device__ __noinline__ void ppo_stats_finish(const float* box, float* __restric
   stats[IMB_PPO_STAT_STOPPED] = stopped ? 1.f : 0.f;
 }
 
-// Weight gradients of ONE tower over the CTA's RL = 8 rows -> GP (P-layout, local shared memory), by NQ warps: thread =
-// (unit gj = lane, every NQ-th input); the unit's dL/dz rows live in registers, the input rows are warp-uniform
-// broadcasts, the scattered GP stores have odd lane strides (conflict free).  The head biases / log_std (plain row sums)
-// ride with the last input group.  The dot products of a group are all computed into registers BEFORE the group's
-// stores: the compiler cannot prove that GP and the activation tiles do not alias, and with a store between two dots it
-// serialises them (load latency + FMA chain per dot, ~55 cycles each; the phase is latency bound).
-struct WgradOff {
-  int w1, b1, w2, b2, wa, ba, wv, bv, ls, ldo, ldh;
-};
+// Weight gradients over the CTA's RL = 8 rows -> GP (P-layout, local shared memory), one block of one tower per routine,
+// by NQ warps: thread = (unit gj = lane, every NQ-th input, wq = the warp's index among the NQ); the unit's dL/dz rows live
+// in registers, the input rows are warp-uniform broadcasts, the scattered GP stores have odd lane strides (conflict free).
+// Bias and head-bias gradients are plain row sums.  Every element is one dot8r / sum8 over the 8 rows in row order, so the
+// thread that computes it and the time it does so do not change its bits.  The dot products of a group are all computed
+// into registers BEFORE the group's stores: the compiler cannot prove that GP and the activation tiles do not alias, and
+// with a store between two dots it serialises them (load latency + FMA chain per dot, ~55 cycles each; the blocks are
+// latency bound).
+// (the loops over inputs run from 0 with the thread's offset added inside, so that their trip counts are compile-time
+// constants when the shape is)
+
+// dW2 and b2 of a tower (operands: its H1 and dL/dz2 tiles); for the value tower also the value head's wv and bv (its
+// latent tile and dL/dvalue)
 template <int NQ, int HPx>
-__device__ __forceinline__ void tower_wgrad(const int tnet, const int gj, const int wq, const int h, const int Do, const int Da,
-                                            const bool discrete, const WgradOff o, float* __restrict__ GP,
-                                            const float* __restrict__ tH1, const float* __restrict__ tLAT,
-                                            const float* __restrict__ tDZ2, const float* __restrict__ tDZ1,
-                                            const float* __restrict__ XNc, const float* __restrict__ DM,
-                                            const float* __restrict__ DLS, const float* __restrict__ DVAL) {
+__device__ __forceinline__ void wgrad_layer2(const bool value, const int gj, const int wq, const int h, const int w2,
+                                             const int b2, const int ldh, const int wv, const int bv,
+                                             float* __restrict__ GP, const float* __restrict__ tH1,
+                                             const float* __restrict__ tLAT, const float* __restrict__ tDZ2,
+                                             const float* __restrict__ DVAL) {
   constexpr int RLc = 8;
   constexpr int T2 = (HPx + NQ - 1) / NQ;  // layer-2 inputs per thread
-  float dz2[8], dz1[8], lt[8];
+  float dz2[8];
   if (gj < h) {
     load8(dz2, tDZ2 + gj * RLc);
-    load8(dz1, tDZ1 + gj * RLc);
-    load8(lt, tLAT + gj * RLc);
-    {  // dW2[gj][i], i = wq + NQ t
-      float r[T2];
+    float r[T2];  // dW2[gj][i], i = wq + NQ t
 #pragma unroll
-      for (int t = 0; t < T2; ++t) {
-        const int i = wq + NQ * t;
-        r[t] = dot8r(dz2, tH1 + (i < HPx ? i : 0) * RLc);
-      }
-#pragma unroll
-      for (int t = 0; t < T2; ++t) {
-        const int i = wq + NQ * t;
-        if (i < h) GP[o.w2 + gj * o.ldh + i] = r[t];
-      }
+    for (int t = 0; t < T2; ++t) {
+      const int i = wq + NQ * t;
+      r[t] = dot8r(dz2, tH1 + (i < HPx ? i : 0) * RLc);
     }
-    // (the loops over inputs run from 0 with the thread's offset added inside, so that their trip counts are compile-time
-    // constants when the shape is)
-#pragma unroll
-    for (int kb = 0; kb < Do; kb += 4 * NQ) {  // dW1[gj][k], four at a time
-      const int k0 = kb + wq;
-      if (k0 >= Do) break;
-      float r[4];
-#pragma unroll
-      for (int t = 0; t < 4; ++t) {
-        const int k = k0 + NQ * t;
-        r[t] = dot8r(dz1, XNc + (k < Do ? k : 0) * RLc);
-      }
-#pragma unroll
-      for (int t = 0; t < 4; ++t) {
-        const int k = k0 + NQ * t;
-        if (k < Do) GP[o.w1 + gj * o.ldo + k] = r[t];
-      }
+    float rv = 0.f;
+    if (value && wq == NQ - 1) {
+      float lt[8];
+      load8(lt, tLAT + gj * RLc);
+      rv = dot8r(lt, DVAL);
     }
-    if (tnet == 0) {
 #pragma unroll
-      for (int ab = 0; ab < Da; ab += 2 * NQ) {
-        const int a0 = ab + wq, a1 = a0 + NQ;
-        if (a0 >= Da) break;
-        const float ra = dot8r(lt, DM + a0 * RLc), rb = dot8r(lt, DM + (a1 < Da ? a1 : a0) * RLc);
-        GP[o.wa + a0 * o.ldh + gj] = ra;
-        if (a1 < Da) GP[o.wa + a1 * o.ldh + gj] = rb;
-      }
-    } else if (wq == 0) {
-      GP[o.wv + gj] = dot8r(lt, DVAL);
+    for (int t = 0; t < T2; ++t) {
+      const int i = wq + NQ * t;
+      if (i < h) GP[w2 + gj * ldh + i] = r[t];
     }
-    if (wq == 0) GP[o.b2 + gj] = sum8(dz2);
-    if (wq == NQ - 1) GP[o.b1 + gj] = sum8(dz1);
+    if (wq == 0) GP[b2 + gj] = sum8(dz2);
+    if (value && wq == NQ - 1) GP[wv + gj] = rv;
   }
-  if (wq == NQ - 1) {
-    if (tnet == 0) {  // ba, log_std
+  if (value && wq == NQ - 1 && gj == 0) {
+    load8(dz2, DVAL);
+    GP[bv] = sum8(dz2);
+  }
+}
+
+// dW1 and b1 of a tower (operands: its dL/dz1 tile and the normalised observations)
+template <int NQ>
+__device__ __forceinline__ void wgrad_layer1(const int gj, const int wq, const int h, const int Do, const int w1,
+                                             const int b1, const int ldo, float* __restrict__ GP,
+                                             const float* __restrict__ tDZ1, const float* __restrict__ XNc) {
+  constexpr int RLc = 8;
+  if (gj >= h) return;
+  float dz1[8];
+  load8(dz1, tDZ1 + gj * RLc);
 #pragma unroll
-      for (int tb = 0; tb < 2 * Da; tb += HPx) {
-        const int t = tb + gj;
-        if (t >= 2 * Da) break;
-        if (t < Da) {
-          load8(dz2, DM + t * RLc);
-          GP[o.ba + t] = sum8(dz2);
-        } else if (!discrete) {
-          load8(dz2, DLS + (t - Da) * RLc);
-          GP[o.ls + t - Da] = sum8(dz2);
-        }
-      }
-    } else if (gj == 0) {  // bv
-      load8(dz2, DVAL);
-      GP[o.bv] = sum8(dz2);
+  for (int kb = 0; kb < Do; kb += 4 * NQ) {  // dW1[gj][k], four at a time
+    const int k0 = kb + wq;
+    if (k0 >= Do) break;
+    float r[4];
+#pragma unroll
+    for (int t = 0; t < 4; ++t) {
+      const int k = k0 + NQ * t;
+      r[t] = dot8r(dz1, XNc + (k < Do ? k : 0) * RLc);
+    }
+#pragma unroll
+    for (int t = 0; t < 4; ++t) {
+      const int k = k0 + NQ * t;
+      if (k < Do) GP[w1 + gj * ldo + k] = r[t];
     }
   }
+  if (wq == NQ - 1) GP[b1 + gj] = sum8(dz1);
+}
+
+// The policy's action head: Wa, ba and log_std (operands: the policy latent tile, dL/d(mean|logits), dL/dlog_std)
+template <int NQ, int HPx>
+__device__ __forceinline__ void wgrad_head(const int gj, const int wq, const int h, const int Da, const bool discrete,
+                                           const PLay& L, float* __restrict__ GP, const float* __restrict__ tLAT,
+                                           const float* __restrict__ DM, const float* __restrict__ DLS) {
+  constexpr int RLc = 8;
+  float d[8];
+  if (gj < h) {
+    load8(d, tLAT + gj * RLc);
+#pragma unroll
+    for (int ab = 0; ab < Da; ab += 2 * NQ) {
+      const int a0 = ab + wq, a1 = a0 + NQ;
+      if (a0 >= Da) break;
+      const float ra = dot8r(d, DM + a0 * RLc), rb = dot8r(d, DM + (a1 < Da ? a1 : a0) * RLc);
+      GP[L.wa + a0 * L.ldh + gj] = ra;
+      if (a1 < Da) GP[L.wa + a1 * L.ldh + gj] = rb;
+    }
+  }
+  if (wq == NQ - 1) {  // ba, log_std
+#pragma unroll
+    for (int tb = 0; tb < 2 * Da; tb += HPx) {
+      const int t = tb + gj;
+      if (t >= 2 * Da) break;
+      if (t < Da) {
+        load8(d, DM + t * RLc);
+        GP[L.ba + t] = sum8(d);
+      } else if (!discrete) {
+        load8(d, DLS + (t - Da) * RLc);
+        GP[L.ls + t - Da] = sum8(d);
+      }
+    }
+  }
+}
+
+// Named barriers that hand a chain's tiles to the warps computing their weight gradients (0 is __syncthreads, 2 the owner
+// warps' slice-norm reduction): the value tower's dL/dz2 tile, the policy head's operands (latent tile, dL/dmean,
+// dL/dlog_std), the policy tower's dL/dz2 tile, the value tower's dL/dz1 tile complete.  The chain warps bar.arrive (never
+// blocking the chain), the gradient warps bar.sync; the count is both together.
+enum { BAR_VDZ2 = 3, BAR_PHEAD = 4, BAR_PDZ2 = 5, BAR_VDZ1 = 6 };
+__device__ __forceinline__ void bar_arrive(const int id, const int n) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory");
+}
+__device__ __forceinline__ void bar_sync(const int id, const int n) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory");
 }
 
 // PPO.train for one rollout: n_epochs x ceil(N / batch) optimiser steps, ONE cluster of CL CTAs.
@@ -405,9 +439,10 @@ __device__ __forceinline__ void tower_wgrad(const int tnet, const int gj, const 
 //     the ~8 dependent stages of the chain cost no CTA barrier, and every weight read from shared memory
 //     feeds four FMAs (with 2 rows per warp on all 8 warps the chain was bound by shared-memory wavefronts);
 //   * weight gradients over the CTA's 8 rows: thread = (unit, input subset) of one tower, staged in local shared
-//     memory in the parameter layout.  The VALUE tower's are computed early by warps 2-7 (its chain ends ~1 k cycles
-//     before the policy tower's: no action head, no loss terms) while warps 0, 1 finish the policy chain; the policy
-//     tower's by all eight warps after the step's second barrier.  The staged vector is pushed to the peer slice
+//     memory in the parameter layout.  Each block (a tower's dW2 + b2, its dW1 + b1, the action head) starts as soon
+//     as the chain warps signal its operand tiles (named barriers, bar.arrive on the chain side), on warps that are
+//     idle then, while warps 0, 1 finish the policy chain; only the policy tower's dW1 + b1 is left for all eight
+//     warps after the step's second barrier.  The staged vector is pushed to the peer slice
 //     owners through distributed shared memory with 16-byte stores; owners sum the CL partials in fixed order (their
 //     own straight from the staging vector), exchange the squared slice norms, run clip_grad_norm_ + Adam on their
 //     slice (the moments never leave their owner) and all-gather the new parameters into every CTA's copy (their
@@ -533,8 +568,6 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
   const int64_t perm_draw0 = state[IMB_ST_PPO_EPOCH];
   double b1pow = pow(0.9, (double)adam_step), b2pow = pow(0.999, (double)adam_step);  // beta^t, kept incrementally
   const int row0 = crank * RL;        // first minibatch row owned by this CTA
-  const WgradOff wo_p = {PL.w1[0], PL.b1[0], PL.w2[0], PL.b2[0], PL.wa, PL.ba, PL.wv, PL.bv, PL.ls, ldo, ldh};
-  const WgradOff wo_v = {PL.w1[1], PL.b1[1], PL.w2[1], PL.b2[1], PL.wa, PL.ba, PL.wv, PL.bv, PL.ls, ldo, ldh};
 
   // Asynchronous row gather of one minibatch (epoch ep, first row start) into buffer `buf` by the nst statistics
   // threads: two (thread) tasks per row draw the row index and copy half of the 16-byte aligned rollout row each with
@@ -947,6 +980,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
           }
         }
         __syncwarp();
+        bar_arrive(BAR_PHEAD, 192);  // the head's gradients can start (warps 4-7)
         PPO_WCLK(7);
 #pragma unroll U_DA
         for (int a = 0; a < Da; ++a) {
@@ -964,6 +998,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
           make_float4(jl ? dl0 * (1.0f - lat0 * lat0) : 0.f, jl ? dl1 * (1.0f - lat1 * lat1) : 0.f,
                       jl ? dl2 * (1.0f - lat2 * lat2) : 0.f, jl ? dl3 * (1.0f - lat3 * lat3) : 0.f));
       __syncwarp();
+      bar_arrive(cnet ? BAR_VDZ2 : BAR_PDZ2, 192);  // the tower's layer-2 gradients can start (warps 4-7)
       a0 = a1 = a2 = a3 = 0.f;
       {
         const float* wp = cW2 + jc;
@@ -982,13 +1017,27 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
                       jl ? a2 * (1.f - h12 * h12) : 0.f, jl ? a3 * (1.f - h13 * h13) : 0.f));
     }
     PPO_WCLK(0);
-    // ---- 1c. the VALUE tower's weight gradients, early: its chain (warps 2, 3) finishes ~1 k cycles before the policy
-    //          tower's (no action head, no loss terms) and the statistics / prefetch warps are done by then as well, so
-    //          warps 2-7 meet on a named barrier and compute them while warps 0, 1 are still in the policy chain ------
-    if (warp >= 2) {
-      asm volatile("bar.sync 1, 192;" ::: "memory");
-      tower_wgrad<6, HP>(1, lane, warp - 2, h, Do, Da, discrete, wo_v, GP, TH1 + HP * RL, TLAT + HP * RL,
-                         TDZ2 + HP * RL, TDZ1 + HP * RL, XNc, DM, DLS, DVAL);
+    // ---- 1c. weight gradients as their operands land, while warps 0, 1 are still in the policy chain: warps 4-7 (done
+    //          with the prefetch, or with the statistics and the prefetch when those stay beside the chain) take the
+    //          value tower's dW2 block, the policy head's and the policy tower's dW2 block, each as soon as the chain
+    //          warps signal its tiles; warps 2, 3 take the value tower's dW1 block at the end of their own chain (each
+    //          holds half of its rows).  Only the policy tower's dW1 block is left for after the chain.  The chain warps
+    //          only arrive on these barriers, so they reach the loss log's CTA barriers below without waiting on a helper,
+    //          and the tiles are not written again before the next step's top barrier. ----------------------------------------
+    if (warp >= 4) {
+      bar_sync(BAR_VDZ2, 192);
+      wgrad_layer2<4, HP>(true, lane, warp - 4, h, PL.w2[1], PL.b2[1], ldh, PL.wv, PL.bv, GP, TH1 + HP * RL,
+                          TLAT + HP * RL, TDZ2 + HP * RL, DVAL);
+      PPO_WCLK(9);
+      bar_sync(BAR_PHEAD, 192);
+      wgrad_head<4, HP>(lane, warp - 4, h, Da, discrete, PL, GP, TLAT, DM, DLS);
+      PPO_WCLK(7);
+      bar_sync(BAR_PDZ2, 192);
+      wgrad_layer2<4, HP>(false, lane, warp - 4, h, PL.w2[0], PL.b2[0], ldh, 0, 0, GP, TH1, TLAT, TDZ2, DVAL);
+    } else if (warp >= 2) {
+      bar_sync(BAR_VDZ1, 64);
+      wgrad_layer1<2>(lane, warp - 2, h, Do, PL.w1[1], PL.b1[1], ldo, GP, TDZ1 + HP * RL, XNc);
+      PPO_WCLK(9);
     }
     PPO_WCLK(8);
     // partial loss sums of this CTA -> CTA 0 (distributed shared memory)
@@ -1005,8 +1054,9 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
     }
     __syncthreads();
     PPO_TICK(3);
-    // ---- 2. the POLICY tower's weight gradients (and the action head's) by all eight warps ------------------------------
-    tower_wgrad<PT / 32, HP>(0, lane, warp, h, Do, Da, discrete, wo_p, GP, TH1, TLAT, TDZ2, TDZ1, XNc, DM, DLS, DVAL);
+    if (warp >= 2) PPO_WCLK(6);  // (slot 6 of the policy warps is taken by the chain)
+    // ---- 2. the POLICY tower's dW1 block by all eight warps --------------------------------------------------------------
+    wgrad_layer1<PT / 32>(lane, warp, h, Do, PL.w1[0], PL.b1[0], ldo, GP, TDZ1, XNc);
     __syncthreads();
     PPO_TICK(7);
     // ---- 3. push the partials to the PEER slice owners: RECV[this CTA][i], one 16-byte DSMEM store per quad ------------

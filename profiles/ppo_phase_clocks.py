@@ -11,8 +11,8 @@ import torch as th
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from imitation_b200 import _desc, _lib  # noqa: E402
 
-NAMES = ["top barrier", "-", "-", "warp chain fwd/loss/bwd", "-", "-", "-",
-         "weight gradients -> GP", "push partials (7 peers)", "barrier a wait", "slice sum + norm exchange issue", "wait: slice norms landed",
+NAMES = ["top barrier", "-", "-", "chain + early wgrad blocks", "-", "-", "-",
+         "policy dW1/b1 -> GP", "push partials (7 peers)", "barrier a wait", "slice sum + norm exchange issue", "wait: slice norms landed",
          "clip + Adam (own slice) + parameter all-gather + wait", "-"]
 pd = _desc.policy_desc(17, 6, False, 32, True)
 N = 4096
@@ -48,7 +48,13 @@ print(f"{'total':<18s} {tot / steps:9.0f} cycles/step")
 w = (ctypes.c_longlong * 80)()
 assert _lib.lib().imb_debug_ppo_warp_clocks(w, 0) == 0
 print("per-warp cycles/step since the top barrier (CTA 0; warps 0,1 policy tower, 2,3 value tower; warps 4-7: slot 1 = "
-      "next-step stats done (in the step's tail), slot 3 = prefetch issued (beside the chain)):")
-for slot, name in ((1, "stats done (w4-7)"), (3, "after layer 1 | prefetch"), (4, "after layer 2"), (5, "after means (policy)"), (6, "after logp reduce"), (7, "after dM/dlogstd"),
-                   (2, "after heads/loss"), (0, "chain end"), (8, "early value wgrad done (w2-7)")):
-    print(f"  {name:<22s}", [round(w[slot * 8 + i] / steps) for i in range(8)])
+      "next-step stats done (in the step's tail), slot 3 = prefetch issued (beside the chain); early weight-gradient "
+      "blocks: value dW2, policy head and policy dW2 on warps 4-7, value dW1 on warps 2,3).\n"
+      "Each warp counts from its own read of the clock after the top barrier; the rows of warps that reach that barrier "
+      "early (4-7) run ahead of the others' by about their wait there: align them on the post-chain barrier row, which "
+      "thread 0 passes at the 'chain + early wgrad blocks' total above.")
+for slot, name in ((1, "stats done (w4-7)"), (3, "after layer 1 | prefetch"), (4, "after layer 2"), (5, "after means (policy)"), (6, "after logp reduce"),
+                   (7, "after dM/dlogstd | head wgrad (w4-7)"), (2, "after heads/loss"), (0, "chain end"),
+                   (9, "value dW1 (w2,3) | value dW2 (w4-7)"), (8, "early wgrad blocks done (w2-7)"),
+                   (6, "after logp reduce | post-chain barrier (w2-7)")):
+    print(f"  {name:<36s}", [round(w[slot * 8 + i] / steps) for i in range(8)])
