@@ -150,6 +150,8 @@ SIGNATURES = {
                                     _ptr, _i64, _ptr, _ptr, _ptr, _i32, _ptr, _ptr], 1),
     "imb_ensemble_relabel_ws_floats": (_i64, [_i32, _i64], 0),
     "imb_ensemble_relabel": (_i32, [_pu, _f32, _ptr, _i32, _i32, _i64, _i64, _ptr, _ptr], None),
+    "imb_rollout_explore": (_i32, [_env, _ptr, _ptr, _pol, _i32, _ptr, _ptr, _disc, _ptr, _ptr, _members, _i32, _hp,
+                                   _i64, _i64, _ptr, _ptr, _ptr, _ptr, _i32, _ptr, _u64, _i64, _ptr, _ptr], 1),
     "imb_sync_buffer_doubles": (_i64, [_sync], 0),
     "imb_sync_snapshot": (_i32, [_sync, _ptr, _ptr], None),
     "imb_sync_pack": (_i32, [_sync, _ptr, _ptr], 1),
@@ -451,6 +453,19 @@ def ensemble_relabel(d: PrefUncDesc, alpha, rollout_tbl, rw, col_rew, n_envs, n_
     norm = any(d.norm_state[m] for m in range(d.n_members))
     _check(lib().imb_ensemble_relabel(d, alpha, _p(rollout_tbl, th.float32), rw, col_rew, n_envs, n_steps,
                                       _p(ws, th.float32), _stream()), "imb_ensemble_relabel", 1 + int(norm))
+
+
+def rollout_explore(env, env_params, env_obs, pol, pol_params, pol_norm, disc, disc_params, disc_norm, members, reward_mode,
+                    hp, n_envs, n_steps, rollout_tbl, flat_out, aux, noise, explore_policy, explore_seed, explore_step0,
+                    state, flags=0, act=ACT_TANH):
+    """`rollout` (members None) or `rollout_ensemble` (members: a RolloutMembers table, reward_mode 2) without a ring,
+    where step t is a random-policy step when explore_policy[t] (uint8 [n_steps]) is 1: actions drawn from Philox keyed
+    by explore_seed at step explore_step0 + t, or read from noise."""
+    _check(lib().imb_rollout_explore(env, _p(env_params, th.float32), _p(env_obs, th.float32), pol, act,
+                                     _p(pol_params, th.float32), _p(pol_norm), disc, _p(disc_params), _p(disc_norm),
+                                     members, reward_mode, hp, n_envs, n_steps, _p(rollout_tbl, th.float32),
+                                     _p(flat_out), _p(aux, th.float32), _p(noise), flags, _p(explore_policy, th.uint8),
+                                     explore_seed, explore_step0, _p(state, th.int64), _stream()), "imb_rollout_explore")
 
 
 def gae(rollout_tbl, rw, col_value, n_envs, n_steps, aux, gamma, gae_lambda, state, horizon):

@@ -18,6 +18,7 @@ import math
 
 from typing import Optional
 
+import numpy as np
 import torch as th
 
 from .. import _lib
@@ -82,6 +83,8 @@ class DevicePPO:
         self._aux = None
         self._ens_raw = None      # ensemble reward: the members' raw rewards [M][T][E]
         self._ens_ws = None       # ensemble reward: the relabel's workspace
+        # buffers of exploration_rollout (table, flat rows, aux, ensemble raw rewards and workspace): never captured
+        self._x_tbl = self._x_flat = self._x_aux = self._x_raw = self._x_ws = None
         self.loss_log = None      # optional [n_minibatch_steps][4] device tensor (parity tests)
         self.noise = None         # optional pinned sampling noise for the next rollout (parity tests)
         self.perm = None          # optional host permutations [n_epochs][N] (parity tests)
@@ -128,8 +131,37 @@ class DevicePPO:
         if self._tbl is None or self._tbl.shape[0] != E * T:
             self._tbl = th.zeros(E * T, rw, device=self.device)
             self._aux = th.zeros(2 * E + 2 * E * T, device=self.device)
-        disc = dparams = dnorm = ens = None
-        mode, out_norm = 0, None
+        flat, ring = (None, None)
+        if self._buffering is not None:
+            flat, ring = self._buffering.rollout_targets(T)
+        t0 = env.host_ep_step
+        ring_args = (ring.table if ring is not None else None, ring.capacity if ring is not None else 0)
+
+        def launch(disc, dparams, dnorm, mode, members):
+            if members is None:
+                _lib.rollout(env.desc, env.params, env.obs, pol.desc, pp, pn, disc, dparams, dnorm, mode, self.hp, E, T,
+                             self._tbl, *ring_args, flat, self._aux, self.noise, env.state, act=pol.act)
+            else:
+                _lib.rollout_ensemble(env.desc, env.params, env.obs, pol.desc, pp, pn, disc, members, self.hp, E, T,
+                                      self._tbl, *ring_args, flat, self._aux, self.noise, env.state, act=pol.act)
+
+        self._ens_raw, self._ens_ws = self._relabelled_rollout(launch, self._tbl, E, T, self._ens_raw, self._ens_ws)
+        da = 1 if pol.discrete else pol.d_act
+        col_val = pol.d_obs + da + 1
+        _lib.gae(self._tbl, rw, col_val, E, T, self._aux, self.hp.gamma, self.hp.gae_lambda, env.state, env.horizon)
+        _lib.rollout_advance(env.state, E, T, env.horizon, ring.capacity if ring is not None else 0)
+        if not self._capturing:
+            self.after_rollout_host(t0)
+
+    def _relabelled_rollout(self, launch, tbl, E: int, T: int, ens_raw, ens_ws):
+        """Launch a rollout over the learned reward the RewardVecEnvWrapper describes, then finish its reward column
+        (rewards/reward_wrapper.py:92-133 -> predict_processed): a NormalizedRewardNet's output normalisation, or the
+        ensemble's per-member normalisation and mean + alpha * std, advancing the output statistics once per env step.
+        launch(disc, disc_params, disc_norm, reward_mode, members) issues the rollout itself (members: the ensemble's
+        member table, else None).  ens_raw / ens_ws: the ensemble's buffers, reused when their size fits; returns them
+        (a captured graph bakes the training rollout's in, so every rollout keeps its own)."""
+        disc = dparams = dnorm = members = None
+        mode, out_norm, ens = 0, None, None
         if self._rw_wrapper is not None:
             net, mode, out_norm = self._rw_wrapper.resolve()
             if isinstance(net, reward_wrapper.EnsembleRelabel):
@@ -137,47 +169,73 @@ class DevicePPO:
             else:
                 eng = net.engine()
                 disc, dparams, dnorm = eng.desc, eng.params, eng.norm_state
-        flat, ring = (None, None)
-        if self._buffering is not None:
-            flat, ring = self._buffering.rollout_targets(T)
-        t0 = env.host_ep_step
-        ring_args = (ring.table if ring is not None else None, ring.capacity if ring is not None else 0)
-        if ens is None:
-            _lib.rollout(env.desc, env.params, env.obs, pol.desc, pp, pn, disc, dparams, dnorm, mode, self.hp, E, T,
-                         self._tbl, *ring_args, flat, self._aux, self.noise, env.state, act=pol.act)
-        else:
-            members, relabel = self._ensemble_tables(ens, E, T)
-            _lib.rollout_ensemble(env.desc, env.params, env.obs, pol.desc, pp, pn, ens.nets[0].engine().desc, members,
-                                  self.hp, E, T, self._tbl, *ring_args, flat, self._aux, self.noise, env.state,
-                                  act=pol.act)
-        da = 1 if pol.discrete else pol.d_act
-        col_val = pol.d_obs + da + 1
         if ens is not None:
-            _lib.ensemble_relabel(relabel, ens.alpha, self._tbl, rw, col_val + 1, E, T, self._ens_ws)
+            ens_raw, ens_ws, members, relabel = self._ensemble_tables(ens, E, T, ens_raw, ens_ws)
+            disc = ens.nets[0].engine().desc
+        launch(disc, dparams, dnorm, mode, members)
+        pol = self.policy
+        rw = tbl.shape[1]
+        col_rew = pol.d_obs + (1 if pol.discrete else pol.d_act) + 2
+        if ens is not None:
+            _lib.ensemble_relabel(relabel, ens.alpha, tbl, rw, col_rew, E, T, ens_ws)
         elif out_norm is not None:
             ns, nc = out_norm.output_norm_vectors()
             layer = out_norm.normalize_output_layer
-            _lib.reward_norm_scan(self._tbl.view(-1)[col_val + 1:], E, T, rw, T * rw, ns, nc, layer.eps, True,
+            _lib.reward_norm_scan(tbl.view(-1)[col_rew:], E, T, rw, T * rw, ns, nc, layer.eps, True,
                                   ema_decay=layer.decay if out_norm.output_norm_is_ema else None)
-        _lib.gae(self._tbl, rw, col_val, E, T, self._aux, self.hp.gamma, self.hp.gae_lambda, env.state, env.horizon)
-        _lib.rollout_advance(env.state, E, T, env.horizon, ring.capacity if ring is not None else 0)
-        if not self._capturing:
-            self.after_rollout_host(t0)
+        return ens_raw, ens_ws
 
-    def _ensemble_tables(self, ens, E: int, T: int):
-        """Member table of the ensemble rollout and member descriptor of its relabel, over buffers kept across rounds
-        (a captured graph bakes their addresses in)."""
+    def _ensemble_tables(self, ens, E: int, T: int, raw, ws):
+        """Member table of the ensemble rollout and member descriptor of its relabel over the buffers raw (the members'
+        raw rewards [M][T][E]) and ws (the relabel's workspace), allocated when missing or too small; -> (raw, ws,
+        members, relabel)."""
         M = len(ens.nets)
         n_ws = _lib.ensemble_relabel_ws_floats(M, T)
-        if self._ens_raw is None or self._ens_raw.numel() != M * T * E:
-            self._ens_raw = th.empty(M * T * E, device=self.device)
-        if self._ens_ws is None or self._ens_ws.numel() < n_ws:
-            self._ens_ws = th.zeros(n_ws, device=self.device)  # zero-filled: the relabel's ticket starts at 0
+        if raw is None or raw.numel() != M * T * E:
+            raw = th.empty(M * T * E, device=self.device)
+        if ws is None or ws.numel() < n_ws:
+            ws = th.zeros(n_ws, device=self.device)  # zero-filled: the relabel's ticket starts at 0
         engines = [n.engine() for n in ens.nets]
         members = _lib.rollout_members([e.params for e in engines],
-                                       [e.norm_state if e.has_norm else None for e in engines], self._ens_raw)
+                                       [e.norm_state if e.has_norm else None for e in engines], raw)
         norms = [None if o is None else o.output_norm_args() for o in ens.out_norms]
-        return members, _lib.pref_uncertainty_desc(list(self._ens_raw.view(M, T * E)), norms)
+        return raw, ws, members, _lib.pref_uncertainty_desc(list(raw.view(M, T * E)), norms)
+
+    def exploration_rollout(self, explore_policy, seed: int, step0: int, deterministic: bool = False, noise=None):
+        """The rollout of an ExplorationWrapper over this algorithm (AgentTrainer.sample's exploration phase,
+        algorithms/preference_comparisons.py:283-301): len(explore_policy) steps, a whole number of episodes, from an
+        episode start, step t taken by the random policy where explore_policy[t] is 1 (actions from the Philox stream
+        keyed by `seed` at step step0 + t, or from `noise`) and by this policy otherwise (sampled, or its mode when
+        `deterministic`).  The learned reward is relabelled as in collect_rollouts, so the output normalisers advance
+        once per step.  Uses buffers of its own: the training rollout's table, ring and flat rows (which a captured
+        graph bakes in) are not touched, nor is num_timesteps, and no GAE runs.  -> (flat rows [E*T][tw] in
+        completion order, ground-truth env rewards [E][T]), device tensors valid until the next call."""
+        env = self._base_env
+        env.ensure_reset()
+        E, H, T = env.num_envs, env.horizon, len(explore_policy)
+        if T % H != 0 or env.host_ep_step != 0:
+            raise ValueError(f"an exploration rollout covers whole episodes from an episode start: {T} steps with "
+                             f"horizon {H} from episode step {env.host_ep_step}")
+        pol = self.policy
+        pp, pn, _ = pol.flat_vectors()
+        rw = _lib.rollout_row_width(pol.desc)
+        tw = 2 * env.d_obs + env.d_act + 1
+        if self._x_tbl is None or self._x_tbl.shape[0] != E * T:
+            self._x_tbl = th.zeros(E * T, rw, device=self.device)
+            self._x_flat = th.zeros(E * T, tw, device=self.device)
+            self._x_aux = th.zeros(2 * E + 2 * E * T, device=self.device)
+        vec = th.as_tensor(np.ascontiguousarray(explore_policy, dtype=np.uint8)).to(self.device)
+        flags = _lib.IMB_RF_DETERMINISTIC if deterministic else 0
+
+        def launch(disc, dparams, dnorm, mode, members):
+            _lib.rollout_explore(env.desc, env.params, env.obs, pol.desc, pp, pn, disc, dparams, dnorm, members, mode,
+                                 self.hp, E, T, self._x_tbl, self._x_flat, self._x_aux, noise, vec, seed, step0,
+                                 env.state, flags=flags, act=pol.act)
+
+        self._x_raw, self._x_ws = self._relabelled_rollout(launch, self._x_tbl, E, T, self._x_raw, self._x_ws)
+        _lib.rollout_advance(env.state, E, T, H, 0)
+        env.host_ep_step = 0
+        return self._x_flat, self._x_aux[2 * E + E * T:].view(E, T)
 
     def after_rollout_host(self, t0: int) -> None:
         """Host-side mirrors of what the rollout kernels just did (also called per graph replay)."""

@@ -28,7 +28,7 @@ from torch.utils import data as data_th
 
 from .. import _desc, _lib, spaces
 from . import base
-from ..data import rollout, types
+from ..data import rollout, types, wrappers
 from ..data.types import TrajectoryWithRew
 from ..rewards import reward_nets
 from ..util import logger as imit_logger
@@ -89,6 +89,28 @@ class TrajectoryDataset(TrajectoryGenerator):
         return _get_trajectories(trajectories, steps)
 
 
+def split_steps(steps: int, exploration_frac: float, logger=None) -> Tuple[int, int]:
+    """(agent_steps, exploration_steps) of AgentTrainer.sample(steps) (:247-254), warning like the reference when a
+    positive exploration_frac rounds to no exploration steps."""
+    exploration_steps = int(exploration_frac * steps)
+    if exploration_frac > 0 and exploration_steps == 0 and logger is not None:
+        logger.warn(f"No exploration steps included: exploration_frac = {exploration_frac} > 0 but steps={steps} is "
+                    "too small.")
+    return steps - exploration_steps, exploration_steps
+
+
+def exploration_plan(wrapper, rng: np.random.Generator, exploration_steps: int, num_envs: int, horizon: int):
+    """The host side of the exploration rollout, with the reference's random-number consumption: on the lock-step
+    fixed-horizon env, generate_trajectories' unbiased stop rule (data/rollout.py:382-506) rolls k = ceil(
+    exploration_steps / (E H)) batches of E whole episodes, i.e. k H calls of the wrapper, then shuffles the k E
+    trajectories with `rng` (the order is discarded: the BufferingWrapper's are used).  -> (k, the wrapper's policy of
+    each of the k H steps)."""
+    k = -(-exploration_steps // (num_envs * horizon))
+    policy_steps = wrapper.advance(k * horizon)
+    rng.shuffle(list(range(k * num_envs)))
+    return k, policy_steps
+
+
 class AgentTrainer(TrajectoryGenerator):
     """Train the device generator on a learned reward and hand its trajectories (with the ENVIRONMENT's rewards) to the
     preference pipeline (:127-316).  `algorithm` is a `DevicePPO` over a `DeviceVecEnv`; the learned reward is fused into
@@ -97,14 +119,10 @@ class AgentTrainer(TrajectoryGenerator):
     def __init__(self, algorithm, reward_fn, venv, rng: np.random.Generator, exploration_frac: float = 0.0,
                  switch_prob: float = 0.5, random_prob: float = 0.5,
                  custom_logger: Optional[imit_logger.HierarchicalLogger] = None) -> None:
-        from ..data import wrappers
         from ..rewards import reward_wrapper
 
         self.algorithm = algorithm
         super().__init__(custom_logger)
-        if exploration_frac > 0:
-            raise NotImplementedError("exploratory rollouts (ExplorationWrapper: host-side policy switching per step) have "
-                                      "no device path; use exploration_frac=0")
         if isinstance(reward_fn, reward_nets.RewardNet):
             reward_fn = reward_fn.predict_processed
         self.reward_fn = reward_fn
@@ -116,6 +134,14 @@ class AgentTrainer(TrajectoryGenerator):
         self.log_callback = self.reward_venv_wrapper.make_log_callback()
         self.algorithm.set_env(self.venv)
         self.algorithm.set_logger(self.logger)
+        self.exploration_wrapper = None
+        if exploration_frac > 0:
+            from ..policies import exploration_wrapper
+
+            # (the reference builds it for any exploration_frac, drawing from rng twice; this one only when it is used)
+            self.exploration_wrapper = exploration_wrapper.ExplorationWrapper(
+                policy=self.algorithm, venv=self.algorithm.get_env(), random_prob=random_prob, switch_prob=switch_prob,
+                rng=self.rng)
 
     def train(self, steps: int, **kwargs) -> None:
         n_transitions = self.buffering_wrapper.n_transitions
@@ -128,24 +154,50 @@ class AgentTrainer(TrajectoryGenerator):
         agent_trajs, _ = self.buffering_wrapper.pop_finished_trajectories()
         agent_trajs = agent_trajs[::-1]  # the latest trajectories come from the most relevant version of the agent
         avail_steps = sum(len(t) for t in agent_trajs)
-        if avail_steps < steps:
-            self.logger.log(f"Requested {steps} transitions but only {avail_steps} in buffer. "
-                            f"Sampling {steps - avail_steps} additional transitions.")
+        agent_steps, exploration_steps = split_steps(steps, self.exploration_frac, self.logger)
+        if avail_steps < agent_steps:
+            self.logger.log(f"Requested {agent_steps} transitions but only {avail_steps} in buffer. "
+                            f"Sampling {agent_steps - avail_steps} additional transitions.")
             # roll the (stochastic) policy without training until enough episodes have finished; the wrapper records them
             per = self.buffering_wrapper.num_envs * self.algorithm.n_steps
             H = self.buffering_wrapper.venv.horizon
             guard = 0
             more: List[TrajectoryWithRew] = []
-            while sum(len(t) for t in more) < steps - avail_steps:
+            while sum(len(t) for t in more) < agent_steps - avail_steps:
                 self.buffering_wrapper.before_rollout()
                 self.algorithm.collect_rollouts()
                 new, _ = self.buffering_wrapper.pop_finished_trajectories()
                 more += list(new)
                 guard += per
-                if guard > 4 * (steps + H * self.buffering_wrapper.num_envs) + per:
+                if guard > 4 * (agent_steps + H * self.buffering_wrapper.num_envs) + per:
                     raise RuntimeError("could not collect enough finished trajectories")
             agent_trajs = list(agent_trajs) + more
-        return list(_get_trajectories(agent_trajs, steps))
+        trajectories = list(_get_trajectories(agent_trajs, agent_steps))
+        if exploration_steps > 0:
+            self.logger.log(f"Sampling {exploration_steps} exploratory transitions.")
+            trajectories.extend(_get_trajectories(self._exploration_trajectories(exploration_steps), exploration_steps))
+        return trajectories
+
+    def _exploration_trajectories(self, exploration_steps: int) -> List[TrajectoryWithRew]:
+        """generate_trajectories(exploration_wrapper, venv, make_sample_until(min_timesteps=exploration_steps), rng) and
+        the BufferingWrapper's finished trajectories afterwards (:283-301): from venv.reset(), which drops the running
+        episodes, whole episodes of the E lock-step envs until they hold exploration_steps transitions, as ONE rollout
+        launch with the learned reward relabelled (advancing its output normalisers) -- in completion order, with the
+        environment's rewards.  The policy acts in eval mode and num_timesteps does not move (SB3's predict)."""
+        bw = self.buffering_wrapper
+        E, H = bw.num_envs, bw.venv.horizon
+        step0 = self.exploration_wrapper.steps_taken
+        k, policy_steps = exploration_plan(self.exploration_wrapper, self.rng, exploration_steps, E, H)
+        self.venv.reset()  # RewardVecEnvWrapper -> BufferingWrapper.reset -> DeviceVecEnv.reset
+        bw.discard()       # the running episodes' steps go with the reset (data/wrappers.py:45-61)
+        flat, rews = self.algorithm.exploration_rollout(policy_steps, self.exploration_wrapper.seed, step0,
+                                                        self.exploration_wrapper.deterministic_policy)
+        flat, rews = flat.cpu().numpy(), rews.cpu().numpy()
+        out: List[TrajectoryWithRew] = []
+        for j in range(k):  # episode batch j: rows [j E H, (j + 1) E H), env-major
+            out += wrappers.finished_trajectories(bw.venv, flat[j * E * H:(j + 1) * E * H],
+                                                  rews[:, j * H:(j + 1) * H].reshape(-1))
+        return out
 
     @property
     def logger(self) -> imit_logger.HierarchicalLogger:

@@ -43,7 +43,7 @@ static int rollout_common(const imb_env_desc* env, const float* env_params, floa
                           const float* disc_params, const float* disc_norm, const imb_rollout_members* members,
                           int reward_mode, const imb_ppo_hparams* hp, int64_t n_envs, int64_t n_steps, float* rollout,
                           float* ring, int64_t ring_capacity, float* flat_out, float* aux, const float* noise, int flags,
-                          const int64_t* state, void* stream) {
+                          const int64_t* state, const RolloutExplore* Xp, void* stream) {
   IMB_REQUIRE(n_envs >= 1 && n_steps >= 1, "rollout needs n_envs, n_steps >= 1");
   IMB_REQUIRE(env->d_obs == pol->d_obs && env->d_act == pol->d_act && env->discrete == pol->discrete,
               "env / policy space mismatch");
@@ -71,7 +71,7 @@ static int rollout_common(const imb_env_desc* env, const float* env_params, floa
   cudaStream_t st = (cudaStream_t)stream;
   if (!members)
     return launch_rollout(A, pol_act, L, nullptr, env_params, env_obs, pol_params, pol_norm, disc_params, rollout, ring,
-                          flat_out, aux, noise, state, st);
+                          flat_out, aux, noise, state, Xp, st);
   const int M = members->n_members;
   IMB_REQUIRE(M >= 2 && M <= IMB_PU_MAX_MEMBERS, "imb_rollout_ensemble: %d members (2 to %d)", M, IMB_PU_MAX_MEMBERS);
   IMB_REQUIRE(members->raw != nullptr, "imb_rollout_ensemble: no raw-output buffer");
@@ -90,7 +90,7 @@ static int rollout_common(const imb_env_desc* env, const float* env_params, floa
     }
   }
   return launch_rollout(A, pol_act, L, &Mb, env_params, env_obs, pol_params, pol_norm, nullptr, rollout, ring, flat_out,
-                        aux, noise, state, st);
+                        aux, noise, state, Xp, st);
 }
 
 extern "C" int imb_rollout(const imb_env_desc* env, const float* env_params, float* env_obs,
@@ -101,7 +101,7 @@ extern "C" int imb_rollout(const imb_env_desc* env, const float* env_params, flo
                            const float* noise, int flags, const int64_t* state, void* stream) {
   return rollout_common(env, env_params, env_obs, pol, pol_act, pol_params, pol_norm, disc, disc_params, disc_norm,
                         nullptr, reward_mode, hp, n_envs, n_steps, rollout, ring, ring_capacity, flat_out, aux, noise,
-                        flags, state, stream);
+                        flags, state, nullptr, stream);
 }
 
 extern "C" int imb_rollout_ensemble(const imb_env_desc* env, const float* env_params, float* env_obs,
@@ -112,7 +112,28 @@ extern "C" int imb_rollout_ensemble(const imb_env_desc* env, const float* env_pa
                                     int flags, const int64_t* state, void* stream) {
   IMB_REQUIRE(disc && members, "imb_rollout_ensemble needs a member architecture and a member table");
   return rollout_common(env, env_params, env_obs, pol, pol_act, pol_params, pol_norm, disc, nullptr, nullptr, members, 2,
-                        hp, n_envs, n_steps, rollout, ring, ring_capacity, flat_out, aux, noise, flags, state, stream);
+                        hp, n_envs, n_steps, rollout, ring, ring_capacity, flat_out, aux, noise, flags, state, nullptr,
+                        stream);
+}
+
+extern "C" int imb_rollout_explore(const imb_env_desc* env, const float* env_params, float* env_obs,
+                                   const imb_policy_desc* pol, int32_t pol_act, const float* pol_params,
+                                   const float* pol_norm, const imb_disc_desc* disc, const float* disc_params,
+                                   const float* disc_norm, const imb_rollout_members* members, int reward_mode,
+                                   const imb_ppo_hparams* hp, int64_t n_envs, int64_t n_steps, float* rollout,
+                                   float* flat_out, float* aux, const float* noise, int flags,
+                                   const uint8_t* explore_policy, uint64_t explore_seed, int64_t explore_step0,
+                                   const int64_t* state, void* stream) {
+  IMB_REQUIRE(explore_policy != nullptr, "imb_rollout_explore needs the per-step policy vector");
+  IMB_REQUIRE(!members || (disc && reward_mode == 2 && !disc_params && !disc_norm),
+              "imb_rollout_explore: a member table goes with reward_mode 2, the member architecture and no single net");
+  RolloutExplore Xp;
+  Xp.policy = explore_policy;
+  Xp.seed = explore_seed;
+  Xp.step0 = explore_step0;
+  return rollout_common(env, env_params, env_obs, pol, pol_act, pol_params, pol_norm, disc, disc_params, disc_norm,
+                        members, reward_mode, hp, n_envs, n_steps, rollout, nullptr, 0, flat_out, aux, noise, flags,
+                        state, &Xp, stream);
 }
 
 extern "C" int imb_rollout_advance(int64_t* state, int64_t n_envs, int64_t n_steps, int32_t horizon,

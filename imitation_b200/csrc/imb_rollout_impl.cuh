@@ -56,6 +56,16 @@ struct RolloutMembers {
   float* raw;
 };
 
+// Exploration rollout (imb_rollout_explore, policies/exploration_wrapper.py): policy[t] = 1 makes step t a random-policy
+// step for every env (action_space.sample(): uniform on the Box [-1, 1], or a uniform action index), drawn from Philox
+// stream IMB_STREAM_EXPLORE keyed by `seed` at counter (env id, step0 + t, a / 4); with pinned noise the uniform is read
+// from the slot the policy step would read.
+struct RolloutExplore {
+  const uint8_t* policy;  // [T]: 0 = the wrapped policy, 1 = random
+  uint64_t seed;
+  int64_t step0;
+};
+
 // flattened (reference-order) index of local step t of env e; see file header
 __device__ __forceinline__ int64_t flat_index(int64_t e, int64_t t, int64_t E, int64_t T, int64_t t0, int64_t H) {
   const int64_t seg = (t0 + t) / H;
@@ -67,7 +77,9 @@ __device__ __forceinline__ int64_t flat_index(int64_t e, int64_t t, int64_t E, i
 
 // ENS: evaluate the Mb.M ensemble members (raw outputs to Mb.raw) instead of the one net at disc_params (reward column);
 // the single-net variant has no member loop.  ACT: the policy towers' activation (env and reward net keep their own).
-template <int RPL, bool ENS, int ACT>
+// EXP: the exploration rollout, Xp.policy[t] picks the policy of step t (random steps skip the policy towers and
+// record logp = value = 0); without it Xp is unused.
+template <int RPL, bool ENS, int ACT, bool EXP>
 __global__ void __launch_bounds__(RT, 1) k_rollout(const RolloutArgs A, const DiscLaunch L, const RolloutMembers Mb,
                                                    const float* __restrict__ env_params, float* __restrict__ env_obs,
                                                    const float* __restrict__ pol_params,
@@ -75,7 +87,7 @@ __global__ void __launch_bounds__(RT, 1) k_rollout(const RolloutArgs A, const Di
                                                    const float* __restrict__ disc_params, float* __restrict__ rollout,
                                                    float* __restrict__ ring, float* __restrict__ flat_out,
                                                    float* __restrict__ aux, const float* __restrict__ noise,
-                                                   const int64_t* __restrict__ state) {
+                                                   const int64_t* __restrict__ state, const RolloutExplore Xp) {
   constexpr int RR = rows_of(RPL), RRS = RR + TILE_PAD;
   extern __shared__ __align__(128) float smem[];
   const int tid = threadIdx.x;
@@ -198,16 +210,42 @@ __global__ void __launch_bounds__(RT, 1) k_rollout(const RolloutArgs A, const Di
   bool done = false;
   for (int64_t t = 0; t < T; ++t) {
     float* row = rollout + (e * T + t) * rw;
+    const bool rnd = EXP && Xp.policy[t] != 0;  // block-uniform: one entry per step
     // ---- policy: value tower, then pi tower (H2 ends up holding the pi latent) ------------------------------
-    const float value = value_of_obs(OBSU);
-    tile_layer<ACT, RPL>(XN, Do, psm + S.w1p, HP, psm + S.b1p, H1, HP);
-    __syncthreads();
-    tile_layer<ACT, RPL>(H1, h, psm + S.w2p, HP, psm + S.b2p, H2, HP);
-    __syncthreads();
+    float value = 0.f;
+    if (!rnd) {
+      value = value_of_obs(OBSU);
+      tile_layer<ACT, RPL>(XN, Do, psm + S.w1p, HP, psm + S.b1p, H1, HP);
+      __syncthreads();
+      tile_layer<ACT, RPL>(H1, h, psm + S.w2p, HP, psm + S.b2p, H2, HP);
+      __syncthreads();
+    }
     // ---- action head + sampling, thread per env ----------------------------------------------------------------
     float logp = 0.f;
     if (!rowthread) {
       // (threads beyond the tile's rows only take part in the tiled layers)
+    } else if (rnd) {
+      // random policy: action_space.sample() (exploration_wrapper.py:58-66)
+      uint32_t k0, k1;
+      philox_key(Xp.seed, IMB_STREAM_EXPLORE, k0, k1);
+      const uint32_t ctr = (uint32_t)(Xp.step0 + t);
+      if (!A.pol.discrete) {
+        constexpr float lo = -1.0f, hi = 1.0f;  // the synthetic env's Box
+        Philox4 r = {0u, 0u, 0u, 0u};
+        for (int a = 0; a < Da; ++a) {
+          if (!noise && (a & 3) == 0) r = philox4x32(egid, ctr, (uint32_t)(a >> 2), 0u, k0, k1);
+          const uint32_t w = (a & 3) == 0 ? r.x : (a & 3) == 1 ? r.y : (a & 3) == 2 ? r.z : r.w;
+          const float u = noise ? (live ? noise[(t * E + e) * Da + a] : 0.f) : u01(w);
+          const float act = lo + u * (hi - lo);
+          if (live) row[Do + a] = act;
+          OBSU[(Do + a) * RRS + tid] = fminf(fmaxf(act, lo), hi);  // (a no-op unless pinned noise leaves [0, 1])
+        }
+      } else {
+        const float u = noise ? (live ? noise[t * E + e] : 0.f) : u01(philox4x32(egid, ctr, 0u, 0u, k0, k1).x);
+        const int chosen = min((int)(u * (float)Da), Da - 1);
+        for (int a = 0; a < Da; ++a) OBSU[(Do + a) * RRS + tid] = (a == chosen) ? 1.f : 0.f;
+        if (live) row[Do] = (float)chosen;
+      }
     } else if (!A.pol.discrete) {
       float z4[4] = {0.f, 0.f, 0.f, 0.f};
       for (int a = 0; a < Da; ++a) {
@@ -515,53 +553,61 @@ static int rollout_plan(RolloutArgs& A, const DiscLaunch& L, int n_members, int6
            "images), more than the %d B limit of a CTA", bytes, n_img * 4, (int)IMB_SMEM_MAX);
 }
 
-template <int RPL, bool ENS, int ACT>
+template <int RPL, bool ENS, int ACT, bool EXP>
 static int launch_rollout_t(const RolloutArgs& A, const DiscLaunch& L, const RolloutMembers& Mb,
                             const float* env_params, float* env_obs, const float* pol_params, const float* pol_norm,
                             const float* disc_params, float* rollout, float* ring, float* flat_out, float* aux,
-                            const float* noise, const int64_t* state, cudaStream_t st) {
+                            const float* noise, const int64_t* state, const RolloutExplore& Xp, cudaStream_t st) {
   constexpr int RR = rows_of(RPL);
   const size_t bytes = (size_t)A.total * 4;
   static size_t attr_bytes = 0;
   if (bytes > attr_bytes) {
-    cudaError_t e = cudaFuncSetAttribute(k_rollout<RPL, ENS, ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e = cudaFuncSetAttribute(k_rollout<RPL, ENS, ACT, EXP>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          (int)bytes);
     if (e != cudaSuccess) IMB_FAIL(-2, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
     attr_bytes = bytes;
   }
   const int blocks = (int)((A.E + RR - 1) / RR);
-  k_rollout<RPL, ENS, ACT><<<blocks, RT, bytes, st>>>(A, L, Mb, env_params, env_obs, pol_params, pol_norm, disc_params,
-                                                      rollout, ring, flat_out, aux, noise, state);
+  k_rollout<RPL, ENS, ACT, EXP><<<blocks, RT, bytes, st>>>(A, L, Mb, env_params, env_obs, pol_params, pol_norm,
+                                                           disc_params, rollout, ring, flat_out, aux, noise, state, Xp);
   IMB_CHECK_LAUNCH("k_rollout");
   return 0;
 }
 
-// Mb == nullptr: the single-net rollout; act: the policy towers' activation (ACT_TANH / ACT_RELU)
+// Mb == nullptr: the single-net rollout; act: the policy towers' activation (ACT_TANH / ACT_RELU); Xp == nullptr: every
+// step on the policy (no exploration variant)
 template <int ACT>
 static int launch_rollout_act(RolloutArgs A, const DiscLaunch& L, const RolloutMembers* Mb,
                               const float* env_params, float* env_obs, const float* pol_params, const float* pol_norm,
                               const float* disc_params, float* rollout, float* ring, float* flat_out, float* aux,
-                              const float* noise, const int64_t* state, cudaStream_t st) {
+                              const float* noise, const int64_t* state, const RolloutExplore* Xp, cudaStream_t st) {
   const int rpl = rollout_plan(A, L, Mb ? Mb->M : 1, imb_num_sms());
   if (rpl < 0) return rpl;
   static const RolloutMembers no_members = {};
-#define IMB_RL(R)                                                                                                      \
-  return Mb ? launch_rollout_t<R, true, ACT>(A, L, *Mb, env_params, env_obs, pol_params, pol_norm, disc_params,       \
-                                             rollout, ring, flat_out, aux, noise, state, st)                           \
-            : launch_rollout_t<R, false, ACT>(A, L, no_members, env_params, env_obs, pol_params, pol_norm, disc_params, \
-                                              rollout, ring, flat_out, aux, noise, state, st)
+  static const RolloutExplore no_explore = {};
+#define IMB_RL_X(R, X, XP)                                                                                             \
+  return Mb ? launch_rollout_t<R, true, ACT, X>(A, L, *Mb, env_params, env_obs, pol_params, pol_norm, disc_params,    \
+                                                rollout, ring, flat_out, aux, noise, state, XP, st)                    \
+            : launch_rollout_t<R, false, ACT, X>(A, L, no_members, env_params, env_obs, pol_params, pol_norm,          \
+                                                 disc_params, rollout, ring, flat_out, aux, noise, state, XP, st)
+#define IMB_RL(R)                        \
+  do {                                   \
+    if (Xp) IMB_RL_X(R, true, *Xp);      \
+    IMB_RL_X(R, false, no_explore);      \
+  } while (0)
   if (rpl == 0) IMB_RL(0);
   if (rpl == 1) IMB_RL(1);
   if (rpl == 2) IMB_RL(2);
   IMB_RL(4);
 #undef IMB_RL
+#undef IMB_RL_X
 }
 
 static int launch_rollout(const RolloutArgs& A, int act, const DiscLaunch& L, const RolloutMembers* Mb,
                           const float* env_params, float* env_obs, const float* pol_params, const float* pol_norm,
                           const float* disc_params, float* rollout, float* ring, float* flat_out, float* aux,
-                          const float* noise, const int64_t* state, cudaStream_t st) {
+                          const float* noise, const int64_t* state, const RolloutExplore* Xp, cudaStream_t st) {
   auto go = act == ACT_TANH ? launch_rollout_act<ACT_TANH> : launch_rollout_act<ACT_RELU>;
   return go(A, L, Mb, env_params, env_obs, pol_params, pol_norm, disc_params, rollout, ring, flat_out, aux, noise,
-            state, st);
+            state, Xp, st);
 }

@@ -17,6 +17,23 @@ from . import buffer as buffer_mod
 from . import types
 
 
+def finished_trajectories(venv, flat: np.ndarray, rews: np.ndarray) -> List[types.TrajectoryWithRew]:
+    """The E finished trajectories of one lock-step episode segment of `venv` (a DeviceVecEnv, E envs), in env order:
+    flat = the segment's transition rows [E * L][tw] (env-major, the reference order) and rews their ground-truth
+    rewards [E * L]."""
+    E = venv.num_envs
+    tr = buffer_mod.rows_to_transitions(flat, venv.d_obs, venv.d_act, venv.observation_space.shape,
+                                        venv.action_space.shape, venv.observation_space.dtype, venv.action_space.dtype,
+                                        venv.discrete, rews=rews.astype(np.float32))
+    L = len(flat) // E
+    trajs = []
+    for e in range(E):
+        sl = slice(e * L, (e + 1) * L)
+        trajs.append(types.TrajectoryWithRew(obs=np.concatenate([tr.obs[sl], tr.next_obs[sl][-1:]]), acts=tr.acts[sl],
+                                             infos=None, terminal=True, rews=tr.rews[sl]))
+    return trajs
+
+
 class BufferingWrapper:
     def __init__(self, venv, error_on_premature_reset: bool = True):
         self.venv = venv
@@ -174,16 +191,8 @@ class BufferingWrapper:
             segs = segs[:-1]
         trajs, lens = [], []
         for a, b in segs:
-            flat = rows[:, a:b].reshape(-1, rows.shape[2])
-            tr = buffer_mod.rows_to_transitions(flat, v.d_obs, v.d_act, v.observation_space.shape, v.action_space.shape,
-                                                v.observation_space.dtype, v.action_space.dtype, v.discrete,
-                                                rews=rews[:, a:b].reshape(-1).astype(np.float32))
-            L = b - a
-            for e in range(E):
-                sl = slice(e * L, (e + 1) * L)
-                trajs.append(types.TrajectoryWithRew(obs=np.concatenate([tr.obs[sl], tr.next_obs[sl][-1:]]),
-                                                     acts=tr.acts[sl], infos=None, terminal=True, rews=tr.rews[sl]))
-                lens.append(L)
+            trajs += finished_trajectories(v, rows[:, a:b].reshape(-1, rows.shape[2]), rews[:, a:b].reshape(-1))
+            lens += [b - a] * E
         self.discard()
         if keep_from < T:
             # (like the reference, `n_transitions` restarts at 0 while the running episodes' steps stay in the accumulator)

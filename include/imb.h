@@ -464,6 +464,27 @@ int64_t imb_ensemble_relabel_ws_floats(int32_t n_members, int64_t n_steps);
 int imb_ensemble_relabel(const imb_pref_unc_desc* d, float alpha, float* rollout, int32_t rw, int32_t col_rew,
                          int64_t n_envs, int64_t n_steps, float* ws, void* stream);
 
+/* ---- exploratory rollouts of preference comparisons -------------------------------------------------------------------
+ * AgentTrainer.sample's exploration phase (algorithms/preference_comparisons.py:194-205, :231-307):
+ * generate_trajectories over an ExplorationWrapper (policies/exploration_wrapper.py:23-95) that switches, for the whole
+ * VecEnv at once, between the wrapped policy and a random one (action_space.sample()).  The switching chain does not
+ * depend on observations, so the host draws it beforehand: explore_policy[t] (uint8 [T]) is 1 when step t is a
+ * random-policy step, 0 when the policy acts.
+ * = imb_rollout (members == NULL) or imb_rollout_ensemble (members != NULL, reward_mode 2, disc = the member
+ * architecture, disc_params = disc_norm = NULL) without a ring, except on random steps: the towers are skipped, logp
+ * and value are 0, and the action is low + u (high - low) on the Box [-1, 1] or min(floor(u n), n - 1) for Discrete(n),
+ * with u a uniform of Philox stream IMB_STREAM_EXPLORE keyed by explore_seed at counter (env id, explore_step0 + t,
+ * a / 4) -- or, with noise != NULL, the value in the slot the policy step would read ([T][E][d_act] or [T][E]).
+ * Policy steps follow flags (IMB_RF_DETERMINISTIC: ExplorationWrapper(deterministic_policy=True)).  The env step, reward
+ * relabel, env-reward column, terminal handling and flattened rows are imb_rollout's. */
+int imb_rollout_explore(const imb_env_desc* env, const float* env_params, float* env_obs,
+                        const imb_policy_desc* pol, int32_t pol_act, const float* pol_params, const float* pol_norm,
+                        const imb_disc_desc* disc, const float* disc_params, const float* disc_norm,
+                        const imb_rollout_members* members, int reward_mode, const imb_ppo_hparams* hp,
+                        int64_t n_envs, int64_t n_steps, float* rollout, float* flat_out, float* aux,
+                        const float* noise, int flags, const uint8_t* explore_policy, uint64_t explore_seed,
+                        int64_t explore_step0, const int64_t* state, void* stream);
+
 /* ---- multi-GPU: replica state around the ONE all-reduce of a round ---------------------------
  * (SURVEY.md section 8e; the reference is single-process, so there is no reference interface to
  * cite: the merge restates RunningNorm's Chan update, util/networks.py:96-134, in its additive
