@@ -100,6 +100,8 @@ PPO_STAT_N_UPDATES, PPO_STAT_N_STEPS, PPO_STAT_N_EPOCHS, PPO_STAT_STOPPED = 8, 9
 PPO_STAT_FLOATS = 16
 # imb_pref_uncertainty modes
 PU_MODES = {"logit": 0, "probability": 1, "label": 2}
+# imb_param_regularize kinds
+REG_LP, REG_WEIGHT_DECAY = 1, 2
 
 _disc, _adam, _pol, _env, _hp, _pu, _members, _sync = map(C.POINTER, (
     DiscDesc, Adam, PolicyDesc, EnvDesc, PpoHparams, PrefUncDesc, RolloutMembers, SyncDesc))
@@ -144,6 +146,7 @@ SIGNATURES = {
     "imb_policy_logp": (_i32, [_pol, _i32, _ptr, _ptr, _ptr, _i64, _i64, _i32, _ptr], 1),
     "imb_disc_reduce_adam": (_i32, [_disc, _adam, _ptr, _ptr, _ptr, _f32, _ptr, _ptr, _ptr, _ptr], 1),
     "imb_pref_loss": (_i32, [_ptr, _i64, _i32, _ptr, _f32, _f32, _f32, _f32, _ptr, _ptr, _ptr, _i32, _ptr], 1),
+    "imb_param_regularize": (_i32, [_disc, _i32, _i32, _f32, _ptr, _ptr, _ptr, _i32, _ptr], 1),
     "imb_pref_uncertainty_ws_floats": (_i64, [_i32, _i64], 0),
     "imb_pref_uncertainty": (_i32, [_pu, _i64, _i32, _i32, _f32, _f32, _f32, _ptr, _ptr, _ptr, _ptr], None),
     "imb_rollout_ensemble": (_i32, [_env, _ptr, _ptr, _pol, _i32, _ptr, _ptr, _disc, _members, _hp, _i64, _i64, _ptr,
@@ -312,6 +315,13 @@ def pref_loss(rews, n_pairs, frag_len, prefs, noise_prob, discount, threshold, g
     _check(lib().imb_pref_loss(_p(rews, th.float32), n_pairs, frag_len, _p(prefs, th.float32), noise_prob, discount,
                                threshold, grad_scale, _p(grad_rews), _p(probs_out), _p(stats_acc), stats_slot,
                                _stream()), "imb_pref_loss")
+
+
+def param_regularize(d, kind, p, coeff, params, ws, stats_acc=None, stats_slot=0):
+    """kind REG_LP: the Lp penalty's gradient (coeff = lambda) into ws's gradient accumulator, its value into statistics
+    slot stats_slot of stats_acc (optional); kind REG_WEIGHT_DECAY: params += coeff * params (coeff = -lambda * lr)."""
+    _check(lib().imb_param_regularize(d, kind, p, coeff, _p(params, th.float32), _p(ws, th.float32),
+                                      _p(stats_acc, th.float32), stats_slot, _stream()), "imb_param_regularize")
 
 
 def pref_uncertainty_desc(rews, norms) -> PrefUncDesc:

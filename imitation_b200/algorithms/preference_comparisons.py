@@ -30,6 +30,7 @@ from .. import _desc, _lib, spaces
 from . import base
 from ..data import rollout, types, wrappers
 from ..data.types import TrajectoryWithRew
+from ..regularization import regularizers
 from ..rewards import reward_nets
 from ..util import logger as imit_logger
 from ..util.flat import views
@@ -873,6 +874,17 @@ def _epoch_permutation(n: int) -> th.Tensor:
     return fast(n) if _PERM_FAST else slow(n)
 
 
+def _resolve_subsets(dataset) -> Tuple[Any, Optional[np.ndarray]]:
+    """(base dataset, item indices into it | None) of nested `Subset`s: an ensemble's bagging subsets and the
+    training / validation split of a regularizer all index one shared base dataset."""
+    index = None
+    while isinstance(dataset, data_th.Subset):
+        ind = np.asarray(dataset.indices, dtype=np.int64)
+        index = ind if index is None else ind[index]
+        dataset = dataset.dataset
+    return dataset, index
+
+
 class BasicRewardTrainer(RewardTrainer):
     """Minibatch gradient accumulation with AdamW over a `PreferenceDataset` (:1139-1323)."""
 
@@ -880,8 +892,6 @@ class BasicRewardTrainer(RewardTrainer):
                  batch_size: int = 32, minibatch_size: Optional[int] = None, epochs: int = 1, lr: float = 1e-3,
                  custom_logger: Optional[imit_logger.HierarchicalLogger] = None, regularizer_factory=None) -> None:
         super().__init__(preference_model, custom_logger)
-        if regularizer_factory is not None:
-            raise NotImplementedError("regularizers (imitation.regularization) are outside this path")
         self.loss = loss
         self.batch_size = batch_size
         self.minibatch_size = minibatch_size or batch_size
@@ -890,8 +900,13 @@ class BasicRewardTrainer(RewardTrainer):
         self.epochs = epochs
         self.optim = th.optim.AdamW(self._preference_model.parameters(), lr=lr)
         self.rng = rng
-        self.regularizer = None
+        self.regularizer: Optional[regularizers.Regularizer] = (
+            regularizer_factory(optimizer=self.optim, logger=self.logger) if regularizer_factory is not None else None)
         self.last_epoch_stats: Dict[str, float] = {}
+        # the regularization keys of the last epoch, recorded as reward/final/<key> (a subset of FINAL_KEYS)
+        self.final_stats: Dict[str, float] = {}
+
+    FINAL_KEYS = ("regularized_loss", "regularization_lambda", "val/loss", "val/accuracy", "val/gt_reward_loss")
 
     def _make_data_loader(self, dataset) -> data_th.DataLoader:
         return data_th.DataLoader(dataset, batch_size=self.minibatch_size, shuffle=True,
@@ -899,18 +914,51 @@ class BasicRewardTrainer(RewardTrainer):
 
     @property
     def requires_regularizer_update(self) -> bool:
-        return False
+        return self.regularizer is not None and self.regularizer.val_split is not None
+
+    def _split(self, dataset):
+        """(training part, validation part | None) of `dataset`: with a regularizer that has a validation split, the
+        reference's `random_split` (:1224-1245), seeded by one `make_seeds(self.rng)` draw per call."""
+        if not self.requires_regularizer_update:
+            return dataset, None
+        val_length = int(len(dataset) * self.regularizer.val_split)
+        train_length = len(dataset) - val_length
+        if val_length < 1 or train_length < 1:
+            raise ValueError("Not enough data samples to split into training and validation, or the validation split "
+                             "is too large/small. Make sure you've generated enough initial preference data. You can "
+                             "adjust this through initial_comparison_frac in PreferenceComparisons.")
+        train, val = data_th.random_split(dataset, lengths=[train_length, val_length],
+                                          generator=th.Generator().manual_seed(make_seeds(self.rng)))
+        return train, val
+
+    def _skip_draws(self, dataset, epoch_multiplier: float = 1.0) -> None:
+        """Make exactly the draws `train(dataset, epoch_multiplier)` makes from `self.rng` and torch's global RNG,
+        without training: the split seed, then per epoch the training loader's and the validation loader's shuffles.
+        A rank of a member-parallel ensemble runs this for the members it does not train."""
+        train, val = self._split(dataset)
+        for _ in range(round(self.epochs * epoch_multiplier)):
+            _epoch_permutation(len(train))
+            if val is not None:
+                _epoch_permutation(len(val))
+
+    def _record_final_stats(self, stats: Dict[str, float]) -> None:
+        self.final_stats = stats
+        for k, v in stats.items():
+            self.logger.record(f"reward/final/{k}", v)
 
     # -- the fused step: a minibatch never leaves the device ------------------------------------------------------------
     use_fused_step = True
 
     def _fused_target(self, dataset):
         """(net, pool, base dataset, item indices | None) when the whole training step can run as kernels on the device:
-        cross-entropy loss on a single fused network, every parameter trained by a plain AdamW, equal-length fragments.
+        cross-entropy loss on a single fused network, every parameter trained by a plain AdamW, no regularizer or one of
+        this package's `LpRegularizer` / `WeightDecayRegularizer` (exactly those classes), equal-length fragments.
         Otherwise None: the per-minibatch autograd path below covers everything else."""
         pm = self._preference_model
         if not (self.use_fused_step and type(self.loss) is CrossEntropyRewardLoss and pm.ensemble_model is None
-                and pm.use_fragment_pool and type(self.optim) is th.optim.AdamW and len(self.optim.param_groups) == 1):
+                and pm.use_fragment_pool and type(self.optim) is th.optim.AdamW and len(self.optim.param_groups) == 1
+                and type(self.regularizer) in (type(None), regularizers.LpRegularizer,
+                                               regularizers.WeightDecayRegularizer)):
             return None
         g = self.optim.param_groups[0]
         if g.get("amsgrad") or g.get("maximize") or g.get("capturable") or g.get("differentiable"):
@@ -923,11 +971,7 @@ class BasicRewardTrainer(RewardTrainer):
         if ({id(p) for p in g["params"]} != {id(p) for p in plist} or not all(p.requires_grad for p in plist)
                 or len(dataset) == 0):
             return None
-        index = None
-        while isinstance(dataset, data_th.Subset):  # bagging subsets of the ensemble: resolve to the shared base dataset
-            ind = np.asarray(dataset.indices, dtype=np.int64)
-            index = ind if index is None else ind[index]
-            dataset = dataset.dataset
+        dataset, index = _resolve_subsets(dataset)
         pool = pm._get_pool(net)
         rows = pool.dataset_rows(dataset)
         if rows is None:
@@ -958,88 +1002,172 @@ class BasicRewardTrainer(RewardTrainer):
         fo["state"][_lib.ST_DISC_STEP] = fo["step"]
         return fo
 
-    def _train_fused(self, target, n_items: int, epochs: int) -> None:
+    def _train_fused(self, target, n_items: int, epochs: int, val_index: Optional[np.ndarray] = None) -> None:
         """The reference's loop (:1218-1323) with every minibatch as device work only: row-index gather from the fragment
         pool -> imb_reward_forward -> imb_pref_loss (returns, Boltzmann probability, cross entropy, d loss / d rewards)
         -> imb_disc_fwd_bwd with that upstream gradient (accumulating over the minibatches of a batch) -> reduction +
         AdamW in one launch.  Minibatch composition is the reference's DataLoader(shuffle=True) order (same consumption of
         torch's global RNG, `_epoch_permutation`); losses and accuracies are accumulated on the device and read back once
-        after the last epoch."""
+        after the last epoch.
+
+        With a regularizer, `imb_param_regularize` runs after every training minibatch's fwd_bwd (Lp: its gradient into
+        the accumulator and its value into a statistics slot; weight decay: on the parameters, before the optimiser
+        step).  With a lambda updater, the epoch's validation items (`val_index`, shuffled by their own loader's draw
+        after the training loader's) go through the training-mode forward and imb_pref_loss without a gradient, and the
+        epoch's statistics are read back to hand the scaled training loss and the validation loss to `update_params`;
+        the new lambda applies from the next epoch."""
         net, pool, (R1, R2, prefs_all, has_gt), index = target
         pm = self._preference_model
         e = net.engine()
         e.sync()
         fo = self._fused_optimizer_state(e)
         dev, L = e.params.device, pool.L
+        reg = self.regularizer
+        lp = type(reg) is regularizers.LpRegularizer
+        # statistics slots per epoch: 0 = model loss / accuracy / count, 1 = ground truth; with a regularizer also
+        # 2 = the model statistics of a short last minibatch (so that the scaled loss sum is exact), 3 = the Lp penalty,
+        # 4 / 5 = the validation model / ground truth
+        S = 2 if reg is None else 6
         index_t = None if index is None else th.as_tensor(index)
-        stats = th.zeros(8 * epochs, device=dev)  # per epoch: slot 2k = model loss / accuracy / count, 2k + 1 = ground truth
+        val_t = None if val_index is None else th.as_tensor(val_index)
+        stats = th.zeros(4 * S * epochs, device=dev)
         train_norm = bool(net.training and e.has_norm)
         bufs: Dict[int, Tuple[th.Tensor, int, th.Tensor, th.Tensor]] = {}
         n_steps = 0
-        for epoch_num in range(epochs):
-            accumulated = 0
-            perm = _epoch_permutation(n_items)
-            perm = (perm if index_t is None else index_t[perm]).to(dev)  # the epoch's item order: one upload
-            for s0 in range(0, n_items, self.minibatch_size):
-                ids = perm[s0:s0 + self.minibatch_size]
-                P = int(ids.numel())
-                idx = th.cat([R1.index_select(0, ids), R2.index_select(0, ids)]).reshape(-1)
-                n = 2 * P * L
-                if n not in bufs:
-                    b, ld = e.new_batch(n)
-                    bufs[n] = (b, ld, th.empty(n, device=dev), th.empty(n, device=dev))
-                batch, ld, rews, grad = bufs[n]
-                _lib.gather_rows(pool.table, pool.table.shape[0], pool.tw, idx, n, batch, ld, 0)
-                if train_norm:
-                    e.norm_update(batch, ld, n)
-                if train_norm and e.desc.shaped:  # the training-mode forward of a shaped net reads the mid-update snapshot
-                    rews = reward_nets._FusedForward._fwd_train(e, batch, ld, n)
-                else:
-                    _lib.reward_forward(e.desc, e.params, e.norm_state, batch, ld, n, 0, rews)
-                y = prefs_all.index_select(0, ids)
-                # (an incomplete batch gets proportionally smaller gradients: loss * len / batch_size, :1288-1291)
-                _lib.pref_loss(rews, P, L, y, pm.noise_prob, pm.discount_factor, pm.threshold, P / self.batch_size, grad,
-                               None, stats, 2 * epoch_num)
-                if has_gt:
-                    _lib.pref_loss(pool.rews.index_select(0, idx), P, L, y, pm.noise_prob, pm.discount_factor, pm.threshold,
-                                   0.0, None, None, stats, 2 * epoch_num + 1)
-                e.fwd_bwd(batch, ld, n, n, 0.0, grad, None, accumulated == 0, train_norm and bool(e.desc.shaped))
-                accumulated += P
-                if accumulated >= self.batch_size:
-                    _lib.disc_reduce_adam(e.desc, fo["hp"], e.params, fo["m"], fo["v"], 1.0, e.ws, fo["state"], None)
-                    n_steps += 1
-                    accumulated = 0
-                else:
-                    e.reduce(None)
-            if accumulated != 0:  # an incomplete batch remains
-                _lib.disc_adam(e.desc, fo["hp"], e.params, fo["m"], fo["v"], None, 1.0, e.ws, fo["state"], None)
-                n_steps += 1
-        for p in e._param_list():
-            self.optim.state[p]["step"] = th.tensor(float(fo["step"] + n_steps))
-        st = stats.cpu().numpy().reshape(epochs, 2, 4)  # the one read-back of the training call
+
+        def forward(ids):
+            """Gather the minibatch's 2 P fragments, update the input norm (training mode) and evaluate the rewards."""
+            P = int(ids.numel())
+            idx = th.cat([R1.index_select(0, ids), R2.index_select(0, ids)]).reshape(-1)
+            n = 2 * P * L
+            if n not in bufs:
+                b, ld = e.new_batch(n)
+                bufs[n] = (b, ld, th.empty(n, device=dev), th.empty(n, device=dev))
+            batch, ld, rews, grad = bufs[n]
+            _lib.gather_rows(pool.table, pool.table.shape[0], pool.tw, idx, n, batch, ld, 0)
+            if train_norm:
+                e.norm_update(batch, ld, n)
+            if train_norm and e.desc.shaped:  # the training-mode forward of a shaped net reads the mid-update snapshot
+                rews = reward_nets._FusedForward._fwd_train(e, batch, ld, n)
+            else:
+                _lib.reward_forward(e.desc, e.params, e.norm_state, batch, ld, n, 0, rews)
+            return P, idx, n, batch, ld, rews, grad, prefs_all.index_select(0, ids)
+
+        def epoch_stats(st):
+            """Host statistics of one epoch's [S, 4] slots: (loss sum, accuracy sum, minibatches) of the model."""
+            model = st[0] if S == 2 else st[0] + st[2]
+            return float(model[0]), float(model[1]), max(float(model[2]), 1.0)
+
+        def scaled_loss_sum(st):
+            """Sum over the epoch's training minibatches of loss * P / batch_size (the reference's train_loss)."""
+            short = n_items % self.minibatch_size
+            return (float(st[0, 0]) * self.minibatch_size + float(st[2, 0]) * short) / self.batch_size
+
         with self.logger.accumulate_means("reward"):
+            for epoch_num in range(epochs):
+                slot = S * epoch_num
+                if reg is not None:  # lambda as it stands at the start of the epoch
+                    coeff = (reg.lambda_ if lp else -reg.lambda_ * self.optim.param_groups[0]["lr"])
+                    kind = _lib.REG_LP if lp else _lib.REG_WEIGHT_DECAY
+                accumulated = 0
+                perm = _epoch_permutation(n_items)
+                perm = (perm if index_t is None else index_t[perm]).to(dev)  # the epoch's item order: one upload
+                for s0 in range(0, n_items, self.minibatch_size):
+                    P, idx, n, batch, ld, rews, grad, y = forward(perm[s0:s0 + self.minibatch_size])
+                    mslot = slot + 2 if (reg is not None and P < self.minibatch_size) else slot
+                    # (an incomplete batch gets proportionally smaller gradients: loss * len / batch_size, :1288-1291)
+                    _lib.pref_loss(rews, P, L, y, pm.noise_prob, pm.discount_factor, pm.threshold, P / self.batch_size,
+                                   grad, None, stats, mslot)
+                    if has_gt:
+                        _lib.pref_loss(pool.rews.index_select(0, idx), P, L, y, pm.noise_prob, pm.discount_factor,
+                                       pm.threshold, 0.0, None, None, stats, slot + 1)
+                    e.fwd_bwd(batch, ld, n, n, 0.0, grad, None, accumulated == 0, train_norm and bool(e.desc.shaped))
+                    if reg is not None:
+                        _lib.param_regularize(e.desc, kind, reg.p if lp else 0, coeff, e.params, e.ws, stats, slot + 3)
+                    accumulated += P
+                    if accumulated >= self.batch_size:
+                        _lib.disc_reduce_adam(e.desc, fo["hp"], e.params, fo["m"], fo["v"], 1.0, e.ws, fo["state"], None)
+                        n_steps += 1
+                        accumulated = 0
+                    else:
+                        e.reduce(None)
+                if accumulated != 0:  # an incomplete batch remains
+                    _lib.disc_adam(e.desc, fo["hp"], e.params, fo["m"], fo["v"], None, 1.0, e.ws, fo["state"], None)
+                    n_steps += 1
+                if val_t is None:
+                    continue
+                vperm = val_t[_epoch_permutation(len(val_t))].to(dev)  # the validation loader's shuffle, after training's
+                for s0 in range(0, len(val_t), self.minibatch_size):
+                    P, idx, n, batch, ld, rews, grad, y = forward(vperm[s0:s0 + self.minibatch_size])
+                    _lib.pref_loss(rews, P, L, y, pm.noise_prob, pm.discount_factor, pm.threshold, 1.0, None, None,
+                                   stats, slot + 4)
+                    if has_gt:
+                        _lib.pref_loss(pool.rews.index_select(0, idx), P, L, y, pm.noise_prob, pm.discount_factor,
+                                       pm.threshold, 0.0, None, None, stats, slot + 5)
+                st = stats[4 * slot:4 * (slot + S)].cpu().numpy().reshape(S, 4)  # the epoch's one read-back
+                with self.logger.add_key_prefix(f"epoch-{epoch_num}"):
+                    reg.update_params(scaled_loss_sum(st), float(st[4, 0]))
+            for p in e._param_list():
+                self.optim.state[p]["step"] = th.tensor(float(fo["step"] + n_steps))
+            st = stats.cpu().numpy().reshape(epochs, S, 4)  # (without an updater: the one read-back of the training call)
+            final: Dict[str, float] = {}
             for k in range(epochs):
-                nb = max(float(st[k, 0, 2]), 1.0)
-                self.logger.record(f"epoch-{k}/train/loss", float(st[k, 0, 0]) / nb)
-                self.logger.record(f"epoch-{k}/train/accuracy", float(st[k, 0, 1]) / nb)
+                loss_sum, acc_sum, nb = epoch_stats(st[k])
+                self.logger.record(f"epoch-{k}/train/loss", loss_sum / nb)
+                self.logger.record(f"epoch-{k}/train/accuracy", acc_sum / nb)
                 if has_gt:
                     self.logger.record(f"epoch-{k}/train/gt_reward_loss", float(st[k, 1, 0]) / nb)
-            nb = max(float(st[-1, 0, 2]), 1.0)
-            self.last_epoch_stats = {"loss": float(st[-1, 0, 0]) / nb, "accuracy": float(st[-1, 0, 1]) / nb}
+                final = {}
+                if lp:
+                    final["regularized_loss"] = (scaled_loss_sum(st[k]) + float(st[k, 3, 0])) / max(float(st[k, 3, 2]), 1.0)
+                    with self.logger.add_key_prefix(f"epoch-{k}"):
+                        reg.logger.record("regularized_loss", final["regularized_loss"])
+                if val_t is not None:
+                    nv = max(float(st[k, 4, 2]), 1.0)
+                    final["val/loss"], final["val/accuracy"] = float(st[k, 4, 0]) / nv, float(st[k, 4, 1]) / nv
+                    if has_gt:
+                        final["val/gt_reward_loss"] = float(st[k, 5, 0]) / nv
+                    for key in ("val/loss", "val/accuracy", "val/gt_reward_loss"):
+                        if key in final:
+                            self.logger.record(f"epoch-{k}/{key}", final[key])
+            loss_sum, acc_sum, nb = epoch_stats(st[-1])
+            self.last_epoch_stats = {"loss": loss_sum / nb, "accuracy": acc_sum / nb}
         for k, v in self.last_epoch_stats.items():
             self.logger.record(f"reward/final/train/{k}", v)
+        self._record_final_stats(self._final_regularization_stats(final))
+
+    def _final_regularization_stats(self, last_epoch: Dict[str, float]) -> Dict[str, float]:
+        """The reward/final/ keys the reference copies from the last epoch's regularization records: the validation
+        statistics, and -- when the regularizer records into this trainer's logger -- regularized_loss and lambda."""
+        out = {k: v for k, v in last_epoch.items() if k.startswith("val/")}
+        reg = self.regularizer
+        if reg is not None and reg.logger is self.logger:
+            if "regularized_loss" in last_epoch:
+                out["regularized_loss"] = last_epoch["regularized_loss"]
+            if self.requires_regularizer_update:
+                out["regularization_lambda"] = reg.lambda_
+        return {k: out[k] for k in self.FINAL_KEYS if k in out}
 
     def _train(self, dataset, epoch_multiplier: float = 1.0) -> None:
+        dataset, val_dataset = self._split(dataset)
         epochs = round(self.epochs * epoch_multiplier)
         assert epochs > 0, "Must train for at least one epoch."
         target = self._fused_target(dataset)
         if target is not None:
-            self._train_fused(target, len(dataset), epochs)
+            val_index = None if val_dataset is None else _resolve_subsets(val_dataset)[1]
+            self._train_fused(target, len(dataset), epochs, val_index)
             return
         dataloader = self._make_data_loader(dataset)
+        val_dataloader = self._make_data_loader(val_dataset) if val_dataset is not None else None
+        reg = self.regularizer
+        final: Dict[str, float] = {}
         with self.logger.accumulate_means("reward"):
             for epoch_num in range(epochs):
                 train_loss, accumulated_size, n_batches, acc, loss_sum = 0.0, 0, 0, 0.0, 0.0
+                # whatever this epoch's minibatches record as regularized_loss (any regularizer recording into this
+                # logger): its mean is recovered from the running mean's value and count before and after the epoch
+                reg_key = f"mean/reward/epoch-{epoch_num}/regularized_loss"
+                reg_before = (self.logger.name_to_value.get(reg_key, 0.0), self.logger.name_to_count.get(reg_key, 0))
                 self.optim.zero_grad()
                 for fragment_pairs, preferences in dataloader:
                     out = self.loss.forward(fragment_pairs, preferences, self._preference_model)
@@ -1052,7 +1180,11 @@ class BasicRewardTrainer(RewardTrainer):
                     # averaged over the whole batch instead of the minibatch (an incomplete batch gets smaller gradients)
                     loss = out.loss * (len(fragment_pairs) / self.batch_size)
                     train_loss += loss.item()
-                    loss.backward()
+                    if reg is not None:
+                        with self.logger.add_key_prefix(f"epoch-{epoch_num}"):
+                            reg.regularize_and_backward(loss)
+                    else:
+                        loss.backward()
                     accumulated_size += len(fragment_pairs)
                     if accumulated_size >= self.batch_size:
                         self.optim.step()
@@ -1063,8 +1195,30 @@ class BasicRewardTrainer(RewardTrainer):
                 # `reward/final/train/loss` of the reference = mean over the last epoch's minibatches of the UNSCALED
                 # minibatch loss (logger.record("loss", ...) under accumulate_means, preference_comparisons.py:1296-1323)
                 self.last_epoch_stats = {"loss": loss_sum / max(n_batches, 1), "accuracy": acc / max(n_batches, 1)}
+                final = {}
+                n_reg = self.logger.name_to_count.get(reg_key, 0) - reg_before[1]
+                if n_reg > 0:
+                    v, c = self.logger.name_to_value[reg_key], self.logger.name_to_count[reg_key]
+                    final["regularized_loss"] = v if n_reg == c else (v * c - reg_before[0] * reg_before[1]) / n_reg
+                if val_dataloader is None:
+                    continue
+                # validation: the training-mode forward (an input RunningNorm updates), no backward (:1284-1296)
+                val_loss, val_sums, n_val = 0.0, defaultdict(float), 0
+                for fragment_pairs, preferences in val_dataloader:
+                    out = self.loss.forward(fragment_pairs, preferences, self._preference_model)
+                    self.logger.record(f"epoch-{epoch_num}/val/loss", out.loss.item())
+                    val_sums["val/loss"] += out.loss.item()
+                    for name, value in out.metrics.items():
+                        self.logger.record(f"epoch-{epoch_num}/val/{name}", value.item())
+                        val_sums[f"val/{name}"] += value.item()
+                    val_loss += out.loss.item()
+                    n_val += 1
+                final.update({k: v / max(n_val, 1) for k, v in val_sums.items()})
+                with self.logger.add_key_prefix(f"epoch-{epoch_num}"):
+                    reg.update_params(train_loss, val_loss)
         for k, v in self.last_epoch_stats.items():
             self.logger.record(f"reward/final/train/{k}", v)
+        self._record_final_stats(self._final_regularization_stats(final))
 
 
 class EnsembleTrainer(BasicRewardTrainer):
@@ -1090,8 +1244,8 @@ class EnsembleTrainer(BasicRewardTrainer):
         """Member-parallel training over the ranks of a `torch.distributed` group (one process per GPU, every rank
         constructed with the same seeds and fed the same dataset): member k is trained by rank k % W, on exactly the
         bagging subset and minibatch order it has in a single-process run -- every rank draws every member's subset and
-        consumes the torch-RNG draws of the members it skips -- and after the last member the owners broadcast their
-        members' parameters, RunningNorm statistics and AdamW state.  Every rank ends with all members, bit-identical to
+        makes the draws of the members it skips (`_skip_draws`) -- and after the last member the owners broadcast their
+        members' parameters, RunningNorm statistics, AdamW state, regularizer strength and final statistics.  Every rank ends with all members, bit-identical to
         the single-process result.  Additive API: the reference trains the members one after the other in one process
         (:1417-1424)."""
         import torch.distributed as dist
@@ -1112,7 +1266,10 @@ class EnsembleTrainer(BasicRewardTrainer):
             e = net.engine()
             e.sync()
             states.append((e, t._fused_optimizer_state(e)))  # (creates the flat moments on the ranks that skipped it)
-        meta = th.zeros(len(trainers), 3, dtype=th.float64, device=states[0][0].params.device)
+        # per member: loss, accuracy, step count, lambda, then FINAL_KEYS (NaN: not recorded); float64 holds the Python
+        # floats exactly, the all-reduce adds only zeros to the owner's row
+        keys = self.FINAL_KEYS
+        meta = th.zeros(len(trainers), 4 + len(keys), dtype=th.float64, device=states[0][0].params.device)
         for k, (t, (e, fo)) in enumerate(zip(trainers, states)):
             src = k % W if group is None else dist.get_global_rank(group, k % W)
             for x in (e.params, fo["m"], fo["v"]) + ((e.norm_state, e.norm_count) if e.has_norm else ()):
@@ -1120,12 +1277,17 @@ class EnsembleTrainer(BasicRewardTrainer):
             if k % W == rank:
                 meta[k, 0], meta[k, 1] = t.last_epoch_stats["loss"], t.last_epoch_stats["accuracy"]
                 meta[k, 2] = float(t.optim.state[e._param_list()[0]]["step"])
+                meta[k, 3] = float(t.regularizer.lambda_) if t.regularizer is not None else 0.0
+                meta[k, 4:] = th.tensor([t.final_stats.get(key, float("nan")) for key in keys], dtype=th.float64)
         dist.all_reduce(meta, group=group)
         meta = meta.cpu()
         for k, (t, (e, fo)) in enumerate(zip(trainers, states)):
             t.last_epoch_stats = {"loss": float(meta[k, 0]), "accuracy": float(meta[k, 1])}
             for p in e._param_list():
                 t.optim.state[p]["step"] = th.tensor(float(meta[k, 2]))
+            if t.regularizer is not None:
+                t.regularizer.lambda_ = float(meta[k, 3])
+            t.final_stats = {key: float(meta[k, 4 + j]) for j, key in enumerate(keys) if not math.isnan(meta[k, 4 + j])}
 
     def _train(self, dataset, epoch_multiplier: float = 1.0) -> None:
         sampler = data_th.RandomSampler(dataset, replacement=True, num_samples=len(dataset),
@@ -1136,18 +1298,23 @@ class EnsembleTrainer(BasicRewardTrainer):
             bagging_dataset = data_th.Subset(dataset, list(sampler))
             if member_idx % W == rank:
                 trainer.train(bagging_dataset, epoch_multiplier=epoch_multiplier)
-            else:  # another rank's member: consume the draws its epochs make from torch's global RNG
-                for _ in range(round(trainer.epochs * epoch_multiplier)):
-                    _epoch_permutation(len(bagging_dataset))
+            else:  # another rank's member: make the draws its training makes from self.rng and torch's global RNG
+                trainer._skip_draws(bagging_dataset, epoch_multiplier)
         if W > 1:
             self._sync_members()
+        final = defaultdict(list)
         for trainer in self.member_trainers:
             for k, v in trainer.last_epoch_stats.items():
                 stats[k].append(v)
+            for k, v in trainer.final_stats.items():
+                final[k].append(v)
         self.last_epoch_stats = {k: float(np.mean(v)) for k, v in stats.items()}
         for k, v in stats.items():
             self.logger.record(f"reward/final/train/{k}", float(np.mean(v)))
             self.logger.record(f"reward/final/train/{k}_std", float(np.std(v)))
+        for k, v in final.items():  # the regularization keys: member mean and standard deviation (:1426-1438)
+            self.logger.record(f"reward/final/{k}", float(np.mean(v)))
+            self.logger.record(f"reward/final/{k}_std", float(np.std(v)))
 
 
 def _make_reward_trainer(preference_model: PreferenceModel, loss: RewardLoss, rng: np.random.Generator,

@@ -636,6 +636,55 @@ __global__ void __launch_bounds__(256) k_disc_reduce_adam(int P, const float* __
   if (threadIdx.x == 0 && stats_out) train_stats<true>(stats, meta, stats_out);
 }
 
+// ---- regularization of the reward model's training step (imb_param_regularize) --------------------------------------
+// x^k for an integer k >= 0 by repeated squaring in float32
+__device__ __forceinline__ float powi_f(float x, int k) {
+  float r = 1.f;
+  while (k > 0) {
+    if (k & 1) r *= x;
+    x *= x;
+    k >>= 1;
+  }
+  return r;
+}
+
+// Single block, like k_disc_adam.  IMB_REG_LP: gacc += coeff * p sign(w) |w|^(p-1) and, when stats is given,
+// stats[0] += coeff * sum |w|^p, stats[2] += 1 -- the sum in a fixed order (per-thread strided sums, then a fixed
+// shuffle tree and warp order), so two launches give the same bits.  IMB_REG_WEIGHT_DECAY: w = w + coeff * w as two
+// separately rounded ops (torch's th.add(w, c * w)).
+__global__ void __launch_bounds__(1024) k_param_regularize(int P, int kind, int p, float coeff,
+                                                         float* __restrict__ params, float* __restrict__ gacc,
+                                                         float* __restrict__ stats) {
+  if (kind == IMB_REG_WEIGHT_DECAY) {
+    for (int i = threadIdx.x; i < P; i += blockDim.x) {
+      const float w = params[i];
+      params[i] = __fadd_rn(w, __fmul_rn(coeff, w));
+    }
+    return;
+  }
+  const float fp = (float)p;
+  float s = 0.f;
+  for (int i = threadIdx.x; i < P; i += blockDim.x) {
+    const float w = params[i], a = fabsf(w);
+    const float a_pm1 = powi_f(a, p - 1);  // |w|^(p-1); 1 for p = 1
+    const float g = w > 0.f ? fp * a_pm1 : (w < 0.f ? -fp * a_pm1 : 0.f);  // d |w|^p / dw, 0 at w = 0
+    gacc[i] = __fadd_rn(gacc[i], __fmul_rn(coeff, g));
+    s += a_pm1 * a;
+  }
+  if (!stats) return;
+  __shared__ float s_part[32];
+  s = warp_sum(s);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (lane == 0) s_part[warp] = s;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float t = 0.f;
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += s_part[w];
+    stats[0] += coeff * t;
+    stats[2] += 1.f;
+  }
+}
+
 // ---- preference comparisons: fragment returns -> Boltzmann probability -> cross entropy (+ its gradient) -------------
 // PreferenceModel.probability (algorithms/preference_comparisons.py:487-530) from the (discounted) return difference
 // s = sum_t g^t (r2 - r1): d = clip(s, -threshold, threshold), m = 1 / (1 + e^d), p = noise / 2 + (1 - noise) m.
@@ -1285,6 +1334,21 @@ extern "C" int imb_disc_reduce_adam(const imb_disc_desc* d, const imb_adam* opt,
       reinterpret_cast<const int*>(ws + w.meta), state + IMB_ST_DISC_STEP, stats_out,
       reinterpret_cast<unsigned int*>(ws + w.ticket) + 8);
   IMB_CHECK_LAUNCH("k_disc_reduce_adam");
+  return 0;
+}
+
+extern "C" int imb_param_regularize(const imb_disc_desc* d, int32_t kind, int32_t p, float coeff, float* params,
+                                    float* ws, float* stats_acc, int32_t stats_slot, void* stream) {
+  IMB_REQUIRE(kind == IMB_REG_LP || kind == IMB_REG_WEIGHT_DECAY,
+              "imb_param_regularize: kind %d (%d Lp, %d weight decay)", kind, IMB_REG_LP, IMB_REG_WEIGHT_DECAY);
+  IMB_REQUIRE(kind != IMB_REG_LP || p >= 1, "imb_param_regularize: p = %d, the Lp penalty needs an integer p >= 1", p);
+  IMB_REQUIRE(kind != IMB_REG_LP || ws != nullptr, "imb_param_regularize: the Lp penalty needs the workspace");
+  IMB_REQUIRE(stats_slot >= 0, "imb_param_regularize: bad statistics slot");
+  IMB_REQUIRE(d->n_params >= 1, "imb_param_regularize: no parameters");
+  float* gacc = kind == IMB_REG_LP ? ws + ws_layout(d->n_params).gacc : nullptr;
+  float* stats = kind == IMB_REG_LP && stats_acc ? stats_acc + 4 * stats_slot : nullptr;
+  k_param_regularize<<<1, 1024, 0, (cudaStream_t)stream>>>(d->n_params, kind, p, coeff, params, gacc, stats);
+  IMB_CHECK_LAUNCH("k_param_regularize");
   return 0;
 }
 

@@ -8,7 +8,7 @@ import csv
 import os
 import sys
 import tempfile
-from typing import Any, Dict, Optional, Sequence
+from typing import Any, Dict, List, Optional, Sequence
 
 
 class _Writer:
@@ -63,7 +63,7 @@ class HierarchicalLogger:
         self.name_to_value: Dict[str, Any] = collections.defaultdict(float)
         self.name_to_count: Dict[str, int] = collections.defaultdict(int)
         self._prefix: Optional[str] = None
-        self._key_prefix: Optional[str] = None
+        self._key_prefixes: List[str] = []
         self.history = []
 
     def get_dir(self):
@@ -81,6 +81,17 @@ class HierarchicalLogger:
             self._prefix = old
 
     @contextlib.contextmanager
+    def add_key_prefix(self, prefix: str):
+        """Inside `accumulate_means`: record(key) records `<prefix>/key` (nested prefixes are joined in order)."""
+        if self._prefix is None:
+            raise RuntimeError("Cannot add key prefix when accumulate_means context is not active.")
+        self._key_prefixes.append(prefix)
+        try:
+            yield
+        finally:
+            self._key_prefixes.pop()
+
+    @contextlib.contextmanager
     def accumulate_means(self, name: str):
         if self._prefix is not None:
             raise RuntimeError("Nested `accumulate_means` context")
@@ -92,6 +103,7 @@ class HierarchicalLogger:
 
     def record(self, key: str, val: Any, exclude=None) -> None:
         if self._prefix is not None:
+            key = "/".join(self._key_prefixes + [key])
             self.name_to_value[f"raw/{self._prefix}/{key}"] = val
             self.record_mean(f"mean/{self._prefix}/{key}", val, _direct=True)
         else:

@@ -396,6 +396,22 @@ int imb_pref_loss(const float* rews, int64_t n_pairs, int32_t frag_len, const fl
                   float discount, float threshold, float grad_scale, float* grad_rews, float* probs_out,
                   float* stats_acc, int32_t stats_slot, void* stream);
 
+/* Regularization of the reward model's training step (regularization/regularizers.py), on the flat parameter vector
+ * params[d->n_params], one single-CTA launch per minibatch:
+ *  IMB_REG_LP (LpRegularizer, coeff = lambda): adds coeff * p * sign(w) |w|^(p-1) (the gradient of
+ *    lambda * sum_tensors ||w||_p^p; 0 at w = 0) to the gradient accumulator of ws, so it goes between imb_disc_fwd_bwd
+ *    (which clears the accumulator with IMB_F_ZERO_GRAD) and imb_disc_reduce / imb_disc_reduce_adam (which add the
+ *    minibatch's gradient to it).  Statistics slot `stats_slot` of stats_acc (optional; imb_pref_loss's layout):
+ *    [0] += coeff * sum |w|^p, [2] += 1, the sum without atomics (two calls give the same bits).
+ *  IMB_REG_WEIGHT_DECAY (WeightDecayRegularizer, coeff = (float)(-lambda * lr)): w = w + coeff * w, a float32
+ *    multiply then a float32 add (torch's th.add(w, c * w), bit for bit); ws and stats_acc are not used.  Goes after
+ *    imb_disc_fwd_bwd has read the parameters and before the optimiser step.
+ * p is an integer >= 1 (ignored by weight decay).  Stream-ordered, no allocation. */
+#define IMB_REG_LP 1
+#define IMB_REG_WEIGHT_DECAY 2
+int imb_param_regularize(const imb_disc_desc* d, int32_t kind, int32_t p, float coeff, float* params, float* ws,
+                         float* stats_acc, int32_t stats_slot, void* stream);
+
 /* Active selection of preference queries: ActiveSelectionFragmenter.__call__ + variance_estimate
  * (algorithms/preference_comparisons.py:721-778), which loops over the candidate pairs in Python and calls
  * PreferenceModel.rewards -> RewardEnsemble.predict_processed_all (rewards/reward_nets.py:926-951) -> each member's
