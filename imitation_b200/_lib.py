@@ -102,6 +102,12 @@ PPO_STAT_FLOATS = 16
 PU_MODES = {"logit": 0, "probability": 1, "label": 2}
 # imb_param_regularize kinds
 REG_LP, REG_WEIGHT_DECAY = 1, 2
+# imb_density_score: demonstration tile rows, widest feature vector, kernels (sklearn's names) and segment modes
+DENSITY_TILE, DENSITY_MAX_D = 64, 128
+KDE_GAUSSIAN, KDE_TOPHAT, KDE_EPANECHNIKOV, KDE_EXPONENTIAL, KDE_LINEAR, KDE_COSINE = 0, 1, 2, 3, 4, 5
+KDE_KERNELS = {"gaussian": KDE_GAUSSIAN, "tophat": KDE_TOPHAT, "epanechnikov": KDE_EPANECHNIKOV,
+               "exponential": KDE_EXPONENTIAL, "linear": KDE_LINEAR, "cosine": KDE_COSINE}
+DENSITY_SEG_NONE, DENSITY_SEG_STEPS, DENSITY_SEG_ROLLOUT = 0, 1, 2
 
 _disc, _adam, _pol, _env, _hp, _pu, _members, _sync = map(C.POINTER, (
     DiscDesc, Adam, PolicyDesc, EnvDesc, PpoHparams, PrefUncDesc, RolloutMembers, SyncDesc))
@@ -155,6 +161,9 @@ SIGNATURES = {
     "imb_ensemble_relabel": (_i32, [_pu, _f32, _ptr, _i32, _i32, _i64, _i64, _ptr, _ptr], None),
     "imb_rollout_explore": (_i32, [_env, _ptr, _ptr, _pol, _i32, _ptr, _ptr, _disc, _ptr, _ptr, _members, _i32, _hp,
                                    _i64, _i64, _ptr, _ptr, _ptr, _ptr, _i32, _ptr, _u64, _i64, _ptr, _ptr], 1),
+    "imb_density_ws_floats": (_i64, [_i64], 0),
+    "imb_density_score": (_i32, [_i32, _i32, _i32, _i32, _i32, _i32, _f32, _i32, _i64, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr,
+                                 _ptr, _i32, _ptr, _i64, _i32, _ptr, _ptr, _i64, _i64, _i32, _ptr, _i64, _ptr, _ptr], None),
     "imb_sync_buffer_doubles": (_i64, [_sync], 0),
     "imb_sync_snapshot": (_i32, [_sync, _ptr, _ptr], None),
     "imb_sync_pack": (_i32, [_sync, _ptr, _ptr], 1),
@@ -476,6 +485,24 @@ def rollout_explore(env, env_params, env_obs, pol, pol_params, pol_norm, disc, d
                                      members, reward_mode, hp, n_envs, n_steps, _p(rollout_tbl, th.float32),
                                      _p(flat_out), _p(aux, th.float32), _p(noise), flags, _p(explore_policy, th.uint8),
                                      explore_seed, explore_step0, _p(state, th.int64), _stream()), "imb_rollout_explore")
+
+
+def density_ws_floats(n_query: int) -> int:
+    return lib().imb_density_ws_floats(n_query)
+
+
+def density_score(model, src, src_ld, n_query, out, out_stride, ws, seg_mode=DENSITY_SEG_NONE, row_map=None, steps=None,
+                  state=None, n_envs=0, n_steps=0, horizon=0):
+    """Kernel density log-likelihood of n_query source rows (imb_density_score).  model: an object with the
+    imb_density_score model arguments as attributes (algorithms/density.py's DeviceDensity); out[row * out_stride]."""
+    m = model
+    _check(lib().imb_density_score(m.d, m.col0, m.n0, m.col1, m.n1, m.kernel, m.bandwidth, m.n_seg, m.n_demo,
+                                   _p(m.demo, th.float32), _p(m.demo_seg, th.int32), _p(m.seg_off, th.int64),
+                                   _p(m.seg_const, th.float64), _p(m.mean, th.float32), _p(m.scale, th.float32),
+                                   _p(src, th.float32), src_ld, _p(row_map, th.int64), n_query, seg_mode,
+                                   _p(steps, th.int64), _p(state, th.int64), n_envs, n_steps, horizon,
+                                   _p(out, th.float32), out_stride, _p(ws, th.float32),
+                                   _stream()), "imb_density_score", 1 if n_query > 0 else 0)
 
 
 def gae(rollout_tbl, rw, col_value, n_envs, n_steps, aux, gamma, gae_lambda, state, horizon):

@@ -82,7 +82,8 @@ class DevicePPO:
         self._tbl = None
         self._aux = None
         self._ens_raw = None      # ensemble reward: the members' raw rewards [M][T][E]
-        self._ens_ws = None       # ensemble reward: the relabel's workspace
+        self._ens_ws = None       # ensemble reward: the relabel's workspace (density reward: the score's workspace)
+        self._dens_flat = None    # density reward without a BufferingWrapper: the transition rows it scores
         # buffers of exploration_rollout (table, flat rows, aux, ensemble raw rewards and workspace): never captured
         self._x_tbl = self._x_flat = self._x_aux = self._x_raw = self._x_ws = None
         self.loss_log = None      # optional [n_minibatch_steps][4] device tensor (parity tests)
@@ -137,7 +138,7 @@ class DevicePPO:
         t0 = env.host_ep_step
         ring_args = (ring.table if ring is not None else None, ring.capacity if ring is not None else 0)
 
-        def launch(disc, dparams, dnorm, mode, members):
+        def launch(disc, dparams, dnorm, mode, members, flat):
             if members is None:
                 _lib.rollout(env.desc, env.params, env.obs, pol.desc, pp, pn, disc, dparams, dnorm, mode, self.hp, E, T,
                              self._tbl, *ring_args, flat, self._aux, self.noise, env.state, act=pol.act)
@@ -145,7 +146,8 @@ class DevicePPO:
                 _lib.rollout_ensemble(env.desc, env.params, env.obs, pol.desc, pp, pn, disc, members, self.hp, E, T,
                                       self._tbl, *ring_args, flat, self._aux, self.noise, env.state, act=pol.act)
 
-        self._ens_raw, self._ens_ws = self._relabelled_rollout(launch, self._tbl, E, T, self._ens_raw, self._ens_ws)
+        self._ens_raw, self._ens_ws = self._relabelled_rollout(launch, self._tbl, flat, t0, E, T, self._ens_raw,
+                                                               self._ens_ws)
         da = 1 if pol.discrete else pol.d_act
         col_val = pol.d_obs + da + 1
         _lib.gae(self._tbl, rw, col_val, E, T, self._aux, self.hp.gamma, self.hp.gae_lambda, env.state, env.horizon)
@@ -153,30 +155,48 @@ class DevicePPO:
         if not self._capturing:
             self.after_rollout_host(t0)
 
-    def _relabelled_rollout(self, launch, tbl, E: int, T: int, ens_raw, ens_ws):
+    def _relabelled_rollout(self, launch, tbl, flat, t0: int, E: int, T: int, ens_raw, ens_ws):
         """Launch a rollout over the learned reward the RewardVecEnvWrapper describes, then finish its reward column
-        (rewards/reward_wrapper.py:92-133 -> predict_processed): a NormalizedRewardNet's output normalisation, or the
-        ensemble's per-member normalisation and mean + alpha * std, advancing the output statistics once per env step.
-        launch(disc, disc_params, disc_norm, reward_mode, members) issues the rollout itself (members: the ensemble's
-        member table, else None).  ens_raw / ens_ws: the ensemble's buffers, reused when their size fits; returns them
-        (a captured graph bakes the training rollout's in, so every rollout keeps its own)."""
+        (rewards/reward_wrapper.py:92-133 -> predict_processed): a NormalizedRewardNet's output normalisation, the
+        ensemble's per-member normalisation and mean + alpha * std, advancing the output statistics once per env step,
+        or a DensityAlgorithm's log density of every transition row.
+        launch(disc, disc_params, disc_norm, reward_mode, members, flat) issues the rollout itself (members: the
+        ensemble's member table, else None; flat: its transition rows, None when nobody reads them).  t0: the episode
+        step the rollout starts at.  ens_raw / ens_ws: the ensemble's buffers (ens_ws: the density relabel's workspace
+        for a density reward), reused when their size fits; returns them (a captured graph bakes the training rollout's
+        in, so every rollout keeps its own)."""
         disc = dparams = dnorm = members = None
-        mode, out_norm, ens = 0, None, None
+        mode, out_norm, ens, dens = 0, None, None, None
         if self._rw_wrapper is not None:
             net, mode, out_norm = self._rw_wrapper.resolve()
             if isinstance(net, reward_wrapper.EnsembleRelabel):
                 ens = net
+            elif isinstance(net, reward_wrapper.DensityRelabel):
+                dens = net
             else:
                 eng = net.engine()
                 disc, dparams, dnorm = eng.desc, eng.params, eng.norm_state
         if ens is not None:
             ens_raw, ens_ws, members, relabel = self._ensemble_tables(ens, E, T, ens_raw, ens_ws)
             disc = ens.nets[0].engine().desc
-        launch(disc, dparams, dnorm, mode, members)
+        env = self._base_env
+        if dens is not None:
+            dens.check_steps(t0, T, env.horizon)
+            if flat is None:  # no BufferingWrapper: the relabel reads rows of its own
+                tw = 2 * env.d_obs + env.d_act + 1
+                if self._dens_flat is None or self._dens_flat.shape[0] != E * T:
+                    self._dens_flat = th.zeros(E * T, tw, device=self.device)
+                flat = self._dens_flat
+            n_ws = _lib.density_ws_floats(E * T)
+            if ens_ws is None or ens_ws.numel() != n_ws:
+                ens_ws = th.zeros(n_ws, device=self.device)  # zero-filled: the score's tickets start at 0
+        launch(disc, dparams, dnorm, mode, members, flat)
         pol = self.policy
         rw = tbl.shape[1]
         col_rew = pol.d_obs + (1 if pol.discrete else pol.d_act) + 2
-        if ens is not None:
+        if dens is not None:
+            dens.relabel(flat, tbl, col_rew, E, T, env.horizon, ens_ws, env.state)
+        elif ens is not None:
             _lib.ensemble_relabel(relabel, ens.alpha, tbl, rw, col_rew, E, T, ens_ws)
         elif out_norm is not None:
             ns, nc = out_norm.output_norm_vectors()
@@ -227,12 +247,13 @@ class DevicePPO:
         vec = th.as_tensor(np.ascontiguousarray(explore_policy, dtype=np.uint8)).to(self.device)
         flags = _lib.IMB_RF_DETERMINISTIC if deterministic else 0
 
-        def launch(disc, dparams, dnorm, mode, members):
+        def launch(disc, dparams, dnorm, mode, members, flat):
             _lib.rollout_explore(env.desc, env.params, env.obs, pol.desc, pp, pn, disc, dparams, dnorm, members, mode,
-                                 self.hp, E, T, self._x_tbl, self._x_flat, self._x_aux, noise, vec, seed, step0,
+                                 self.hp, E, T, self._x_tbl, flat, self._x_aux, noise, vec, seed, step0,
                                  env.state, flags=flags, act=pol.act)
 
-        self._x_raw, self._x_ws = self._relabelled_rollout(launch, self._x_tbl, E, T, self._x_raw, self._x_ws)
+        self._x_raw, self._x_ws = self._relabelled_rollout(launch, self._x_tbl, self._x_flat, 0, E, T, self._x_raw,
+                                                           self._x_ws)
         _lib.rollout_advance(env.state, E, T, H, 0)
         env.host_ep_step = 0
         return self._x_flat, self._x_aux[2 * E + E * T:].view(E, T)
@@ -298,6 +319,9 @@ class DevicePPO:
                     if o is not None:
                         key += [t.data_ptr() for t in o.output_norm_vectors()]
                         key += [o.output_norm_is_ema, getattr(o.normalize_output_layer, "decay", None)]
+            elif isinstance(net, reward_wrapper.DensityRelabel):
+                key += list(net.pointer_key())
+                key += [t.data_ptr() if t is not None else 0 for t in (self._ens_ws, self._dens_flat)]
             else:
                 eng = net.engine()
                 key += [eng.params.data_ptr(), eng.norm_state.data_ptr(), mode, id(out_norm)]
@@ -340,6 +364,10 @@ class DevicePPO:
             self._graph_launches = _lib.LAUNCHES["count"] - before
             _lib.LAUNCHES["count"] = before
         t0 = self._base_env.host_ep_step
+        if self._rw_wrapper is not None:
+            net = self._rw_wrapper.resolve()[0]
+            if isinstance(net, reward_wrapper.DensityRelabel):
+                net.check_steps(t0, self.n_steps, self._base_env.horizon)  # the replayed launches take no host check
         self._graph[0].replay()
         self.ev_rollout.record()
         self._graph[1].replay()

@@ -44,6 +44,18 @@ static inline int imb_num_sms() {
   return n;
 }
 
+// Flattened (reference-order) index of local step t of env e in a rollout of T steps of E lock-step envs of horizon H
+// that starts at episode step t0: the order pop_trajectories + flatten_trajectories give (finished trajectories in
+// completion order, then the partial ones in env order; imb_rollout_impl.cuh).  The rollout writes its transition rows
+// there and imb_density_score reads them back from there.
+__device__ __forceinline__ int64_t flat_index(int64_t e, int64_t t, int64_t E, int64_t T, int64_t t0, int64_t H) {
+  const int64_t seg = (t0 + t) / H;
+  const int64_t start = seg == 0 ? 0 : seg * H - t0;
+  int64_t end = (seg + 1) * H - t0;
+  if (end > T) end = T;
+  return E * start + e * (end - start) + (t - start);
+}
+
 // ---- warp helpers ---------------------------------------------------------------------------
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

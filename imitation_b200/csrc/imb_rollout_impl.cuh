@@ -66,15 +66,6 @@ struct RolloutExplore {
   int64_t step0;
 };
 
-// flattened (reference-order) index of local step t of env e; see file header
-__device__ __forceinline__ int64_t flat_index(int64_t e, int64_t t, int64_t E, int64_t T, int64_t t0, int64_t H) {
-  const int64_t seg = (t0 + t) / H;
-  const int64_t start = seg == 0 ? 0 : seg * H - t0;
-  int64_t end = (seg + 1) * H - t0;
-  if (end > T) end = T;
-  return E * start + e * (end - start) + (t - start);
-}
-
 // ENS: evaluate the Mb.M ensemble members (raw outputs to Mb.raw) instead of the one net at disc_params (reward column);
 // the single-net variant has no member loop.  ACT: the policy towers' activation (env and reward net keep their own).
 // EXP: the exploration rollout, Xp.policy[t] picks the policy of step t (random steps skip the policy towers and

@@ -43,10 +43,16 @@ class RewardVecEnvWrapper:
 
     def resolve(self):
         """-> (fused net with engine, reward_mode, NormalizedRewardNet or None) for the rollout kernel; for an ensemble
-        reward (`AddSTDRewardWrapper(RewardEnsemble)` or a bare `RewardEnsemble`) -> (EnsembleRelabel, 2, None)."""
+        reward (`AddSTDRewardWrapper(RewardEnsemble)` or a bare `RewardEnsemble`) -> (EnsembleRelabel, 2, None); for a
+        `DensityAlgorithm` reward -> (DensityRelabel, 0, None)."""
+        from ..algorithms import density
+
+        if isinstance(self.reward_fn, density.DensityAlgorithm):
+            return DensityRelabel(self.reward_fn), 0, None
         net = getattr(self.reward_fn, "__self__", None)
         if not isinstance(net, reward_nets.RewardNet) or getattr(self.reward_fn, "__name__", "") != "predict_processed":
-            raise NotImplementedError("RewardVecEnvWrapper on the GPU path needs reward_fn = <RewardNet>.predict_processed")
+            raise NotImplementedError("RewardVecEnvWrapper on the GPU path needs reward_fn = <RewardNet>.predict_processed "
+                                      "or a DensityAlgorithm")
         if isinstance(net, (reward_nets.AddSTDRewardWrapper, reward_nets.RewardEnsemble)):
             # built once per ensemble (its checks sync every member's engine); rebuilt when the members change
             ens = net.base if isinstance(net, reward_nets.AddSTDRewardWrapper) else net
@@ -117,3 +123,36 @@ class EnsembleRelabel:
     @property
     def alpha(self) -> float:
         return float(self.wrapper.default_alpha) if self.wrapper is not None else 0.0
+
+
+class DensityRelabel:
+    """A `DensityAlgorithm` reward as the rollout applies it: the rollout runs with the env reward (mode 0), then one
+    `imb_density_score` launch overwrites its reward column from the terminal-fixed transition rows it wrote, before
+    GAE.  A non-stationary model scores episode step t with its segment t."""
+
+    def __init__(self, algo):
+        self.algo = algo
+
+    @property
+    def model(self):
+        return self.algo.device_model
+
+    def check_steps(self, t0: int, n_steps: int, horizon: int) -> None:
+        """The reference's error for an episode step the model has no segment for, raised on the host before the
+        rollout of n_steps from episode step t0 is launched."""
+        bad = self.algo.out_of_range_step(t0, n_steps, horizon)
+        if bad is not None:
+            raise ValueError(f"Time {bad} out of range (0, {self.model.n_seg}], and absorbing states not currently "
+                             "supported")
+
+    def relabel(self, flat, tbl, col_rew: int, n_envs: int, n_steps: int, horizon: int, ws, state) -> None:
+        """tbl[(e * T + t), col_rew] = log density of the flattened row of (e, t) in flat (imb_rollout's flat_out)."""
+        _lib.density_score(self.model, flat, flat.shape[1], n_envs * n_steps, tbl.view(-1)[col_rew:], tbl.shape[1],
+                           ws, seg_mode=_lib.DENSITY_SEG_ROLLOUT, state=state, n_envs=n_envs, n_steps=n_steps,
+                           horizon=horizon)
+
+    def pointer_key(self) -> tuple:
+        """Every launch argument of relabel() that a captured graph bakes in, besides the caller's buffers."""
+        m = self.model
+        return (m.d, m.col0, m.n0, m.col1, m.n1, m.kernel, m.bandwidth, m.n_seg, m.n_demo) + tuple(
+            t.data_ptr() for t in m.tensors())

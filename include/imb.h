@@ -501,6 +501,59 @@ int imb_rollout_explore(const imb_env_desc* env, const float* env_params, float*
                         const float* noise, int flags, const uint8_t* explore_policy, uint64_t explore_seed,
                         int64_t explore_step0, const int64_t* state, void* stream);
 
+/* ---- density-based reward (algorithms/density.py) ----------------------------------------------------------------------
+ * DensityAlgorithm.__call__ (:295-360), which calls sklearn KernelDensity.score once per transition:
+ *   r = log( (1/N_s) sum_i K_h(x - x_i) ),  x = (features - mean) / scale,
+ * over the N_s standardised demonstration rows of segment s (a stationary model has one segment, a non-stationary one a
+ * segment per episode step).  The query features are columns [col0, col0 + n0) then [col1, col1 + n1) of a source row in
+ * transition-table format (state: obs; state-action: obs | act; state-state: obs | next_obs).
+ * Demonstrations: n_tiles = ceil(N / IMB_DENSITY_TILE) tiles of IMB_DENSITY_TILE rows, grouped by segment in order,
+ * demo[tile][k][row] feature-major inside a tile (so one bulk copy stages a tile), and demo_seg[tile][row] = the row's
+ * segment, -1 for the padding rows of the last tile; seg_off[n_seg + 1] = each segment's first row (and N);
+ * seg_const[n_seg] = sklearn's log kernel normalisation for (h, D, kernel) minus log N_s (float64).
+ * Arithmetic: fp32 direct differences sum_k (q_k - x_k)^2 (no |q|^2 + |x|^2 - 2 q.x expansion), an online log-sum-exp
+ * per query in fp32, then max + log(sum) + seg_const in float64, rounded to float32.  A compact kernel counts a pair
+ * when d < h (fp32), as sklearn does; a query with no pair counted scores -inf.  Exact: sklearn's tree evaluation
+ * with atol = rtol = 0 is not (DESIGN.md). */
+#define IMB_DENSITY_TILE 64
+#define IMB_DENSITY_MAX_D 128
+#define IMB_KDE_GAUSSIAN 0
+#define IMB_KDE_TOPHAT 1
+#define IMB_KDE_EPANECHNIKOV 2
+#define IMB_KDE_EXPONENTIAL 3
+#define IMB_KDE_LINEAR 4
+#define IMB_KDE_COSINE 5
+/* The model (arguments d .. scale):
+ *  d: the feature width D, 1 .. IMB_DENSITY_MAX_D; the features of a query are its source row's columns
+ *     [col0, col0 + n0) then [col1, col1 + n1), n0 + n1 = D;
+ *  kernel: IMB_KDE_*; bandwidth h > 0;
+ *  n_seg segments of n_demo rows in all: demo [n_tiles][D][IMB_DENSITY_TILE] floats, demo_seg [n_tiles][IMB_DENSITY_TILE],
+ *  seg_off [n_seg + 1], seg_const [n_seg] as described above; mean, scale [D]: the scaler. */
+/* Query segments (seg_mode):
+ *  IMB_DENSITY_SEG_NONE    query q reads source row q (row_map == NULL) or row_map[q], segment 0, writes out[row * out_stride];
+ *  IMB_DENSITY_SEG_STEPS   as NONE with segment steps[q] (a host-provided steps vector; queries sorted by segment run
+ *                          fastest, since a query tile reads only the demonstration tiles of its segments);
+ *  IMB_DENSITY_SEG_ROLLOUT the E*T steps of the rollout that started at episode step t0 = state[IMB_ST_EP_STEP] (read on
+ *                          the device: the launch can be captured in a graph): query q = t * E + e reads the flattened row
+ *                          flat_index(e, t, E, T, t0, horizon) of `src` (imb_rollout's flat_out), has segment
+ *                          (t0 + t) mod horizon, 0 when n_seg = 1 (a caller with n_seg > 1 checks that the episode
+ *                          steps stay below n_seg), and writes out[(e * T + t) * out_stride] (the rollout table's reward
+ *                          column); n_query = n_envs * n_steps.
+ * A query whose segment is outside [0, n_seg) scores NaN.  When there are too few query tiles to fill the GPU, each
+ * tile's demonstration tiles are split over several CTAs and the last one to finish (ticket) combines the partial sums
+ * in split order; the split depends only on the shapes, so two calls give bit-identical results.
+ * ws: imb_density_ws_floats(n_query) floats, zero-filled when allocated (it holds launch tickets every call re-arms).
+ * One launch. */
+#define IMB_DENSITY_SEG_NONE 0
+#define IMB_DENSITY_SEG_STEPS 1
+#define IMB_DENSITY_SEG_ROLLOUT 2
+int64_t imb_density_ws_floats(int64_t n_query);
+int imb_density_score(int32_t d, int32_t col0, int32_t n0, int32_t col1, int32_t n1, int32_t kernel, float bandwidth,
+                      int32_t n_seg, int64_t n_demo, const float* demo, const int32_t* demo_seg, const int64_t* seg_off,
+                      const double* seg_const, const float* mean, const float* scale, const float* src, int32_t src_ld,
+                      const int64_t* row_map, int64_t n_query, int32_t seg_mode, const int64_t* steps, const int64_t* state, int64_t n_envs,
+                      int64_t n_steps, int32_t horizon, float* out, int64_t out_stride, float* ws, void* stream);
+
 /* ---- multi-GPU: replica state around the ONE all-reduce of a round ---------------------------
  * (SURVEY.md section 8e; the reference is single-process, so there is no reference interface to
  * cite: the merge restates RunningNorm's Chan update, util/networks.py:96-134, in its additive
