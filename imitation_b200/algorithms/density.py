@@ -6,7 +6,7 @@ agent with its log.  The reference fits sklearn's `KernelDensity` and scores eve
 `StandardScaler` semantics, and sklearn's kernel normalisation constants restated by `log_kernel_norm`) and uploads the
 standardised demonstration rows once; every score is then one launch of `imb_density_score` (csrc/imb_density.cu).  In
 training, the rollout's reward column is overwritten by one such launch from the transition rows the rollout writes
-(`RewardVecEnvWrapper.resolve` -> `DensityRelabel`, `DevicePPO._relabelled_rollout`).
+(`RewardVecEnvWrapper.resolve` -> `reward_wrapper.DensityRelabel`, whose `finish` runs after the rollout).
 
 Two deliberate differences from the reference:
 - The device evaluates the exact estimator.  sklearn's tree evaluation with its defaults (atol = rtol = 0) is not
@@ -296,16 +296,6 @@ class DensityAlgorithm(base.DemonstrationAlgorithm):
         if self._model is None:
             raise RuntimeError("DensityAlgorithm: call train() before scoring")
         return self._model
-
-    def out_of_range_step(self, t0: int, n_steps: int, horizon: int) -> Optional[int]:
-        """The first episode step a rollout of n_steps from episode step t0 reaches that this model has no segment for
-        (None: all covered)."""
-        n = self.device_model.n_seg
-        if self.is_stationary:
-            return None
-        if t0 >= n:
-            return t0
-        return n if min(t0 + n_steps, horizon) > n else None
 
     # -- reward ------------------------------------------------------------------------------------------------------
     def __call__(self, state, action, next_state, done, steps=None) -> np.ndarray:

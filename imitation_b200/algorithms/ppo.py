@@ -81,11 +81,9 @@ class DevicePPO:
         self.record_in_learn = True
         self._tbl = None
         self._aux = None
-        self._ens_raw = None      # ensemble reward: the members' raw rewards [M][T][E]
-        self._ens_ws = None       # ensemble reward: the relabel's workspace (density reward: the score's workspace)
-        self._dens_flat = None    # density reward without a BufferingWrapper: the transition rows it scores
-        # buffers of exploration_rollout (table, flat rows, aux, ensemble raw rewards and workspace): never captured
-        self._x_tbl = self._x_flat = self._x_aux = self._x_raw = self._x_ws = None
+        self._scratch = {}        # the training rollout's reward relabel buffers (reward_wrapper.Relabel)
+        # buffers of exploration_rollout (table, flat rows, aux, relabel buffers): never captured
+        self._x_tbl, self._x_flat, self._x_aux, self._x_scratch = None, None, None, {}
         self.loss_log = None      # optional [n_minibatch_steps][4] device tensor (parity tests)
         self.noise = None         # optional pinned sampling noise for the next rollout (parity tests)
         self.perm = None          # optional host permutations [n_epochs][N] (parity tests)
@@ -146,8 +144,7 @@ class DevicePPO:
                 _lib.rollout_ensemble(env.desc, env.params, env.obs, pol.desc, pp, pn, disc, members, self.hp, E, T,
                                       self._tbl, *ring_args, flat, self._aux, self.noise, env.state, act=pol.act)
 
-        self._ens_raw, self._ens_ws = self._relabelled_rollout(launch, self._tbl, flat, t0, E, T, self._ens_raw,
-                                                               self._ens_ws)
+        self._relabelled_rollout(launch, self._tbl, flat, t0, E, T, self._scratch)
         da = 1 if pol.discrete else pol.d_act
         col_val = pol.d_obs + da + 1
         _lib.gae(self._tbl, rw, col_val, E, T, self._aux, self.hp.gamma, self.hp.gae_lambda, env.state, env.horizon)
@@ -155,71 +152,27 @@ class DevicePPO:
         if not self._capturing:
             self.after_rollout_host(t0)
 
-    def _relabelled_rollout(self, launch, tbl, flat, t0: int, E: int, T: int, ens_raw, ens_ws):
-        """Launch a rollout over the learned reward the RewardVecEnvWrapper describes, then finish its reward column
-        (rewards/reward_wrapper.py:92-133 -> predict_processed): a NormalizedRewardNet's output normalisation, the
-        ensemble's per-member normalisation and mean + alpha * std, advancing the output statistics once per env step,
-        or a DensityAlgorithm's log density of every transition row.
-        launch(disc, disc_params, disc_norm, reward_mode, members, flat) issues the rollout itself (members: the
-        ensemble's member table, else None; flat: its transition rows, None when nobody reads them).  t0: the episode
-        step the rollout starts at.  ens_raw / ens_ws: the ensemble's buffers (ens_ws: the density relabel's workspace
-        for a density reward), reused when their size fits; returns them (a captured graph bakes the training rollout's
-        in, so every rollout keeps its own)."""
-        disc = dparams = dnorm = members = None
-        mode, out_norm, ens, dens = 0, None, None, None
-        if self._rw_wrapper is not None:
-            net, mode, out_norm = self._rw_wrapper.resolve()
-            if isinstance(net, reward_wrapper.EnsembleRelabel):
-                ens = net
-            elif isinstance(net, reward_wrapper.DensityRelabel):
-                dens = net
-            else:
-                eng = net.engine()
-                disc, dparams, dnorm = eng.desc, eng.params, eng.norm_state
-        if ens is not None:
-            ens_raw, ens_ws, members, relabel = self._ensemble_tables(ens, E, T, ens_raw, ens_ws)
-            disc = ens.nets[0].engine().desc
-        env = self._base_env
-        if dens is not None:
-            dens.check_steps(t0, T, env.horizon)
-            if flat is None:  # no BufferingWrapper: the relabel reads rows of its own
-                tw = 2 * env.d_obs + env.d_act + 1
-                if self._dens_flat is None or self._dens_flat.shape[0] != E * T:
-                    self._dens_flat = th.zeros(E * T, tw, device=self.device)
-                flat = self._dens_flat
-            n_ws = _lib.density_ws_floats(E * T)
-            if ens_ws is None or ens_ws.numel() != n_ws:
-                ens_ws = th.zeros(n_ws, device=self.device)  # zero-filled: the score's tickets start at 0
-        launch(disc, dparams, dnorm, mode, members, flat)
-        pol = self.policy
-        rw = tbl.shape[1]
-        col_rew = pol.d_obs + (1 if pol.discrete else pol.d_act) + 2
-        if dens is not None:
-            dens.relabel(flat, tbl, col_rew, E, T, env.horizon, ens_ws, env.state)
-        elif ens is not None:
-            _lib.ensemble_relabel(relabel, ens.alpha, tbl, rw, col_rew, E, T, ens_ws)
-        elif out_norm is not None:
-            ns, nc = out_norm.output_norm_vectors()
-            layer = out_norm.normalize_output_layer
-            _lib.reward_norm_scan(tbl.view(-1)[col_rew:], E, T, rw, T * rw, ns, nc, layer.eps, True,
-                                  ema_decay=layer.decay if out_norm.output_norm_is_ema else None)
-        return ens_raw, ens_ws
+    def _relabel(self) -> reward_wrapper.Relabel:
+        """What fills the rollout's reward column: the RewardVecEnvWrapper's relabel, else the env reward."""
+        return self._rw_wrapper.resolve() if self._rw_wrapper is not None else reward_wrapper.Relabel()
 
-    def _ensemble_tables(self, ens, E: int, T: int, raw, ws):
-        """Member table of the ensemble rollout and member descriptor of its relabel over the buffers raw (the members'
-        raw rewards [M][T][E]) and ws (the relabel's workspace), allocated when missing or too small; -> (raw, ws,
-        members, relabel)."""
-        M = len(ens.nets)
-        n_ws = _lib.ensemble_relabel_ws_floats(M, T)
-        if raw is None or raw.numel() != M * T * E:
-            raw = th.empty(M * T * E, device=self.device)
-        if ws is None or ws.numel() < n_ws:
-            ws = th.zeros(n_ws, device=self.device)  # zero-filled: the relabel's ticket starts at 0
-        engines = [n.engine() for n in ens.nets]
-        members = _lib.rollout_members([e.params for e in engines],
-                                       [e.norm_state if e.has_norm else None for e in engines], raw)
-        norms = [None if o is None else o.output_norm_args() for o in ens.out_norms]
-        return raw, ws, members, _lib.pref_uncertainty_desc(list(raw.view(M, T * E)), norms)
+    def _relabelled_rollout(self, launch, tbl, flat, t0: int, E: int, T: int, scratch: dict) -> None:
+        """Launch a rollout over the reward the RewardVecEnvWrapper describes and finish its reward column
+        (rewards/reward_wrapper.py:92-133 -> predict_processed).  launch(disc, disc_params, disc_norm, reward_mode,
+        members, flat) issues the rollout itself (flat: its transition rows, None when nobody reads them).  t0: the
+        episode step the rollout starts at; scratch: this rollout's relabel buffers."""
+        relabel = self._relabel()
+        env = self._base_env
+        relabel.check_steps(t0, T, env.horizon)
+        if flat is None and relabel.needs_flat:  # no BufferingWrapper: the relabel reads rows of the scratch
+            if scratch.get("flat") is None or scratch["flat"].shape[0] != E * T:
+                scratch["flat"] = th.zeros(E * T, 2 * env.d_obs + env.d_act + 1, device=self.device)
+            flat = scratch["flat"]
+        disc, dparams, dnorm, members = relabel.rollout_args(scratch, E, T)
+        launch(disc, dparams, dnorm, relabel.mode, members, flat)
+        pol = self.policy
+        col_rew = pol.d_obs + (1 if pol.discrete else pol.d_act) + 2
+        relabel.finish(tbl, col_rew, flat, E, T, env.horizon, env.state, scratch)
 
     def exploration_rollout(self, explore_policy, seed: int, step0: int, deterministic: bool = False, noise=None):
         """The rollout of an ExplorationWrapper over this algorithm (AgentTrainer.sample's exploration phase,
@@ -252,8 +205,7 @@ class DevicePPO:
                                  self.hp, E, T, self._x_tbl, flat, self._x_aux, noise, vec, seed, step0,
                                  env.state, flags=flags, act=pol.act)
 
-        self._x_raw, self._x_ws = self._relabelled_rollout(launch, self._x_tbl, self._x_flat, 0, E, T, self._x_raw,
-                                                           self._x_ws)
+        self._relabelled_rollout(launch, self._x_tbl, self._x_flat, 0, E, T, self._x_scratch)
         _lib.rollout_advance(env.state, E, T, H, 0)
         env.host_ep_step = 0
         return self._x_flat, self._x_aux[2 * E + E * T:].view(E, T)
@@ -300,38 +252,17 @@ class DevicePPO:
         for k, v in self.read_train_stats().items():
             lg.record(k, v, exclude="tensorboard" if k == "train/n_updates" else None)
 
-    def _pointer_key(self):
+    def _pointer_key(self, relabel: reward_wrapper.Relabel):
         """Everything a captured graph bakes in: device pointers of the vectors the kernels touch."""
         pp, pn, pc = self.policy.flat_vectors()
-        key = [pp.data_ptr(), pn.data_ptr(), pc.data_ptr(), self._tbl.data_ptr() if self._tbl is not None else 0,
+        key = (pp.data_ptr(), pn.data_ptr(), pc.data_ptr(), self._tbl.data_ptr() if self._tbl is not None else 0,
                self.n_steps, id(self._rw_wrapper), id(self._buffering),
+               *[t.data_ptr() for t in self._scratch.values()],
                # launch arguments of the PPO update
-               self.target_kl, self.clip_range_vf, self.train_stats.data_ptr()]
-        if self._rw_wrapper is not None:
-            net, mode, out_norm = self._rw_wrapper.resolve()
-            if isinstance(net, reward_wrapper.EnsembleRelabel):
-                # alpha is a launch argument of the relabel: a new default_alpha needs a new graph
-                key += [net.alpha, self._ens_raw.data_ptr() if self._ens_raw is not None else 0,
-                        self._ens_ws.data_ptr() if self._ens_ws is not None else 0]
-                for n, o in zip(net.nets, net.out_norms):
-                    eng = n.engine()
-                    key += [eng.params.data_ptr(), eng.norm_state.data_ptr(), id(o)]
-                    if o is not None:
-                        key += [t.data_ptr() for t in o.output_norm_vectors()]
-                        key += [o.output_norm_is_ema, getattr(o.normalize_output_layer, "decay", None)]
-            elif isinstance(net, reward_wrapper.DensityRelabel):
-                key += list(net.pointer_key())
-                key += [t.data_ptr() if t is not None else 0 for t in (self._ens_ws, self._dens_flat)]
-            else:
-                eng = net.engine()
-                key += [eng.params.data_ptr(), eng.norm_state.data_ptr(), mode, id(out_norm)]
-                if out_norm is not None:
-                    # the output norm's vectors and an EMANorm's decay are launch arguments of the scan
-                    key += [t.data_ptr() for t in out_norm.output_norm_vectors()]
-                    key += [out_norm.output_norm_is_ema, getattr(out_norm.normalize_output_layer, "decay", None)]
+               self.target_kl, self.clip_range_vf, self.train_stats.data_ptr())
         if self._buffering is not None and self._buffering._ring is not None:
-            key.append(self._buffering._ring.table.data_ptr())
-        return tuple(key)
+            key += (self._buffering._ring.table.data_ptr(),)
+        return key + relabel.graph_key()
 
     def _iteration(self) -> None:
         """One collect_rollouts + train, replayed from a CUDA graph once it is warm (the kernels read every
@@ -346,7 +277,8 @@ class DevicePPO:
             self.train()
             self._eager_iters += 1
             return
-        key = self._pointer_key()
+        relabel = self._relabel()
+        key = self._pointer_key(relabel)
         if self._graph is None or key != self._graph_key:
             before = _lib.LAUNCHES["count"]
             self._capturing = True
@@ -364,10 +296,7 @@ class DevicePPO:
             self._graph_launches = _lib.LAUNCHES["count"] - before
             _lib.LAUNCHES["count"] = before
         t0 = self._base_env.host_ep_step
-        if self._rw_wrapper is not None:
-            net = self._rw_wrapper.resolve()[0]
-            if isinstance(net, reward_wrapper.DensityRelabel):
-                net.check_steps(t0, self.n_steps, self._base_env.horizon)  # the replayed launches take no host check
+        relabel.check_steps(t0, self.n_steps, self._base_env.horizon)  # the replayed launches take no host check
         self._graph[0].replay()
         self.ev_rollout.record()
         self._graph[1].replay()

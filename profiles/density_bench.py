@@ -92,12 +92,12 @@ def bench(name, steps, warmup):
             if i >= warmup:
                 roll[k].append(ms)
     algo, dens, D = s["density"]
-    relabel = algo._rw_wrapper.resolve()[0]
+    relabel = algo._rw_wrapper.resolve()
     col_rew = Do + Da + 2
     flat = algo._buffering._flat
 
     def launch():
-        relabel.relabel(flat, algo._tbl, col_rew, E, T, algo._base_env.horizon, algo._ens_ws, algo._base_env.state)
+        relabel.finish(algo._tbl, col_rew, flat, E, T, algo._base_env.horizon, algo._base_env.state, algo._scratch)
 
     for _ in range(warmup):
         launch()

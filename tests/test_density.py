@@ -598,9 +598,9 @@ def test_rollout_without_buffering_wrapper_scores_rows_of_its_own():
     algo.set_env(reward_wrapper.RewardVecEnvWrapper(venv, dens))
     algo.collect_rollouts()
     th.cuda.synchronize()
-    assert algo._dens_flat is not None and algo._buffering is None
+    assert algo._scratch.get("flat") is not None and algo._buffering is None
     rw = algo._tbl.shape[1]
-    flat = algo._dens_flat.cpu().numpy()
+    flat = algo._scratch["flat"].cpu().numpy()
     tbl = algo._tbl.cpu().numpy().reshape(E, T, rw)
     boot = algo._aux[2 * E:2 * E + E * T].cpu().numpy().reshape(E, T)
     # from t0 = 0 with T > H: rows of the first episode are env-major [e][0, H), then the partial one [e][H, T)

@@ -303,7 +303,7 @@ def test_agent_trainer_on_ema_ensemble_matches_restatement(L):
         agent.train(steps=E * T)
         agent.buffering_wrapper.discard()
         th.cuda.synchronize()
-        raw = algo._ens_raw.view(M, T, E).cpu().numpy()
+        raw = algo._scratch["ensemble_raw"].view(M, T, E).cpu().numpy()
         vals, finals = zip(*[_ema_f64(raw[m], *before[m], decay, 1e-5) for m in range(M)])
         v = np.stack(vals)
         want = v.mean(0) + alpha * np.sqrt(v.var(0, ddof=1))
@@ -491,7 +491,7 @@ def test_mixed_kind_ensemble_and_input_ema_raise(L):
         reward_wrapper.RewardVecEnvWrapper(venv, ens.predict_processed).resolve()
     same = [reward_nets.NormalizedRewardNet(basic(), networks.EMANorm) for _ in range(2)]
     ens = reward_nets.RewardEnsemble(obs_sp, act_sp, same).cuda()
-    rel, _, _ = reward_wrapper.RewardVecEnvWrapper(venv, ens.predict_processed).resolve()
+    rel = reward_wrapper.RewardVecEnvWrapper(venv, ens.predict_processed).resolve()
     assert all(o.output_norm_is_ema for o in rel.out_norms)
     with pytest.raises(NotImplementedError, match="normalize_input_layer must be RunningNorm or None"):
         reward_nets.BasicShapedRewardNet(obs_sp, act_sp, normalize_input_layer=networks.EMANorm)

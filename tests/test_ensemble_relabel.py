@@ -282,7 +282,7 @@ def test_graph_replay_equals_eager_and_alpha_takes_effect(L):
     agent.train(steps=E * T)
     agent.buffering_wrapper.discard()
     th.cuda.synchronize()
-    raw = algo._ens_raw.view(5, T, E).cpu().numpy()
+    raw = algo._scratch["ensemble_raw"].view(5, T, E).cpu().numpy()
     want, final = _relabel_f64(raw, [(b[0], b[1], b[2], 1e-5) for b in before], 1.5)
     rw = algo._tbl.shape[1]
     col_rew = 11 + 3 + 2
@@ -347,14 +347,14 @@ def test_unsupported_ensembles_raise(L):
         resolve(reward_nets.NormalizedRewardNet(ens, networks.RunningNorm))
     # accepted: both members' engines, alpha read from the wrapper
     ens = reward_nets.AddSTDRewardWrapper(reward_nets.RewardEnsemble(obs_sp, act_sp, [basic(), basic()]).cuda(), -0.5)
-    rel, mode, out_norm = resolve(ens)
-    assert isinstance(rel, reward_wrapper.EnsembleRelabel) and mode == 2 and out_norm is None
+    rel = resolve(ens)
+    assert isinstance(rel, reward_wrapper.EnsembleRelabel) and rel.mode == 2
     assert rel.alpha == -0.5 and rel.out_norms == [None, None] and len(rel.nets) == 2
     # one wrapper resolves its ensemble once; a new default_alpha is still read at every access
     w = reward_wrapper.RewardVecEnvWrapper(venv, ens.predict_processed)
-    first = w.resolve()[0]
+    first = w.resolve()
     ens.default_alpha = 0.25
-    assert w.resolve()[0] is first and first.alpha == 0.25
+    assert w.resolve() is first and first.alpha == 0.25
 
 
 def test_member_images_that_do_not_fit_fail_with_the_limit(L):
