@@ -149,6 +149,9 @@ SIGNATURES = {
                                  _ptr, _ptr, _ptr], 1),
     "imb_ppo_plan": (_i32, [_pol, _i32, _i32], 0),
     "imb_ppo_update_variant": (_i32, [_pol], 0),
+    "imb_bc_train": (_i32, [_pol, _i32, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _i64, _i32, _i32, _i64, _i64, _i32, _f32, _f32,
+                            _f32, _f32, _i32, _ptr, _ptr, _ptr, _i32, _ptr, _ptr], 1),
+    "imb_bc_plan": (_i32, [_pol, _i32, _i32], 0),
     "imb_policy_logp": (_i32, [_pol, _i32, _ptr, _ptr, _ptr, _i64, _i64, _i32, _ptr], 1),
     "imb_disc_reduce_adam": (_i32, [_disc, _adam, _ptr, _ptr, _ptr, _f32, _ptr, _ptr, _ptr, _ptr], 1),
     "imb_pref_loss": (_i32, [_ptr, _i64, _i32, _ptr, _f32, _f32, _f32, _f32, _ptr, _ptr, _ptr, _i32, _ptr], 1),
@@ -558,3 +561,30 @@ def ppo_update_variant(pol: PolicyDesc) -> int:
 def policy_logp(pol, params, norm, batch, ld, n, row_logp, act=ACT_TANH):
     _check(lib().imb_policy_logp(pol, act, _p(params, th.float32), _p(norm), _p(batch, th.float32), ld, n, row_logp,
                                  _stream()), "imb_policy_logp")
+
+
+# imb_bc_train: columns of a metrics row
+BC_METRICS = ("neglogp", "entropy", "ent_loss", "prob_true_act", "l2_norm", "l2_loss", "loss")
+BC_METRIC_FLOATS = 8  # the seven BCTrainingMetrics and the batch number
+
+
+def bc_train(pol, params, norm, norm_count, exp_avg, exp_avg_sq, table, n_rows, minibatch_size, batch_size, j0,
+             n_minibatches, final_flush, l2_weight, ent_weight, lr, adam_eps, norm_update, perm, grad_carry, metrics,
+             log_interval, state, act=ACT_TANH):
+    """Minibatches [j0, j0 + n_minibatches) of one BC train() call in one launch (imb_bc_train): `table` the
+    demonstrations in rollout-row format, `perm` int64 [epochs][n_rows] from epoch j0 // (n_rows // minibatch_size) on,
+    `metrics` float32 [n_logged][BC_METRIC_FLOATS] or None."""
+    _check(lib().imb_bc_train(pol, act, _p(params, th.float32), _p(norm), _p(norm_count), _p(exp_avg, th.float32),
+                              _p(exp_avg_sq, th.float32), _p(table, th.float32), n_rows, minibatch_size, batch_size, j0,
+                              n_minibatches, int(final_flush), l2_weight, ent_weight, lr, adam_eps, int(norm_update),
+                              _p(perm, th.int64), _p(grad_carry, th.float32), _p(metrics, th.float32), log_interval,
+                              _p(state, th.int64), _stream()), "imb_bc_train", 1 if n_minibatches > 0 or final_flush == 1 else 0)
+
+
+def bc_plan(pol: PolicyDesc, minibatch_size: int, act: int = ACT_TANH) -> int:
+    """PPO_PLAN_GEN1 / PPO_PLAN_GEN2: the kernel `bc_train` runs for `pol` at minibatch_size (host only, no GPU needed);
+    ImbError naming the shared-memory need and limit when the shape does not fit."""
+    rc = lib().imb_bc_plan(pol, act, minibatch_size)
+    if rc < 0:
+        raise ImbError(f"imb_bc_plan: {lib().imb_last_error().decode()} (rc={rc})")
+    return rc

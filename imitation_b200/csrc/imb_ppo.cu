@@ -1338,11 +1338,11 @@ static size_t ppo_smem_floats(const PpoArgs& A) {
   return o;
 }
 
-// cluster launch of one of the two PPO kernels (CL CTAs of PT threads, one cluster)
-template <typename K>
+// cluster launch of one of the two PPO kernels (CL CTAs of PT threads, one cluster); `extra`: k_ppo_update_gen's BcArgs
+template <typename K, typename... Extra>
 static int launch_cluster(K kernel, const char* name, size_t smem_bytes, size_t* attr_bytes, cudaStream_t st, const PpoArgs& A,
                           float* params, float* norm, int32_t* norm_count, float* m, float* v, const float* rollout,
-                          const int64_t* perm, float* loss_log, int64_t* state) {
+                          const int64_t* perm, float* loss_log, int64_t* state, Extra... extra) {
   IMB_REQUIRE(smem_bytes <= IMB_SMEM_MAX, "%s needs %zu B of shared memory per CTA (policy / minibatch too large)", name,
               smem_bytes);
   if (smem_bytes > *attr_bytes) {
@@ -1362,12 +1362,41 @@ static int launch_cluster(K kernel, const char* name, size_t smem_bytes, size_t*
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, A, params, norm, norm_count, m, v, rollout, perm, loss_log, state);
+  cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, A, params, norm, norm_count, m, v, rollout, perm, loss_log, state,
+                                     extra...);
   if (e != cudaSuccess) IMB_FAIL(-2, "%s (cluster launch): %s", name, cudaGetErrorString(e));
   return 0;
 }
 
 extern "C" int imb_rollout_row_width(const imb_policy_desc* pol);
+
+// The shape checks and launch geometry (rw, KP, S, RS2) every PPO kernel shares; `what` names the caller's update.
+static int ppo_plan_shape(PpoArgs& A, int act, const char* what) {
+  const imb_policy_desc& pd = A.pol;
+  IMB_REQUIRE(act == IMB_ACT_TANH || act == IMB_ACT_RELU,
+              "pol_act must be IMB_ACT_TANH (0) or IMB_ACT_RELU (1), got %d", act);
+  IMB_REQUIRE(pd.hidden >= 1 && pd.hidden <= 64, "policy tower width must be <= 64");
+  IMB_REQUIRE(pd.d_obs >= 1 && pd.d_obs <= IMB_MAX_DIN && pd.d_act >= 1 && pd.d_act <= IMB_MAX_DIN,
+              "d_obs/d_act must be in [1, %d]", IMB_MAX_DIN);
+  IMB_REQUIRE(A.hp.batch_size >= 1 && A.hp.batch_size <= GEN_MAX_MB, "%s minibatch size must be in [1, %d]", what,
+              GEN_MAX_MB);
+  A.rw = imb_rollout_row_width(&pd);
+  IMB_REQUIRE(A.rw % 4 == 0, "rollout row width must be a multiple of 4 floats (bulk row copies)");
+  A.KP = ppo_kp(pd.d_obs);
+  A.S = ppo_slice(make_play(pd));
+  A.RS2 = ppo_row_stride(A.rw);
+  return 0;
+}
+
+// k_ppo_update_gen's plan: U = 1 or 2 hidden units per lane (IMB_PPO_PLAN_GEN1 / GEN2), HP into A, its dynamic shared
+// memory into *bytes; < 0 naming the need and the limit when it does not fit.
+static int gen_plan(PpoArgs& A, size_t* bytes, const char* what) {
+  A.HP = A.pol.hidden <= 32 ? 32 : 64;
+  *bytes = (size_t)gen_layout(A.S, A.HP, A.KP, A.pol.d_act, A.hp.batch_size).total * 4;
+  IMB_REQUIRE(*bytes <= IMB_SMEM_MAX, "policy / minibatch too large for the %s update: k_ppo_update_gen<%d> needs %zu B "
+              "of shared memory per CTA, the limit is %d B", what, A.HP / 32, *bytes, (int)IMB_SMEM_MAX);
+  return A.HP == 32 ? IMB_PPO_PLAN_GEN1 : IMB_PPO_PLAN_GEN2;
+}
 
 // Which PPO kernel runs the policy A.pol at minibatch A.hp.batch_size (the IMB_PPO_PLAN_* codes of imb_ppo_plan), with
 // the launch geometry (rw, KP, S, RS2, HP) filled into A and the dynamic shared memory into *bytes.  k_ppo_update
@@ -1376,17 +1405,8 @@ extern "C" int imb_rollout_row_width(const imb_policy_desc* pol);
 // (act = IMB_ACT_RELU) always run k_ppo_update_gen: k_ppo_update is built for the tanh policies bench.py trains.
 static int ppo_plan(PpoArgs& A, int act, size_t* bytes) {
   const imb_policy_desc& pd = A.pol;
-  IMB_REQUIRE(act == IMB_ACT_TANH || act == IMB_ACT_RELU,
-              "pol_act must be IMB_ACT_TANH (0) or IMB_ACT_RELU (1), got %d", act);
-  IMB_REQUIRE(pd.hidden >= 1 && pd.hidden <= 64, "policy tower width must be <= 64");
-  IMB_REQUIRE(pd.d_obs >= 1 && pd.d_obs <= IMB_MAX_DIN && pd.d_act >= 1 && pd.d_act <= IMB_MAX_DIN,
-              "d_obs/d_act must be in [1, %d]", IMB_MAX_DIN);
-  IMB_REQUIRE(A.hp.batch_size >= 1 && A.hp.batch_size <= GEN_MAX_MB, "PPO minibatch size must be in [1, %d]", GEN_MAX_MB);
-  A.rw = imb_rollout_row_width(&pd);
-  IMB_REQUIRE(A.rw % 4 == 0, "rollout row width must be a multiple of 4 floats (bulk row copies)");
-  A.KP = ppo_kp(pd.d_obs);
-  A.S = ppo_slice(make_play(pd));
-  A.RS2 = ppo_row_stride(A.rw);
+  const int rc = ppo_plan_shape(A, act, "PPO");
+  if (rc != 0) return rc;
   // IMB_PPO_FORCE_GENERAL=1 (tests): run the general kernel on shapes the specialised one covers
   const char* force = getenv("IMB_PPO_FORCE_GENERAL");
   if (act == IMB_ACT_TANH && pd.hidden <= 32 && A.hp.batch_size <= PR && !(force && force[0] == '1')) {
@@ -1394,11 +1414,13 @@ static int ppo_plan(PpoArgs& A, int act, size_t* bytes) {
     *bytes = ppo_smem_floats(A) * 4;
     if (A.S / 4 <= PT && *bytes <= IMB_SMEM_MAX) return IMB_PPO_PLAN_UPDATE;
   }
-  A.HP = pd.hidden <= 32 ? 32 : 64;
-  *bytes = (size_t)gen_layout(A.S, A.HP, A.KP, pd.d_act, A.hp.batch_size).total * 4;
-  IMB_REQUIRE(*bytes <= IMB_SMEM_MAX, "policy / minibatch too large for the PPO update: k_ppo_update_gen<%d> needs %zu B "
-              "of shared memory per CTA, the limit is %d B", A.HP / 32, *bytes, (int)IMB_SMEM_MAX);
-  return A.HP == 32 ? IMB_PPO_PLAN_GEN1 : IMB_PPO_PLAN_GEN2;
+  return gen_plan(A, bytes, "PPO");
+}
+
+// The BC update runs k_ppo_update_gen<U, act, LOSS_BC> for every shape (the specialised k_ppo_update has no BC loss).
+static int bc_plan(PpoArgs& A, int act, size_t* bytes) {
+  const int rc = ppo_plan_shape(A, act, "BC");
+  return rc != 0 ? rc : gen_plan(A, bytes, "BC");
 }
 
 extern "C" int imb_ppo_plan(const imb_policy_desc* pol, int32_t pol_act, int32_t batch_size) {
@@ -1473,7 +1495,7 @@ static int launch_ppo(const PpoArgs& A0, int act, float* params, float* norm, in
                                          {"k_ppo_update_gen<2>", "k_ppo_update_gen<2, relu>"}};
     const int u = plan == IMB_PPO_PLAN_GEN1 ? 0 : 1;
     return launch_cluster(kernels[u][act], names[u][act], bytes, &attr_bytes[u][act], st, A, params, norm, norm_count, m,
-                          v, rollout, perm, loss_log, state);
+                          v, rollout, perm, loss_log, state, BcArgs{});
   }
   return plan;
 }
@@ -1502,6 +1524,66 @@ extern "C" int imb_ppo_update(const imb_policy_desc* pol, int32_t pol_act, float
                               float* loss_log, int64_t* state, void* stream) {
   return imb_ppo_update_ex(pol, pol_act, pol_params, pol_norm, pol_norm_count, exp_avg, exp_avg_sq, rollout, n_rows, hp,
                            0.f, 0.f, perm, seed, loss_log, nullptr, state, stream);
+}
+
+extern "C" int imb_bc_plan(const imb_policy_desc* pol, int32_t pol_act, int32_t minibatch_size) {
+  PpoArgs A = {};
+  A.pol = *pol;
+  A.hp.batch_size = minibatch_size;
+  size_t bytes;
+  return bc_plan(A, pol_act, &bytes);
+}
+
+extern "C" int imb_bc_train(const imb_policy_desc* pol, int32_t pol_act, float* pol_params, float* pol_norm,
+                            int32_t* pol_norm_count, float* exp_avg, float* exp_avg_sq, const float* table,
+                            int64_t n_rows, int32_t minibatch_size, int32_t batch_size, int64_t j0,
+                            int64_t n_minibatches, int32_t final_flush, float l2_weight, float ent_weight, float lr,
+                            float adam_eps, int32_t norm_update, const int64_t* perm, float* grad_carry, float* metrics,
+                            int32_t log_interval, int64_t* state, void* stream) {
+  IMB_REQUIRE(n_rows >= 1 && n_rows < (1ll << 31), "bad n_rows");
+  IMB_REQUIRE(minibatch_size >= 1 && n_rows >= minibatch_size, "BC needs at least minibatch_size (%d) demonstration "
+              "rows, got %lld", minibatch_size, (long long)n_rows);
+  IMB_REQUIRE(batch_size >= minibatch_size && batch_size % minibatch_size == 0,
+              "batch_size (%d) must be a multiple of minibatch_size (%d)", batch_size, minibatch_size);
+  IMB_REQUIRE(j0 >= 0 && n_minibatches >= 0, "bad minibatch range");
+  IMB_REQUIRE(final_flush >= 0 && final_flush <= 2, "final_flush must be 0, 1 or 2");
+  IMB_REQUIRE(n_minibatches > 0 || final_flush != 1 || j0 % (batch_size / minibatch_size) != 0,
+              "a flush-only launch (n_minibatches = 0) needs an incomplete batch to step");
+  IMB_REQUIRE(perm != nullptr || n_minibatches == 0, "perm is required");
+  IMB_REQUIRE(log_interval >= 1 || metrics == nullptr, "log_interval must be >= 1");
+  const int k = batch_size / minibatch_size;
+  IMB_REQUIRE(grad_carry != nullptr || (k == 1), "grad_carry is required when batch_size > minibatch_size");
+  if (n_minibatches == 0 && final_flush != 1) return 0;
+  PpoArgs A = {};
+  A.pol = *pol;
+  A.hp.batch_size = minibatch_size;
+  A.hp.ent_coef = ent_weight;
+  A.hp.lr = lr;
+  A.hp.adam_eps = adam_eps;
+  A.n_rows = n_rows;
+  size_t bytes;
+  const int plan = bc_plan(A, pol_act, &bytes);
+  if (plan < 0) return plan;
+  BcArgs B = {};
+  B.j0 = j0;
+  B.n_mb = n_minibatches;
+  B.k = k;
+  B.final_flush = final_flush;
+  B.norm_update = norm_update != 0;
+  B.log_interval = log_interval >= 1 ? log_interval : 1;
+  B.l2_weight = l2_weight;
+  B.inv_bs = 1.0f / (float)batch_size;
+  B.carry = grad_carry;
+  B.metrics = metrics;
+  static size_t attr_bytes[2][2] = {};
+  constexpr decltype(&k_ppo_update_gen<1, ACT_TANH, LOSS_BC>) kernels[2][2] = {
+      {k_ppo_update_gen<1, ACT_TANH, LOSS_BC>, k_ppo_update_gen<1, ACT_RELU, LOSS_BC>},
+      {k_ppo_update_gen<2, ACT_TANH, LOSS_BC>, k_ppo_update_gen<2, ACT_RELU, LOSS_BC>}};
+  constexpr const char* names[2][2] = {{"k_ppo_update_gen<1, bc>", "k_ppo_update_gen<1, relu, bc>"},
+                                       {"k_ppo_update_gen<2, bc>", "k_ppo_update_gen<2, relu, bc>"}};
+  const int u = plan == IMB_PPO_PLAN_GEN1 ? 0 : 1;
+  return launch_cluster(kernels[u][pol_act], names[u][pol_act], bytes, &attr_bytes[u][pol_act], (cudaStream_t)stream, A,
+                        pol_params, pol_norm, pol_norm_count, exp_avg, exp_avg_sq, table, perm, nullptr, state, B);
 }
 
 template <int HP, int ACT>

@@ -16,6 +16,32 @@
 // Three cluster barriers per optimiser step instead of the mbarrier-signalled exchange of k_ppo_update: simpler, and
 // the barriers' cost is small against steps that carry 2-32x the arithmetic.
 // ACT is the towers' activation: every ReLU policy runs here whatever its shape (k_ppo_update is tanh only).
+// LK is the loss of the step: LOSS_PPO (PPO.train) or LOSS_BC (behavioural cloning, algorithms/bc.py:94-156 and
+// :481-510).  A BC step is this kernel's step with
+//   * the minibatch drawn from the host's per-epoch permutations in full minibatches (DataLoader drop_last=True), the
+//     launch running minibatches [j0, j0 + n) of one train() call (BcArgs);
+//   * only the obs | act columns of the rows read, d loss / d logp = -1 / batch_size per row, the entropy term with
+//     ent_weight / batch_size, no ratio, clipping or advantage, and no value tower (no forward, backward or value loss);
+//   * the feature RunningNorm updated per minibatch only when the policy is in training mode (norm_update);
+//   * the reduced gradient accumulated over batch_size / minibatch_size minibatches (the gradient of an unfinished
+//     batch is carried between launches in BcArgs::carry); the optimiser step adds l2_weight * w to every gradient, then
+//     runs Adam without clip_grad_norm_ (no squared-norm exchange); the last, incomplete batch of a train() also steps;
+//   * the BCTrainingMetrics of every logged batch's last minibatch written to BcArgs::metrics.
+constexpr int LOSS_PPO = 0, LOSS_BC = 1;
+struct BcArgs {
+  int64_t j0, n_mb;    // minibatches [j0, j0 + n_mb) of the train() call's sequence (numbered from 0 in every train())
+  int k;               // minibatches per optimiser batch: batch_size / minibatch_size
+  int final_flush;     // minibatch j0 + n_mb - 1 ends the train(): 1 = an incomplete batch there takes its optimiser
+                       // step; 2 = that step is left to a later flush-only launch (n_mb = 0, final_flush = 1), this
+                       // launch only writes the batch's metrics (the reference steps after the last on_epoch_end)
+  int norm_update;     // policy.training: the feature RunningNorm is updated by every minibatch
+  int log_interval;    // batches whose number is a multiple of it write their metrics
+  float l2_weight;
+  float inv_bs;        // 1 / batch_size
+  float* carry;        // [n_params] (flat order) summed gradient of the batch the launch starts / ends inside
+  float* metrics;      // [n_logged][8]: BC_M_* of each logged batch, in order
+};
+enum { BC_M_NEGLOGP, BC_M_ENTROPY, BC_M_ENT_LOSS, BC_M_PROB_TRUE_ACT, BC_M_L2_NORM, BC_M_L2_LOSS, BC_M_LOSS, BC_M_BATCH };
 constexpr int RG = 16;             // minibatch rows per CTA and pass
 constexpr int GEN_MAX_MB = 4096;   // index list of one minibatch in shared memory
 
@@ -93,13 +119,18 @@ __device__ __forceinline__ float ppo_act_grad(float g, float a) {
   return ACT == ACT_TANH ? g * (1.0f - a * a) : (a > 0.f ? g : 0.f);
 }
 
-template <int U, int PACT>  // PACT: the towers' activation (ACT names the shared-memory action tile below)
+// PACT: the towers' activation (ACT names the shared-memory action tile below); LK: the loss, LOSS_PPO or LOSS_BC.  Under LOSS_BC
+// `rollout` is the demonstration table, perm_in holds the permutations of the epochs from (j0 / (N / mb)) on, [epoch][N],
+// A.hp.ent_coef is ent_weight, and loss_log is unused.
+template <int U, int PACT, int LK = LOSS_PPO>
 __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float* __restrict__ g_params,
                                                           float* __restrict__ g_norm, int32_t* __restrict__ g_norm_count,
                                                           float* __restrict__ g_m, float* __restrict__ g_v,
                                                           const float* __restrict__ rollout,
                                                           const int64_t* __restrict__ perm_in,
-                                                          float* __restrict__ loss_log, int64_t* __restrict__ state) {
+                                                          float* __restrict__ loss_log, int64_t* __restrict__ state,
+                                                          const BcArgs B) {
+  constexpr bool BC = LK == LOSS_BC;
   constexpr int HP = 32 * U;
   namespace cg = cooperative_groups;
   cg::cluster_group cluster = cg::this_cluster();
@@ -165,14 +196,16 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
     if (q / S == crank) {
       Ms[q - crank * S] = g_m[p];
       Vs[q - crank * S] = g_v[p];
+      if (BC && B.j0 % B.k != 0) Gs[q - crank * S] = B.carry[p];  // the batch began in the previous launch
     }
   }
   int32_t run_count = pd.has_norm ? *g_norm_count : 0;
 
   const int64_t N = A.n_rows;
   const int Ni = (int)N;
-  const int64_t steps_per_epoch = (N + mb - 1) / mb;
-  const int64_t n_steps = steps_per_epoch * A.hp.n_epochs;
+  const int64_t steps_per_epoch = BC ? N / mb : (N + mb - 1) / mb;
+  const bool flush_only = BC && B.n_mb == 0;  // BC: only the optimiser step of the carried incomplete batch
+  const int64_t n_steps = BC ? (flush_only ? 1 : B.n_mb) : steps_per_epoch * A.hp.n_epochs;
   int64_t adam_step = state[IMB_ST_PPO_STEP];
   const int64_t perm_draw0 = state[IMB_ST_PPO_EPOCH];
   double b1pow = pow(0.9, (double)adam_step), b2pow = pow(0.999, (double)adam_step);
@@ -181,12 +214,29 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
 
   int ep_now = 0, start = 0;
   int64_t kstop = 0;  // target_kl: the stopping step + 1
+  int n_logged = 0;   // BC: metrics rows written
+  if (BC) start = (int)(B.j0 % steps_per_epoch) * mb;
   for (int64_t gs = 0; gs < n_steps; ++gs) {
     const int nb = min(mb, Ni - start);
     const float inv_nb = 1.0f / (float)nb;
-    ++adam_step;
+    // BC: minibatch i of the train() call ends a batch when (i + 1) * mb is a multiple of batch_size (bc.py:505) or,
+    // incomplete, when it is the call's last (bc.py:507-510); that batch is number i / k, or i / k + 1 when incomplete
+    bool bc_step = true, bc_log = false;
+    float l2c = 0.f;  // BC: l2_weight x (the batch's minibatches so far) x mb / batch_size
+    int64_t batch_num = 0;
+    if (BC) {
+      const int64_t i = B.j0 + gs - (flush_only ? 1 : 0);
+      const bool full = (i + 1) % B.k == 0, last = B.final_flush != 0 && gs == n_steps - 1;
+      bc_step = full || (last && B.final_flush == 1);
+      batch_num = i / B.k + (full ? 0 : 1);
+      bc_log = (bc_step || last) && !flush_only && B.metrics != nullptr && batch_num % B.log_interval == 0;
+      l2c = B.l2_weight * ((float)(i % B.k + 1) / (float)B.k);
+      if (bc_step) ++adam_step;
+    } else {
+      ++adam_step;
+    }
     // ---- 0. the step's rollout rows, a clean gradient vector, Adam bias corrections ------------------------------
-    for (int r = tid; r < nb; r += PT) {
+    for (int r = tid; r < (flush_only ? 0 : nb); r += PT) {
       int64_t idx;
       if (perm_in) {
         idx = perm_in[(int64_t)ep_now * N + start + r];
@@ -199,8 +249,13 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
     for (int i = tid; i < CL * S; i += PT) GP[i] = 0.f;
     if (rec && tid < RS_N * RG) RSL[tid] = 0.f;
     if (tid == PT - 1) {
-      b1pow *= 0.9;
-      b2pow *= 0.999;
+      if (BC) {  // from the step count alone, so that a train() split over launches computes the same bits
+        b1pow = pow(0.9, (double)adam_step);
+        b2pow = pow(0.999, (double)adam_step);
+      } else {
+        b1pow *= 0.9;
+        b2pow *= 0.999;
+      }
       bc[0] = (float)((double)A.hp.lr / (1.0 - b1pow));
       bc[1] = (float)sqrt(1.0 - b2pow);
     }
@@ -209,9 +264,12 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
     //         forward pass applies with the UPDATED statistics; last column: advantage normalisation) -----------------
     for (int c = warp; c <= Do; c += PT / 32) {
       const bool is_feat = c < Do;
-      const bool need = is_feat ? (pd.has_norm != 0) : (A.hp.normalize_advantage && nb > 1);
+      const bool need = is_feat ? (pd.has_norm != 0 && !flush_only) : (!BC && A.hp.normalize_advantage && nb > 1);
       float mean = 0.f, istd = 1.f;
-      if (need) {  // (warp-uniform)
+      if (BC && need && !B.norm_update) {  // evaluation mode: normalise with the statistics as they stand
+        mean = rstat[c];
+        istd = rsqrtf(rstat[64 + c] + pd.norm_eps);
+      } else if (need) {  // (warp-uniform)
         const int col = is_feat ? c : col_adv;
         float s = 0.f;
         for (int r = lane; r < nb; r += 32) s += rollout[(int64_t)IDX[r] * rw + col];
@@ -248,16 +306,17 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
         CSI[c] = istd;
       }
     }
-    if (pd.has_norm) run_count += nb;
+    if (pd.has_norm && (!BC || (B.norm_update && !flush_only))) run_count += nb;
     __syncthreads();
 
     // ---- 2. passes of CL x RG rows: stage own rows -> warp-autonomous forward / loss / backward -> weight gradients ----
     float l_pg = 0.f, l_v = 0.f, l_ent = 0.f;
-    const int npass = (nb + CL * RG - 1) / (CL * RG);
+    const int npass = flush_only ? 0 : (nb + CL * RG - 1) / (CL * RG);
     for (int pass = 0; pass < npass; ++pass) {
       const int base = pass * (CL * RG) + crank * RG;  // first minibatch row of this CTA in this pass
-      for (int e = tid; e < RG * rw; e += PT) {
-        const int i = e / rw, c = e - i * rw, r = base + i;
+      const int rws = BC ? col_logp : rw;  // BC reads the obs | act columns only
+      for (int e = tid; e < RG * rws; e += PT) {
+        const int i = e / rws, c = e - i * rws, r = base + i;
         const bool rl = r < nb;
         const float v = rl ? rollout[(int64_t)IDX[rl ? r : 0] * rw + c] : 0.f;
         if (c < Do) {
@@ -273,7 +332,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
         }
       }
       __syncthreads();
-      {
+      if (!BC || warp < 4) {  // (BC has no value tower)
         // warp = (tower, 4 own rows), lane = hidden unit(s) lane + 32 u; only __syncwarp() between the layers
         const int cnet = warp >> 2, r0 = 4 * (warp & 3);
         const int rr = lane >> 3, la = lane & 7;  // per-row parts: lane octet rr handles row r0 + rr
@@ -447,12 +506,24 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
           }
           logp = oct_sum(logp);
           ent = oct_sum(ent);
+          float dl_dlogp, dent;
+          if constexpr (BC) {
+            // loss x mb / batch_size (bc.py:501): d / d logp = -1 / batch_size, d / d entropy = -ent_weight / batch_size;
+            // l_pg, l_v, l_ent collect sum logp, sum exp(logp), sum entropy for the metrics
+            dl_dlogp = live ? -B.inv_bs : 0.f;
+            dent = live ? -A.hp.ent_coef * B.inv_bs : 0.f;
+            if (live && la == 0) {
+              l_pg += logp;
+              l_v += expf(logp);
+              l_ent += ent;
+            }
+          } else {
           const float ratio = __expf(logp - logp_old);
           const float lo = 1.0f - A.hp.clip_range, hi = 1.0f + A.hp.clip_range;
           const float pl1 = adv * ratio, pl2 = adv * fminf(fmaxf(ratio, lo), hi);
           const bool inside = (ratio >= lo) && (ratio <= hi);
-          float dl_dlogp = (inside || pl1 < pl2) ? -adv * ratio * inv_nb : 0.f;
-          float dent = -A.hp.ent_coef * inv_nb;  // d(ent_coef * ent_loss) / d(entropy)
+          dl_dlogp = (inside || pl1 < pl2) ? -adv * ratio * inv_nb : 0.f;
+          dent = -A.hp.ent_coef * inv_nb;  // d(ent_coef * ent_loss) / d(entropy)
           if (live) {
             if (la == 0) {
               l_pg += -fminf(pl1, pl2);
@@ -467,6 +538,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
           } else {
             dl_dlogp = 0.f;
             dent = 0.f;
+          }
           }
           if (!pd.discrete) {
             for (int a = la; a < Da; a += 8) {
@@ -539,7 +611,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
         const int o_w1 = net ? PL.w1[1] : PL.w1[0], o_b1 = net ? PL.b1[1] : PL.b1[0];
         const int o_w2 = net ? PL.w2[1] : PL.w2[0], o_b2 = net ? PL.b2[1] : PL.b2[0];
         float dz[16];
-        if (gj < h) {
+        if (gj < h && (!BC || net == 0)) {
           load16(dz, DZ2 + gj * RG);
           for (int i = wq; i < h; i += NWQ) GP[o_w2 + gj * ldh + i] += dot16r(dz, H1 + i * RG);
           if (wq == 0) GP[o_b2 + gj] += sum16(dz);
@@ -574,7 +646,13 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
     }
 
     // ---- 3. loss terms -> CTA 0; cluster barrier: every CTA's partial gradient is complete ---------------------------
-    if (loss_log) {  // (uniform)
+    float l2sum = 0.f;  // BC metrics: sum of w^2 at the minibatch's parameters (every CTA holds all of them)
+    if (BC && bc_log && crank == 0) {
+      float q = 0.f;
+      for (int i = tid; i < CL * S; i += PT) q = fmaf(Pm[i], Pm[i], q);  // (pad elements are 0)
+      l2sum = block_sum(q, red);
+    }
+    if (BC ? bc_log : loss_log != nullptr) {  // (uniform)
       const float s_pg = block_sum(l_pg, red);
       const float s_v = block_sum(l_v, red);
       const float s_ent = block_sum(l_ent, red);
@@ -600,8 +678,30 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
       loss_log[gs * 4 + 2] = el;
       loss_log[gs * 4 + 3] = pg + A.hp.ent_coef * el + A.hp.vf_coef * vl;
     }
+    if constexpr (BC) {
+      if (crank == 0 && tid == 0 && bc_log) {  // BCTrainingMetrics (bc.py:134-146)
+        float lp = 0.f, pt = 0.f, en = 0.f;
+        for (int c = 0; c < CL; ++c) {
+          lp += LOSS[c * 3 + 0];
+          pt += LOSS[c * 3 + 1];
+          en += LOSS[c * 3 + 2];
+        }
+        float* o = B.metrics + (int64_t)n_logged * 8;
+        const float neglogp = -(lp * inv_nb), entropy = en * inv_nb, ent_loss = -A.hp.ent_coef * entropy;
+        const float l2_norm = l2sum * 0.5f, l2_loss = B.l2_weight * l2_norm;
+        o[BC_M_NEGLOGP] = neglogp;
+        o[BC_M_ENTROPY] = entropy;
+        o[BC_M_ENT_LOSS] = ent_loss;
+        o[BC_M_PROB_TRUE_ACT] = pt * inv_nb;
+        o[BC_M_L2_NORM] = l2_norm;
+        o[BC_M_L2_LOSS] = l2_loss;
+        o[BC_M_LOSS] = neglogp + ent_loss + l2_loss;
+        o[BC_M_BATCH] = (float)batch_num;
+      }
+      if (bc_log) ++n_logged;
+    }
     // ---- 4. slice owners: sum the CL partials of the owned slice in fixed order (DSMEM loads), exchange the squared
-    //         slice norms for clip_grad_norm_ ---------------------------------------------------------------------------
+    //         slice norms for clip_grad_norm_.  BC: add the sum to the batch's gradient so far; no norms -------------
     float ss = 0.f;
     for (int i0 = 4 * tid; i0 < S; i0 += 4 * PT) {
       float4 g = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -611,34 +711,43 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
         const float4 t = ld4(rg + crank * S + i0);
         g.x += t.x, g.y += t.y, g.z += t.z, g.w += t.w;
       }
-      st4(Gs + i0, g);
-      ss += (g.x * g.x + g.y * g.y) + (g.z * g.z + g.w * g.w);
-    }
-    const float my_ssq = block_sum(ss, red);
-    if (tid < CL) {
-      cluster.map_shared_rank(SSQ, tid)[crank] = my_ssq;
-      if (kl_on) cluster.map_shared_rank(KLS, tid)[crank] = ppo_kl_part<RG>(RSL, inv_nb);
-    }
-    cluster.sync();  // all slice norms are in place everywhere; nobody reads a peer's GP any more
-    if (kl_on) {
-      // target_kl (SB3: approx_kl > 1.5 target_kl): the CL shares summed in the same order everywhere, so every CTA
-      // reaches the same decision; a stopping step takes no Adam step and all CTAs leave the loop here
-      float kl = 0.f;
-#pragma unroll
-      for (int c = 0; c < CL; ++c) kl += KLS[c];
-      if (kl > 1.5f * A.target_kl) {
-        kstop = gs + 1;
-        break;
+      if constexpr (BC) {  // loss.backward() accumulating into .grad (bc.py:502)
+        const float4 a = ld4(Gs + i0);
+        g.x = a.x + g.x, g.y = a.y + g.y, g.z = a.z + g.z, g.w = a.w + g.w;
       }
+      st4(Gs + i0, g);
+      if constexpr (!BC) ss += (g.x * g.x + g.y * g.y) + (g.z * g.z + g.w * g.w);
     }
-    // ---- 5. clip_grad_norm_ + Adam on the OWNED slice; the new parameters go into every CTA's parameter vector ---------
-    float total = 0.f;
+    float clip = 1.0f;  // BC: no clip_grad_norm_
+    if constexpr (!BC) {
+      const float my_ssq = block_sum(ss, red);
+      if (tid < CL) {
+        cluster.map_shared_rank(SSQ, tid)[crank] = my_ssq;
+        if (kl_on) cluster.map_shared_rank(KLS, tid)[crank] = ppo_kl_part<RG>(RSL, inv_nb);
+      }
+      cluster.sync();  // all slice norms are in place everywhere; nobody reads a peer's GP any more
+      if (kl_on) {
+        // target_kl (SB3: approx_kl > 1.5 target_kl): the CL shares summed in the same order everywhere, so every CTA
+        // reaches the same decision; a stopping step takes no Adam step and all CTAs leave the loop here
+        float kl = 0.f;
 #pragma unroll
-    for (int c = 0; c < CL; ++c) total += SSQ[c];  // same order everywhere: the replicas' clip factors agree bit for bit
-    total = sqrtf(total);
-    float clip = A.hp.max_grad_norm / (total + 1e-6f);
-    clip = clip > 1.0f ? 1.0f : clip;
-    {
+        for (int c = 0; c < CL; ++c) kl += KLS[c];
+        if (kl > 1.5f * A.target_kl) {
+          kstop = gs + 1;
+          break;
+        }
+      }
+      float total = 0.f;
+#pragma unroll
+      for (int c = 0; c < CL; ++c) total += SSQ[c];  // same order everywhere: the replicas' clip factors agree bit for bit
+      total = sqrtf(total);
+      clip = A.hp.max_grad_norm / (total + 1e-6f);
+      clip = clip > 1.0f ? 1.0f : clip;
+    }
+    // ---- 5. clip_grad_norm_ + Adam on the OWNED slice; the new parameters go into every CTA's parameter vector.  BC:
+    //         only a minibatch that ends a batch steps.  No CTA reads parameters between the barrier of section 3 and
+    //         the one below, nor a peer's GP after it, so one barrier closes a BC minibatch ----------------------------
+    if (bc_step) {
       const float step_size = bc[0], inv_bc2s = rcp_fast(bc[1]);
       auto adam1 = [&](float gg, float& m, float& v, float& pw) {
         gg *= clip;
@@ -647,8 +756,12 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
         pw -= step_size * __fdividef(m, fmaf(sqrt_fast(v), inv_bc2s, A.hp.adam_eps));
       };
       for (int i0 = 4 * tid; i0 < S; i0 += 4 * PT) {
-        const float4 g = ld4(Gs + i0);
+        float4 g = ld4(Gs + i0);
         float4 m = ld4(Ms + i0), v = ld4(Vs + i0), pw = ld4(Pm + crank * S + i0);
+        if constexpr (BC) {  // + the L2 term's gradient (bc.py:138-145, every parameter); the next batch starts from 0
+          g.x = fmaf(l2c, pw.x, g.x), g.y = fmaf(l2c, pw.y, g.y), g.z = fmaf(l2c, pw.z, g.z), g.w = fmaf(l2c, pw.w, g.w);
+          st4(Gs + i0, make_float4(0.f, 0.f, 0.f, 0.f));
+        }
         adam1(g.x, m.x, v.x, pw.x);
         adam1(g.y, m.y, v.y, pw.y);
         adam1(g.z, m.z, v.z, pw.z);
@@ -664,7 +777,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
     }
     cluster.sync();  // every CTA holds all new parameter slices
     start += mb;
-    if (start >= Ni) {
+    if (start >= (BC ? (int)steps_per_epoch * mb : Ni)) {  // (BC: the remainder rows are dropped, drop_last=True)
       start = 0;
       ++ep_now;
     }
@@ -676,6 +789,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
     if (q / S == crank) {
       g_m[p] = Ms[q - crank * S];
       g_v[p] = Vs[q - crank * S];
+      if (BC && (B.j0 + B.n_mb) % B.k != 0 && B.final_flush != 1) B.carry[p] = Gs[q - crank * S];  // the batch goes on
     }
   }
   if (crank == 0) {
@@ -689,7 +803,11 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
     }
     if (tid == 0) {
       state[IMB_ST_PPO_STEP] = kstop ? adam_step - 1 : adam_step;  // (the stopping step took no Adam step)
-      state[IMB_ST_PPO_EPOCH] = perm_draw0 + (kstop ? ep_now + 1 : A.hp.n_epochs);
+      if constexpr (BC) {  // the epochs the launch completed
+        state[IMB_ST_PPO_EPOCH] = perm_draw0 + (B.j0 + B.n_mb) / steps_per_epoch - B.j0 / steps_per_epoch;
+      } else {
+        state[IMB_ST_PPO_EPOCH] = perm_draw0 + (kstop ? ep_now + 1 : A.hp.n_epochs);
+      }
     }
   }
   if (A.stats) {

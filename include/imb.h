@@ -371,6 +371,38 @@ int imb_ppo_plan(const imb_policy_desc* pol, int32_t pol_act, int32_t batch_size
  * IMB_PPO_FORCE_RUNTIME_SHAPE=1, which imb_ppo_update reads at every call and which makes it run instantiation 0. */
 int imb_ppo_update_variant(const imb_policy_desc* pol);
 
+/* Behavioural cloning: minibatches [j0, j0 + n_minibatches) of one BC.train() call (algorithms/bc.py:381-510) as ONE
+ * launch of k_ppo_update_gen with the BC loss (the PPO update's persistent cluster kernel, forward / backward / slice
+ * reduction / Adam shared with PPO).  Per minibatch: evaluate_actions on its rows, loss = -mean logp
+ * - ent_weight * mean entropy + l2_weight * sum(w^2) / 2 (BehaviorCloningLossCalculator, bc.py:94-156) scaled by
+ * minibatch_size / batch_size (bc.py:501) and accumulated; every batch_size / minibatch_size minibatches of the call
+ * (bc.py:505) and after the call's last minibatch when final_flush = 1 (the incomplete batch, bc.py:507-510) one torch
+ * Adam step (betas 0.9 / 0.999, lr, adam_eps; no gradient clipping).  final_flush = 2: the last minibatch ends the call
+ * but its incomplete batch steps in a later flush-only launch (n_minibatches = 0, final_flush = 1, j0 = the call's
+ * minibatch count), as the reference steps it after the last on_epoch_end; this launch writes the batch's metrics.  The value tower is not evaluated; its parameters get
+ * only the L2 term.
+ *  - table: [n_rows][imb_rollout_row_width(pol)] rollout-format rows; only obs | act (Discrete: the index) are read.
+ *  - perm: int64 [epochs][n_rows], the DataLoader(shuffle=True, drop_last=True) order of the epochs the launch touches,
+ *    from epoch j0 / (n_rows / minibatch_size) on; minibatch i is perm[epoch][(i % (n_rows / minibatch_size)) * mb ...].
+ *  - norm_update: the policy is in training mode, so each minibatch updates the feature RunningNorm before its forward
+ *    pass (evaluate_actions); 0 normalises with the statistics as they stand.
+ *  - grad_carry: [n_params] floats (flat order), needed when batch_size > minibatch_size: the summed gradient of a batch
+ *    a launch ends inside (j0 + n_minibatches not a multiple of batch_size / minibatch_size, final_flush 0), read back by
+ *    the launch that starts inside it.
+ *  - metrics (optional): [n_logged][8] = neglogp, entropy, ent_loss, prob_true_act, l2_norm, l2_loss, loss
+ *    (BCTrainingMetrics of the batch's last minibatch; l2_norm at its parameters) and the batch number, one row per
+ *    batch that steps in this launch whose number (bc.py:504-509) is a multiple of log_interval, in order.
+ *  - state[IMB_ST_PPO_STEP]: the Adam step count, advanced per step; state[IMB_ST_PPO_EPOCH]: epochs completed.
+ * A split train() computes the same bits as one launch. */
+int imb_bc_train(const imb_policy_desc* pol, int32_t pol_act, float* pol_params, float* pol_norm,
+                 int32_t* pol_norm_count, float* exp_avg, float* exp_avg_sq, const float* table, int64_t n_rows,
+                 int32_t minibatch_size, int32_t batch_size, int64_t j0, int64_t n_minibatches, int32_t final_flush,
+                 float l2_weight, float ent_weight, float lr, float adam_eps, int32_t norm_update, const int64_t* perm,
+                 float* grad_carry, float* metrics, int32_t log_interval, int64_t* state, void* stream);
+/* The kernel imb_bc_train runs for `pol` at minibatch_size (IMB_PPO_PLAN_GEN1 or IMB_PPO_PLAN_GEN2); host only, no GPU
+ * needed.  <0 (imb_last_error() names the shared-memory need and limit) when the shape does not fit. */
+int imb_bc_plan(const imb_policy_desc* pol, int32_t pol_act, int32_t minibatch_size);
+
 /* log pi(a|s) of the generator policy for the disc batch (common.py:476-519 ->
  * ActorCriticPolicy.evaluate_actions), written into the batch's last feature row. */
 int imb_policy_logp(const imb_policy_desc* pol, int32_t pol_act, const float* pol_params, const float* pol_norm,
