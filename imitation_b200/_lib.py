@@ -164,6 +164,9 @@ SIGNATURES = {
     "imb_ensemble_relabel": (_i32, [_pu, _f32, _ptr, _i32, _i32, _i64, _i64, _ptr, _ptr], None),
     "imb_rollout_explore": (_i32, [_env, _ptr, _ptr, _pol, _i32, _ptr, _ptr, _disc, _ptr, _ptr, _members, _i32, _hp,
                                    _i64, _i64, _ptr, _ptr, _ptr, _ptr, _i32, _ptr, _u64, _i64, _ptr, _ptr], 1),
+    "imb_rollout_dagger": (_i32, [_env, _ptr, _ptr, _pol, _i32, _ptr, _ptr, _pol, _i32, _ptr, _ptr, _i64, _i64, _ptr, _ptr,
+                                  _ptr, _ptr, _ptr, _i32, _ptr, _ptr, _ptr], 1),
+    "imb_rollout_dagger_plan": (_i32, [_pol, _pol, _i64, _i32], 0),
     "imb_density_ws_floats": (_i64, [_i64], 0),
     "imb_density_score": (_i32, [_i32, _i32, _i32, _i32, _i32, _i32, _f32, _i32, _i64, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr,
                                  _ptr, _i32, _ptr, _i64, _i32, _ptr, _ptr, _i64, _i64, _i32, _ptr, _i64, _ptr, _ptr], None),
@@ -488,6 +491,29 @@ def rollout_explore(env, env_params, env_obs, pol, pol_params, pol_norm, disc, d
                                      members, reward_mode, hp, n_envs, n_steps, _p(rollout_tbl, th.float32),
                                      _p(flat_out), _p(aux, th.float32), _p(noise), flags, _p(explore_policy, th.uint8),
                                      explore_seed, explore_step0, _p(state, th.int64), _stream()), "imb_rollout_explore")
+
+
+def rollout_dagger(env, env_params, env_obs, expert, expert_params, expert_norm, learner, learner_params, learner_norm,
+                   n_envs, n_steps, rollout_tbl, flat_out, aux, noise, robot_noise, robot_mask, state, flags=0,
+                   expert_act=ACT_TANH, learner_act=ACT_TANH):
+    """The DAgger rollout (imb_rollout_dagger): the expert acts, except where robot_mask[t][e] (uint8 [n_steps][n_envs])
+    is 1, where env e executes the learner's sampled action; rows obs | the expert's clipped action (or index).
+    noise / robot_noise (None: Philox) pin the expert's / the learner's sampling, laid out as `rollout`'s noise."""
+    _check(lib().imb_rollout_dagger(env, _p(env_params, th.float32), _p(env_obs, th.float32), expert, expert_act,
+                                    _p(expert_params, th.float32), _p(expert_norm), learner, learner_act,
+                                    _p(learner_params, th.float32), _p(learner_norm), n_envs, n_steps,
+                                    _p(rollout_tbl, th.float32), _p(flat_out), _p(aux, th.float32), _p(noise),
+                                    _p(robot_noise), flags, _p(robot_mask, th.uint8), _p(state, th.int64), _stream()),
+           "imb_rollout_dagger")
+
+
+def rollout_dagger_plan(expert: PolicyDesc, learner: PolicyDesc, n_envs: int, n_sms: int = 0) -> int:
+    """Rows per CTA (8, 32, 64 or 128) `rollout_dagger` runs for these policies over n_envs envs on n_sms SMs (<= 0: the
+    current device's).  Host only; ImbError when not even the 8-row tile fits."""
+    rc = lib().imb_rollout_dagger_plan(expert, learner, n_envs, n_sms)
+    if rc < 0:
+        raise ImbError(f"imb_rollout_dagger_plan: {lib().imb_last_error().decode()} (rc={rc})")
+    return rc
 
 
 def density_ws_floats(n_query: int) -> int:

@@ -256,6 +256,22 @@ class BC(algo_base.DemonstrationAlgorithm):
         self._shuffle = shuffle
         self._demo_table = self.demo_table(obs, acts).to(self._dev)
 
+    def _set_demonstration_rows(self, table: th.Tensor, n: int, loader_batch_size: int) -> None:
+        """Demonstrations from the first n rows of a device table in the kernel's row format, each epoch shuffled as
+        the reference's `DataLoader(transitions, loader_batch_size, shuffle=True, drop_last=True)` is (DAgger's
+        dataset).  The reference's errors for a loader batch that is not minibatch_size rows and for fewer than
+        minibatch_size rows."""
+        if loader_batch_size != self.minibatch_size:
+            raise ValueError(f"Expected batch size {self.minibatch_size} != {loader_batch_size} = len(batch['obs'])")
+        if n < self.minibatch_size:
+            raise ValueError(f"Number of transitions in `demonstrations` {n} is smaller than batch size "
+                             f"{self.minibatch_size}.")
+        if not table.is_cuda or table.shape[1] != _lib.rollout_row_width(self.policy.desc):
+            raise ValueError("the demonstration table must be a device table in the kernel's row format")
+        self._demo_table = table
+        self._demo_n = n
+        self._shuffle = True
+
     def _demo_arrays(self, demonstrations) -> Tuple[np.ndarray, np.ndarray, bool]:
         return demonstration_arrays(demonstrations, self.minibatch_size)
 

@@ -120,6 +120,7 @@ __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, u
 #define IMB_STREAM_EXPERT 0x4004u
 #define IMB_STREAM_PPO_PERM 0x5005u
 #define IMB_STREAM_EXPLORE 0x7007u  // random-policy actions of the exploration rollout (0x6006: oracle expert policy)
+#define IMB_STREAM_DAGGER 0x8008u   // the learner's sampled actions in the DAgger rollout
 
 struct Philox4 {
   uint32_t x, y, z, w;

@@ -43,7 +43,7 @@ static int rollout_common(const imb_env_desc* env, const float* env_params, floa
                           const float* disc_params, const float* disc_norm, const imb_rollout_members* members,
                           int reward_mode, const imb_ppo_hparams* hp, int64_t n_envs, int64_t n_steps, float* rollout,
                           float* ring, int64_t ring_capacity, float* flat_out, float* aux, const float* noise, int flags,
-                          const int64_t* state, const RolloutExplore* Xp, void* stream) {
+                          const int64_t* state, const RolloutExplore* Xp, const RolloutDagger* Dg, void* stream) {
   IMB_REQUIRE(n_envs >= 1 && n_steps >= 1, "rollout needs n_envs, n_steps >= 1");
   IMB_REQUIRE(env->d_obs == pol->d_obs && env->d_act == pol->d_act && env->discrete == pol->discrete,
               "env / policy space mismatch");
@@ -71,7 +71,7 @@ static int rollout_common(const imb_env_desc* env, const float* env_params, floa
   cudaStream_t st = (cudaStream_t)stream;
   if (!members)
     return launch_rollout(A, pol_act, L, nullptr, env_params, env_obs, pol_params, pol_norm, disc_params, rollout, ring,
-                          flat_out, aux, noise, state, Xp, st);
+                          flat_out, aux, noise, state, Xp, Dg, st);
   const int M = members->n_members;
   IMB_REQUIRE(M >= 2 && M <= IMB_PU_MAX_MEMBERS, "imb_rollout_ensemble: %d members (2 to %d)", M, IMB_PU_MAX_MEMBERS);
   IMB_REQUIRE(members->raw != nullptr, "imb_rollout_ensemble: no raw-output buffer");
@@ -90,7 +90,7 @@ static int rollout_common(const imb_env_desc* env, const float* env_params, floa
     }
   }
   return launch_rollout(A, pol_act, L, &Mb, env_params, env_obs, pol_params, pol_norm, nullptr, rollout, ring, flat_out,
-                        aux, noise, state, Xp, st);
+                        aux, noise, state, Xp, Dg, st);
 }
 
 extern "C" int imb_rollout(const imb_env_desc* env, const float* env_params, float* env_obs,
@@ -101,7 +101,7 @@ extern "C" int imb_rollout(const imb_env_desc* env, const float* env_params, flo
                            const float* noise, int flags, const int64_t* state, void* stream) {
   return rollout_common(env, env_params, env_obs, pol, pol_act, pol_params, pol_norm, disc, disc_params, disc_norm,
                         nullptr, reward_mode, hp, n_envs, n_steps, rollout, ring, ring_capacity, flat_out, aux, noise,
-                        flags, state, nullptr, stream);
+                        flags, state, nullptr, nullptr, stream);
 }
 
 extern "C" int imb_rollout_ensemble(const imb_env_desc* env, const float* env_params, float* env_obs,
@@ -113,7 +113,7 @@ extern "C" int imb_rollout_ensemble(const imb_env_desc* env, const float* env_pa
   IMB_REQUIRE(disc && members, "imb_rollout_ensemble needs a member architecture and a member table");
   return rollout_common(env, env_params, env_obs, pol, pol_act, pol_params, pol_norm, disc, nullptr, nullptr, members, 2,
                         hp, n_envs, n_steps, rollout, ring, ring_capacity, flat_out, aux, noise, flags, state, nullptr,
-                        stream);
+                        nullptr, stream);
 }
 
 extern "C" int imb_rollout_explore(const imb_env_desc* env, const float* env_params, float* env_obs,
@@ -133,7 +133,62 @@ extern "C" int imb_rollout_explore(const imb_env_desc* env, const float* env_par
   Xp.step0 = explore_step0;
   return rollout_common(env, env_params, env_obs, pol, pol_act, pol_params, pol_norm, disc, disc_params, disc_norm,
                         members, reward_mode, hp, n_envs, n_steps, rollout, nullptr, 0, flat_out, aux, noise, flags,
-                        state, &Xp, stream);
+                        state, &Xp, nullptr, stream);
+}
+
+// the learner of a DAgger rollout against the expert it stands in for
+static int check_learner(const imb_policy_desc* expert, const imb_policy_desc* learner, int learner_act) {
+  IMB_REQUIRE(expert && learner, "the DAgger rollout needs an expert and a learner policy");
+  IMB_REQUIRE(learner->d_obs == expert->d_obs && learner->d_act == expert->d_act &&
+                  learner->discrete == expert->discrete,
+              "expert / learner space mismatch");
+  IMB_REQUIRE(learner_act == IMB_ACT_TANH || learner_act == IMB_ACT_RELU,
+              "learner_act must be IMB_ACT_TANH (0) or IMB_ACT_RELU (1), got %d", learner_act);
+  return check_shapes(learner, nullptr);
+}
+
+extern "C" int imb_rollout_dagger_plan(const imb_policy_desc* expert, const imb_policy_desc* learner, int64_t n_envs,
+                                       int32_t n_sms) {
+  IMB_REQUIRE(n_envs >= 1, "rollout plan needs n_envs >= 1");
+  if (int rc = check_learner(expert, learner, IMB_ACT_TANH)) return rc;
+  if (int rc = check_shapes(expert, nullptr)) return rc;
+  RolloutArgs A;
+  memset(&A, 0, sizeof(A));
+  A.env.d_obs = expert->d_obs;
+  A.env.d_act = expert->d_act;
+  A.pol = *expert;
+  A.E = n_envs;
+  DiscLaunch L;
+  memset(&L, 0, sizeof(L));
+  RolloutDagger Dg;
+  memset(&Dg, 0, sizeof(Dg));
+  Dg.pol = *learner;
+  const int rpl = rollout_plan(A, L, 1, n_sms > 0 ? n_sms : imb_num_sms(), &Dg);
+  return rpl < 0 ? rpl : rows_of(rpl);
+}
+
+extern "C" int imb_rollout_dagger(const imb_env_desc* env, const float* env_params, float* env_obs,
+                                  const imb_policy_desc* expert, int32_t expert_act, const float* expert_params,
+                                  const float* expert_norm, const imb_policy_desc* learner, int32_t learner_act,
+                                  const float* learner_params, const float* learner_norm, int64_t n_envs,
+                                  int64_t n_steps, float* rollout, float* flat_out, float* aux, const float* noise,
+                                  const float* robot_noise, int flags, const uint8_t* robot_mask,
+                                  const int64_t* state, void* stream) {
+  IMB_REQUIRE(robot_mask != nullptr, "imb_rollout_dagger needs the [n_steps][n_envs] robot mask");
+  if (int rc = check_learner(expert, learner, learner_act)) return rc;
+  RolloutDagger Dg;
+  memset(&Dg, 0, sizeof(Dg));
+  Dg.pol = *learner;
+  Dg.act = learner_act;
+  Dg.params = learner_params;
+  Dg.norm = learner_norm;
+  Dg.noise = robot_noise;
+  Dg.mask = robot_mask;
+  imb_ppo_hparams hp;
+  memset(&hp, 0, sizeof(hp));
+  return rollout_common(env, env_params, env_obs, expert, expert_act, expert_params, expert_norm, nullptr, nullptr,
+                        nullptr, nullptr, 0, &hp, n_envs, n_steps, rollout, nullptr, 0, flat_out, aux, noise, flags,
+                        state, nullptr, &Dg, stream);
 }
 
 extern "C" int imb_rollout_advance(int64_t* state, int64_t n_envs, int64_t n_steps, int32_t horizon,

@@ -66,11 +66,106 @@ struct RolloutExplore {
   int64_t step0;
 };
 
+// DAgger rollout (imb_rollout_dagger, algorithms/dagger.py): the policy of k_rollout is the expert; a second policy image,
+// the learner (its own width, activation and feature norm), sits beside it.  mask[t * E + e] = 1 makes env e execute
+// the learner's action at step t (sampled from Philox stream IMB_STREAM_DAGGER at counter (env id, global step + t,
+// a / 4), or read from `noise`, laid out as k_rollout's); the row records obs | the expert's action, clipped to the Box.
+struct RolloutDagger {
+  imb_policy_desc pol;
+  int act;          // the learner's tower activation (ACT_TANH / ACT_RELU)
+  int HP, img_off;  // the learner's padded width and image offset (floats), set by rollout_layout
+  const float* params;
+  const float* norm;
+  const float* noise;
+  const uint8_t* mask;
+};
+
+enum { RM_PLAIN = 0, RM_EXPLORE = 1, RM_DAGGER = 2 };
+
+// The action head of one policy for this thread's tile row (thread per env), on the pi latent H2: Box -> mean + std * z,
+// z = 0 (deterministic), the pinned noise[nidx * Da + a] or a normal of Philox stream `stream` at counter (egid, ctr,
+// a / 4); Discrete -> inverse-CDF sampling with the uniform noise[nidx] or one of that stream (argmax when
+// deterministic).  CTRL[a * RRS] receives the control the env sees (the clipped action / the one-hot; Discrete uses it
+// for the logits first); rec (nullable) the recorded action: Box unclipped unless clip_rec, Discrete the index.
+// Returns log pi(action).
+__device__ __forceinline__ float action_head(const float* __restrict__ psm, const PolImg& S, int HP, int h, int Da,
+                                             bool discrete, const float* __restrict__ H2, int RRS, int rt,
+                                             float* __restrict__ CTRL, float* __restrict__ rec, bool clip_rec,
+                                             bool deterministic, const float* __restrict__ noise, int64_t nidx,
+                                             bool live, uint64_t seed, uint32_t stream, uint32_t egid, uint32_t ctr) {
+  float logp = 0.f;
+  if (!discrete) {
+    float z4[4] = {0.f, 0.f, 0.f, 0.f};
+    for (int a = 0; a < Da; ++a) {
+      float m0 = 0.f, m1 = 0.f;
+      const float* wa = psm + S.wa + a * HP;
+      int j = 0;
+      for (; j + 2 <= h; j += 2) {
+        m0 = fmaf(wa[j], H2[j * RRS + rt], m0);
+        m1 = fmaf(wa[j + 1], H2[(j + 1) * RRS + rt], m1);
+      }
+      if (j < h) m0 = fmaf(wa[j], H2[j * RRS + rt], m0);
+      const float m = psm[S.ba + a] + (m0 + m1);
+      if (!deterministic && !noise && (a & 3) == 0) philox_normal4(seed, stream, egid, ctr, a >> 2, z4);
+      const float z = deterministic ? 0.f : noise ? (live ? noise[nidx * Da + a] : 0.f) : ((a & 3) == 0 ? z4[0] : (a & 3) == 1 ? z4[1] : (a & 3) == 2 ? z4[2] : z4[3]);
+      const float ls = psm[S.lstd + a];
+      const float sd = expf(ls);
+      const float act = fmaf(sd, z, m);
+      const float diff = act - m;
+      logp += -(diff * diff) / (2.0f * sd * sd) - ls - 0.9189385332046727f;
+      const float ctl = fminf(fmaxf(act, -1.0f), 1.0f);
+      if (rec) rec[a] = clip_rec ? ctl : act;  // SB3 stores the UNCLIPPED action; predict() returns the clipped one
+      CTRL[a * RRS] = ctl;                     // env and wrappers see the clipped one
+    }
+  } else {
+    float mx = -INFINITY;
+    for (int a = 0; a < Da; ++a) {
+      float m0 = 0.f;
+      const float* wa = psm + S.wa + a * HP;
+      for (int j = 0; j < h; ++j) m0 = fmaf(wa[j], H2[j * RRS + rt], m0);
+      const float m = psm[S.ba + a] + m0;
+      CTRL[a * RRS] = m;  // logits, overwritten by the one-hot below
+      mx = fmaxf(mx, m);
+    }
+    float se = 0.f;
+    for (int a = 0; a < Da; ++a) se += expf(CTRL[a * RRS] - mx);
+    const float lse = mx + logf(se);
+    float u;
+    if (noise) {
+      u = live ? noise[nidx] : 0.f;
+    } else {
+      uint32_t k0, k1;
+      philox_key(seed, stream, k0, k1);
+      u = u01(philox4x32(egid, ctr, 0u, 0u, k0, k1).x);
+    }
+    int chosen = Da - 1;
+    float cdf = 0.f;
+    bool found = false;
+    for (int a = 0; a < Da; ++a) {
+      cdf += expf(CTRL[a * RRS] - lse);
+      if (!found && !(u >= cdf)) {
+        chosen = a;
+        found = true;
+      }
+    }
+    if (deterministic) {
+      chosen = 0;
+      for (int a = 1; a < Da; ++a)
+        if (CTRL[a * RRS] > CTRL[chosen * RRS]) chosen = a;
+    }
+    logp = CTRL[chosen * RRS] - lse;
+    for (int a = 0; a < Da; ++a) CTRL[a * RRS] = (a == chosen) ? 1.f : 0.f;
+    if (rec) rec[0] = (float)chosen;
+  }
+  return logp;
+}
+
 // ENS: evaluate the Mb.M ensemble members (raw outputs to Mb.raw) instead of the one net at disc_params (reward column);
 // the single-net variant has no member loop.  ACT: the policy towers' activation (env and reward net keep their own).
-// EXP: the exploration rollout, Xp.policy[t] picks the policy of step t (random steps skip the policy towers and
-// record logp = value = 0); without it Xp is unused.
-template <int RPL, bool ENS, int ACT, bool EXP>
+// MODE RM_EXPLORE: the exploration rollout, Xp.policy[t] picks the policy of step t (random steps skip the policy
+// towers and record logp = value = 0); otherwise Xp is unused.  MODE RM_DAGGER: the DAgger rollout (Dg; LACT the
+// learner's activation): no value tower, bootstrap, reward net or ring, rows obs | expert label; otherwise Dg is unused.
+template <int RPL, bool ENS, int ACT, int MODE, int LACT>
 __global__ void __launch_bounds__(RT, 1) k_rollout(const RolloutArgs A, const DiscLaunch L, const RolloutMembers Mb,
                                                    const float* __restrict__ env_params, float* __restrict__ env_obs,
                                                    const float* __restrict__ pol_params,
@@ -78,7 +173,9 @@ __global__ void __launch_bounds__(RT, 1) k_rollout(const RolloutArgs A, const Di
                                                    const float* __restrict__ disc_params, float* __restrict__ rollout,
                                                    float* __restrict__ ring, float* __restrict__ flat_out,
                                                    float* __restrict__ aux, const float* __restrict__ noise,
-                                                   const int64_t* __restrict__ state, const RolloutExplore Xp) {
+                                                   const int64_t* __restrict__ state, const RolloutExplore Xp,
+                                                   const RolloutDagger Dg) {
+  constexpr bool DAG = MODE == RM_DAGGER;
   constexpr int RR = rows_of(RPL), RRS = RR + TILE_PAD;
   extern __shared__ __align__(128) float smem[];
   const int tid = threadIdx.x;
@@ -104,6 +201,9 @@ __global__ void __launch_bounds__(RT, 1) k_rollout(const RolloutArgs A, const Di
         load_timg(smem + A.img_off + (m * L.npass + p) * A.img_sz, L.pass[p], JP, ENS ? Mb.params[m] : disc_params,
                   ENS ? Mb.norm[m][p] : (L.pass[p].has_norm ? L.pass[p].norm : nullptr), L.pass[p].eps);
   load_policy_img(psm, S, A.pol, HP, pol_params, pol_norm);
+  const PolImg LS(Do, Da, DAG ? Dg.HP : HP);
+  float* lsm = smem + (DAG ? Dg.img_off : A.pol_off);
+  if (DAG) load_policy_img(lsm, LS, Dg.pol, Dg.HP, Dg.params, Dg.norm);
   for (int i = tid; i < (KU + 2) * IP; i += RT) esm[i] = 0.f;
   __syncthreads();
   {
@@ -177,18 +277,18 @@ __global__ void __launch_bounds__(RT, 1) k_rollout(const RolloutArgs A, const Di
     if (j < h) v0 = fmaf(psm[S.wv + j], H2[j * RRS + rt], v0);
     return psm[S.bv] + (v0 + v1);
   };
-  // XN <- feature-normalised copy of a [Do][RRS] observation tile
-  auto norm_obs = [&](const float* __restrict__ SRC) {
+  // XN <- copy of a [Do][RRS] observation tile normalised by the features of policy image img
+  auto norm_obs = [&](const float* __restrict__ SRC, const float* __restrict__ img, const PolImg& SI) {
     for (int i = tid; i < Do * (RR / 4); i += RT) {
       const int k = i / (RR / 4), r4 = (i - k * (RR / 4)) * 4;
       const float4 x = ld4(SRC + k * RRS + r4);
-      const float m = psm[S.mean + k], is = psm[S.istd + k];
+      const float m = img[SI.mean + k], is = img[SI.istd + k];
       st4(XN + k * RRS + r4, make_float4((x.x - m) * is, (x.y - m) * is, (x.z - m) * is, (x.w - m) * is));
     }
     __syncthreads();
   };
   auto value_of_obs = [&](const float* __restrict__ SRC) {
-    norm_obs(SRC);
+    norm_obs(SRC, psm, S);
     tile_layer<ACT, RPL>(XN, Do, psm + S.w1v, HP, psm + S.b1v, H1, HP);
     __syncthreads();
     tile_layer<ACT, RPL>(H1, h, psm + S.w2v, HP, psm + S.b2v, H2, HP);
@@ -201,11 +301,12 @@ __global__ void __launch_bounds__(RT, 1) k_rollout(const RolloutArgs A, const Di
   bool done = false;
   for (int64_t t = 0; t < T; ++t) {
     float* row = rollout + (e * T + t) * rw;
-    const bool rnd = EXP && Xp.policy[t] != 0;  // block-uniform: one entry per step
+    const bool rnd = MODE == RM_EXPLORE && Xp.policy[t] != 0;  // block-uniform: one entry per step
     // ---- policy: value tower, then pi tower (H2 ends up holding the pi latent) ------------------------------
     float value = 0.f;
     if (!rnd) {
-      value = value_of_obs(OBSU);
+      if (DAG) norm_obs(OBSU, psm, S);
+      else value = value_of_obs(OBSU);
       tile_layer<ACT, RPL>(XN, Do, psm + S.w1p, HP, psm + S.b1p, H1, HP);
       __syncthreads();
       tile_layer<ACT, RPL>(H1, h, psm + S.w2p, HP, psm + S.b2p, H2, HP);
@@ -237,73 +338,32 @@ __global__ void __launch_bounds__(RT, 1) k_rollout(const RolloutArgs A, const Di
         for (int a = 0; a < Da; ++a) OBSU[(Do + a) * RRS + tid] = (a == chosen) ? 1.f : 0.f;
         if (live) row[Do] = (float)chosen;
       }
-    } else if (!A.pol.discrete) {
-      float z4[4] = {0.f, 0.f, 0.f, 0.f};
-      for (int a = 0; a < Da; ++a) {
-        float m0 = 0.f, m1 = 0.f;
-        const float* wa = psm + S.wa + a * HP;
-        int j = 0;
-        for (; j + 2 <= h; j += 2) {
-          m0 = fmaf(wa[j], H2[j * RRS + rt], m0);
-          m1 = fmaf(wa[j + 1], H2[(j + 1) * RRS + rt], m1);
-        }
-        if (j < h) m0 = fmaf(wa[j], H2[j * RRS + rt], m0);
-        const float m = psm[S.ba + a] + (m0 + m1);
-        if (!A.deterministic && !noise && (a & 3) == 0)
-          philox_normal4(A.env.seed, IMB_STREAM_ACT_NOISE, egid, (uint32_t)(gstep0 + t), a >> 2, z4);
-        const float z = A.deterministic ? 0.f : noise ? (live ? noise[(t * E + e) * Da + a] : 0.f) : ((a & 3) == 0 ? z4[0] : (a & 3) == 1 ? z4[1] : (a & 3) == 2 ? z4[2] : z4[3]);
-        const float ls = psm[S.lstd + a];
-        const float sd = expf(ls);
-        const float act = fmaf(sd, z, m);
-        const float diff = act - m;
-        logp += -(diff * diff) / (2.0f * sd * sd) - ls - 0.9189385332046727f;
-        if (live) row[Do + a] = act;                                   // SB3 stores the UNCLIPPED action
-        OBSU[(Do + a) * RRS + tid] = fminf(fmaxf(act, -1.0f), 1.0f);   // env and wrappers see the clipped one
-      }
     } else {
-      float mx = -INFINITY;
-      for (int a = 0; a < Da; ++a) {
-        float m0 = 0.f;
-        const float* wa = psm + S.wa + a * HP;
-        for (int j = 0; j < h; ++j) m0 = fmaf(wa[j], H2[j * RRS + rt], m0);
-        const float m = psm[S.ba + a] + m0;
-        OBSU[(Do + a) * RRS + tid] = m;  // logits, overwritten by the one-hot below
-        mx = fmaxf(mx, m);
+      logp = action_head(psm, S, HP, h, Da, A.pol.discrete, H2, RRS, rt, OBSU + Do * RRS + tid, live ? row + Do : nullptr,
+                         DAG, A.deterministic, noise, t * E + e, live, A.env.seed, IMB_STREAM_ACT_NOISE, egid,
+                         (uint32_t)(gstep0 + t));
+    }
+    if (DAG) {
+      // ---- the learner acts where the mask says so; its tower runs only when some row of the tile needs it --------
+      const bool robot = live && Dg.mask[t * E + e] != 0;
+      if (__syncthreads_or(robot)) {
+        const int lh = Dg.pol.hidden, LHP = Dg.HP;
+        norm_obs(OBSU, lsm, LS);
+        tile_layer<LACT, RPL>(XN, Do, lsm + LS.w1p, LHP, lsm + LS.b1p, H1, LHP);
+        __syncthreads();
+        tile_layer<LACT, RPL>(H1, lh, lsm + LS.w2p, LHP, lsm + LS.b2p, H2, LHP);
+        __syncthreads();
+        if (robot)
+          action_head(lsm, LS, LHP, lh, Da, Dg.pol.discrete, H2, RRS, rt, OBSU + Do * RRS + tid, nullptr, false, false,
+                      Dg.noise, t * E + e, live, A.env.seed, IMB_STREAM_DAGGER, egid, (uint32_t)(gstep0 + t));
       }
-      float se = 0.f;
-      for (int a = 0; a < Da; ++a) se += expf(OBSU[(Do + a) * RRS + tid] - mx);
-      const float lse = mx + logf(se);
-      float u;
-      if (noise) {
-        u = live ? noise[t * E + e] : 0.f;
-      } else {
-        uint32_t k0, k1;
-        philox_key(A.env.seed, IMB_STREAM_ACT_NOISE, k0, k1);
-        u = u01(philox4x32(egid, (uint32_t)(gstep0 + t), 0u, 0u, k0, k1).x);
-      }
-      int chosen = Da - 1;
-      float cdf = 0.f;
-      bool found = false;
-      for (int a = 0; a < Da; ++a) {
-        cdf += expf(OBSU[(Do + a) * RRS + tid] - lse);
-        if (!found && !(u >= cdf)) {
-          chosen = a;
-          found = true;
-        }
-      }
-      if (A.deterministic) {
-        chosen = 0;
-        for (int a = 1; a < Da; ++a)
-          if (OBSU[(Do + a) * RRS + tid] > OBSU[(Do + chosen) * RRS + tid]) chosen = a;
-      }
-      logp = OBSU[(Do + chosen) * RRS + tid] - lse;
-      for (int a = 0; a < Da; ++a) OBSU[(Do + a) * RRS + tid] = (a == chosen) ? 1.f : 0.f;
-      if (live) row[Do] = (float)chosen;
     }
     if (live) {
       for (int k = 0; k < Do; ++k) row[k] = OBSU[k * RRS + tid];
-      row[col_logp] = logp;
-      row[col_val] = value;
+      if (!DAG) {
+        row[col_logp] = logp;
+        row[col_val] = value;
+      }
     }
     __syncthreads();
 
@@ -379,7 +439,7 @@ __global__ void __launch_bounds__(RT, 1) k_rollout(const RolloutArgs A, const Di
 
     // ---- time-limit bootstrap term gamma * V(terminal obs) (added after reward normalisation) -------------------
     float boot = 0.f;
-    if (done) boot = A.hp.gamma * value_of_obs(NOBS);  // block-uniform branch (lock-step envs)
+    if (!DAG && done) boot = A.hp.gamma * value_of_obs(NOBS);  // block-uniform branch (lock-step envs)
     if (live) {
       aux[2 * E + e * T + t] = boot;
       aux[2 * E + E * T + e * T + t] = rew_env;  // ground-truth env reward (BufferingWrapper records it)
@@ -409,7 +469,7 @@ __global__ void __launch_bounds__(RT, 1) k_rollout(const RolloutArgs A, const Di
     __syncthreads();
   }
   // ---- tail: state back to HBM, V(last obs) for GAE ------------------------------------------------------
-  const float vlast = value_of_obs(OBSU);
+  const float vlast = DAG ? 0.f : value_of_obs(OBSU);
   if (bulk_tile) {  // state tile back to HBM through the TMA unit as well (shared -> global bulk copies)
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     __syncthreads();
@@ -484,9 +544,10 @@ __global__ void k_env_reset(float* __restrict__ env_obs, int64_t E, int d_obs, u
 }  // namespace
 
 // Shared-memory layout of k_rollout for a tile of rows_of(rpl) envs and n_members reward nets (A.reward_mode, A.env and
-// A.pol set): fills A's widths and offsets (floats) and returns the bytes; n_img_floats receives the reward-net images'
-// share.
-static size_t rollout_layout(RolloutArgs& A, const DiscLaunch& L, int n_members, int rpl, size_t* n_img_floats) {
+// A.pol set) and, with Dg (Dg->pol set), the DAgger learner's image: fills A's (and Dg's) widths and offsets (floats) and
+// returns the bytes; n_img_floats receives the reward-net images' share.
+static size_t rollout_layout(RolloutArgs& A, const DiscLaunch& L, int n_members, int rpl, size_t* n_img_floats,
+                             RolloutDagger* Dg = nullptr) {
   const int RRS = rows_of(rpl) + TILE_PAD;
   auto al = [](int x) { return (x + 31) / 32 * 32; };
   const int Do = A.env.d_obs, Da = A.env.d_act;
@@ -496,10 +557,16 @@ static size_t rollout_layout(RolloutArgs& A, const DiscLaunch& L, int n_members,
   const LaunchWidths lw = A.reward_mode != 0 ? launch_widths(L) : LaunchWidths{32, Do};
   A.JP = lw.JP;
   const int dmax = lw.dmax > Do ? lw.dmax : Do;
-  const int wmax = A.HP > A.JP ? A.HP : A.JP;
+  int wmax = A.HP > A.JP ? A.HP : A.JP;
   int o = 0;
   A.pol_off = o;
   o += al(PolImg(Do, Da, A.HP).total);
+  if (Dg) {
+    Dg->HP = Dg->pol.hidden <= 32 ? 32 : 64;
+    wmax = wmax > Dg->HP ? wmax : Dg->HP;
+    Dg->img_off = o;
+    o += al(PolImg(Do, Da, Dg->HP).total);
+  }
   A.env_off = o;
   o += al((A.KU + 2) * A.IP);
   A.img_off = o;
@@ -528,12 +595,12 @@ static size_t rollout_layout(RolloutArgs& A, const DiscLaunch& L, int n_members,
 // SM -> 8 rows, <= 32 -> 32 rows, <= 128 -> 64 rows, else 128 rows.  When the preferred tile's shared memory exceeds
 // IMB_SMEM_MAX, the next smaller tile that fits runs instead (more CTAs, each as fast); <0 when not even the 8-row tile
 // fits.
-static int rollout_plan(RolloutArgs& A, const DiscLaunch& L, int n_members, int64_t n_sms) {
+static int rollout_plan(RolloutArgs& A, const DiscLaunch& L, int n_members, int64_t n_sms, RolloutDagger* Dg = nullptr) {
   static const int order[4] = {0, 1, 2, 4};
   int i = A.E <= n_sms * 16 ? 0 : A.E <= n_sms * 32 ? 1 : A.E <= n_sms * 128 ? 2 : 3;
   size_t n_img = 0, bytes = 0;
   for (; i >= 0; --i) {
-    bytes = rollout_layout(A, L, n_members, order[i], &n_img);
+    bytes = rollout_layout(A, L, n_members, order[i], &n_img, Dg);
     if (bytes <= IMB_SMEM_MAX) return order[i];
   }
   IMB_REQUIRE(n_members <= 1,
@@ -541,64 +608,77 @@ static int rollout_plan(RolloutArgs& A, const DiscLaunch& L, int n_members, int6
               "the member images), more than the %d B limit of a CTA: use fewer or narrower members", n_members, bytes,
               n_img * 4, (int)IMB_SMEM_MAX);
   IMB_FAIL(-1, "rollout kernel needs %zu B of shared memory at its smallest (8-row) tile (%zu B for the reward-net "
-           "images), more than the %d B limit of a CTA", bytes, n_img * 4, (int)IMB_SMEM_MAX);
+           "images%s), more than the %d B limit of a CTA", bytes, n_img * 4, Dg ? ", with the learner's image" : "",
+           (int)IMB_SMEM_MAX);
 }
 
-template <int RPL, bool ENS, int ACT, bool EXP>
+template <int RPL, bool ENS, int ACT, int MODE, int LACT = ACT>
 static int launch_rollout_t(const RolloutArgs& A, const DiscLaunch& L, const RolloutMembers& Mb,
                             const float* env_params, float* env_obs, const float* pol_params, const float* pol_norm,
                             const float* disc_params, float* rollout, float* ring, float* flat_out, float* aux,
-                            const float* noise, const int64_t* state, const RolloutExplore& Xp, cudaStream_t st) {
+                            const float* noise, const int64_t* state, const RolloutExplore& Xp, const RolloutDagger& Dg,
+                            cudaStream_t st) {
   constexpr int RR = rows_of(RPL);
   const size_t bytes = (size_t)A.total * 4;
   static size_t attr_bytes = 0;
   if (bytes > attr_bytes) {
-    cudaError_t e = cudaFuncSetAttribute(k_rollout<RPL, ENS, ACT, EXP>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)bytes);
+    cudaError_t e = cudaFuncSetAttribute(k_rollout<RPL, ENS, ACT, MODE, LACT>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
     if (e != cudaSuccess) IMB_FAIL(-2, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
     attr_bytes = bytes;
   }
   const int blocks = (int)((A.E + RR - 1) / RR);
-  k_rollout<RPL, ENS, ACT, EXP><<<blocks, RT, bytes, st>>>(A, L, Mb, env_params, env_obs, pol_params, pol_norm,
-                                                           disc_params, rollout, ring, flat_out, aux, noise, state, Xp);
+  k_rollout<RPL, ENS, ACT, MODE, LACT><<<blocks, RT, bytes, st>>>(A, L, Mb, env_params, env_obs, pol_params, pol_norm,
+                                                                  disc_params, rollout, ring, flat_out, aux, noise,
+                                                                  state, Xp, Dg);
   IMB_CHECK_LAUNCH("k_rollout");
   return 0;
 }
 
 // Mb == nullptr: the single-net rollout; act: the policy towers' activation (ACT_TANH / ACT_RELU); Xp == nullptr: every
-// step on the policy (no exploration variant)
+// step on the policy (no exploration variant); Dg != nullptr: the DAgger rollout (no members, no exploration)
 template <int ACT>
 static int launch_rollout_act(RolloutArgs A, const DiscLaunch& L, const RolloutMembers* Mb,
                               const float* env_params, float* env_obs, const float* pol_params, const float* pol_norm,
                               const float* disc_params, float* rollout, float* ring, float* flat_out, float* aux,
-                              const float* noise, const int64_t* state, const RolloutExplore* Xp, cudaStream_t st) {
-  const int rpl = rollout_plan(A, L, Mb ? Mb->M : 1, imb_num_sms());
+                              const float* noise, const int64_t* state, const RolloutExplore* Xp,
+                              const RolloutDagger* Dg_in, cudaStream_t st) {
+  RolloutDagger dg = Dg_in ? *Dg_in : RolloutDagger{};
+  const int rpl = rollout_plan(A, L, Mb ? Mb->M : 1, imb_num_sms(), Dg_in ? &dg : nullptr);
   if (rpl < 0) return rpl;
   static const RolloutMembers no_members = {};
   static const RolloutExplore no_explore = {};
 #define IMB_RL_X(R, X, XP)                                                                                             \
   return Mb ? launch_rollout_t<R, true, ACT, X>(A, L, *Mb, env_params, env_obs, pol_params, pol_norm, disc_params,    \
-                                                rollout, ring, flat_out, aux, noise, state, XP, st)                    \
+                                                rollout, ring, flat_out, aux, noise, state, XP, dg, st)                \
             : launch_rollout_t<R, false, ACT, X>(A, L, no_members, env_params, env_obs, pol_params, pol_norm,          \
-                                                 disc_params, rollout, ring, flat_out, aux, noise, state, XP, st)
-#define IMB_RL(R)                        \
-  do {                                   \
-    if (Xp) IMB_RL_X(R, true, *Xp);      \
-    IMB_RL_X(R, false, no_explore);      \
+                                                 disc_params, rollout, ring, flat_out, aux, noise, state, XP, dg, st)
+#define IMB_RL_D(R, LA)                                                                                                \
+  return launch_rollout_t<R, false, ACT, RM_DAGGER, LA>(A, L, no_members, env_params, env_obs, pol_params, pol_norm,  \
+                                                        nullptr, rollout, nullptr, flat_out, aux, noise, state,       \
+                                                        no_explore, dg, st)
+#define IMB_RL(R)                                   \
+  do {                                              \
+    if (Dg_in && dg.act == ACT_TANH) IMB_RL_D(R, ACT_TANH); \
+    if (Dg_in) IMB_RL_D(R, ACT_RELU);               \
+    if (Xp) IMB_RL_X(R, RM_EXPLORE, *Xp);           \
+    IMB_RL_X(R, RM_PLAIN, no_explore);              \
   } while (0)
   if (rpl == 0) IMB_RL(0);
   if (rpl == 1) IMB_RL(1);
   if (rpl == 2) IMB_RL(2);
   IMB_RL(4);
 #undef IMB_RL
+#undef IMB_RL_D
 #undef IMB_RL_X
 }
 
 static int launch_rollout(const RolloutArgs& A, int act, const DiscLaunch& L, const RolloutMembers* Mb,
                           const float* env_params, float* env_obs, const float* pol_params, const float* pol_norm,
                           const float* disc_params, float* rollout, float* ring, float* flat_out, float* aux,
-                          const float* noise, const int64_t* state, const RolloutExplore* Xp, cudaStream_t st) {
+                          const float* noise, const int64_t* state, const RolloutExplore* Xp, const RolloutDagger* Dg,
+                          cudaStream_t st) {
   auto go = act == ACT_TANH ? launch_rollout_act<ACT_TANH> : launch_rollout_act<ACT_RELU>;
   return go(A, L, Mb, env_params, env_obs, pol_params, pol_norm, disc_params, rollout, ring, flat_out, aux, noise,
-            state, Xp, st);
+            state, Xp, Dg, st);
 }

@@ -11,7 +11,7 @@ reduces to "roll whole episodes (one kernel launch per episode, thread per env) 
 predicate holds after a batch of E completed trajectories", appended in env order exactly as
 `add_steps_and_auto_finish` would, then `rng.shuffle`.
 """
-from typing import Callable, Dict, Mapping, Optional, Sequence
+from typing import Callable, Dict, List, Mapping, Optional, Sequence
 
 import numpy as np
 import torch as th
@@ -62,9 +62,13 @@ def _policy_of(policy):
 
 def generate_trajectories(policy, venv, sample_until: GenTrajTerminationFn, rng: np.random.Generator, *,
                           deterministic_policy: bool = False) -> Sequence[types.TrajectoryWithRew]:
-    """Roll `policy` in the device VecEnv until `sample_until` holds (unbiased, see module doc)."""
+    """Roll `policy` in the device VecEnv until `sample_until` holds (unbiased, see module doc).  With a DAgger
+    `InteractiveTrajectoryCollector` as `venv`, `policy` is the expert it collects demonstrations from."""
+    from ..algorithms import dagger
     from ..envs import synth
 
+    if isinstance(venv, dagger.InteractiveTrajectoryCollector):
+        return venv.generate_trajectories(policy, sample_until, rng, deterministic_policy=deterministic_policy)
     base = venv
     while not isinstance(base, synth.DeviceVecEnv):
         if not hasattr(base, "venv"):
@@ -73,7 +77,6 @@ def generate_trajectories(policy, venv, sample_until: GenTrajTerminationFn, rng:
     pol = _policy_of(policy)
     pp, pn, _ = pol.flat_vectors()
     E, H, Do = base.num_envs, base.horizon, base.d_obs
-    da = 1 if pol.discrete else pol.d_act
     rw = _lib.rollout_row_width(pol.desc)
     hp = _lib.PpoHparams(gamma=0.99, gae_lambda=0.95, clip_range=0.2, ent_coef=0.0, vf_coef=0.5, max_grad_norm=0.5,
                          lr=0.0, adam_eps=1e-5, n_epochs=1, batch_size=1, normalize_advantage=0)
@@ -89,21 +92,33 @@ def generate_trajectories(policy, venv, sample_until: GenTrajTerminationFn, rng:
                      act=pol.act)
         _lib.rollout_advance(base.state, E, H, H, 0)
         base.host_ep_step = 0
-        rows = tbl.cpu().numpy().reshape(E, H, rw)
-        term = flat.view(E, H, tw)[:, -1, Do + base.d_act:2 * Do + base.d_act].cpu().numpy()  # terminal observations
-        rews = aux[2 * E + E * H:2 * E + 2 * E * H].cpu().numpy().reshape(E, H)
-        for e in range(E):
-            obs = np.concatenate([rows[e, :, :Do], term[e:e + 1]]).astype(base.observation_space.dtype)
-            if pol.discrete:
-                acts = rows[e, :, Do].astype(base.action_space.dtype)
-            else:  # the env (and the recorded trajectory) sees the clipped action (SURVEY Appendix A.7)
-                acts = np.clip(rows[e, :, Do:Do + da], base.action_space.low, base.action_space.high)
-            trajectories.append(types.TrajectoryWithRew(obs=obs, acts=acts, infos=None, terminal=True,
-                                                        rews=rews[e].astype(np.float32)))
+        trajectories += batch_trajectories(base, tbl, flat, aux)
         if sample_until(trajectories):
             break
     rng.shuffle(trajectories)
     return trajectories
+
+
+def batch_trajectories(base, tbl, flat, aux) -> List[types.TrajectoryWithRew]:
+    """The E whole episodes of one rollout launch from episode step 0 over the env's horizon H, in env order: rollout
+    rows `tbl` ([E * H][rw], obs | act first), flattened rows `flat` (for the terminal observations) and `aux` (for the
+    env rewards)."""
+    E, H, Do, Da = base.num_envs, base.horizon, base.d_obs, base.d_act
+    da = 1 if base.discrete else Da
+    tw = 2 * Do + Da + 1
+    rows = tbl.cpu().numpy().reshape(E, H, -1)
+    term = flat.view(E, H, tw)[:, -1, Do + Da:2 * Do + Da].cpu().numpy()  # terminal observations
+    rews = aux[2 * E + E * H:2 * E + 2 * E * H].cpu().numpy().reshape(E, H)
+    out = []
+    for e in range(E):
+        obs = np.concatenate([rows[e, :, :Do], term[e:e + 1]]).astype(base.observation_space.dtype)
+        if base.discrete:
+            acts = rows[e, :, Do].astype(base.action_space.dtype)
+        else:  # the env (and the recorded trajectory) sees the clipped action (SURVEY Appendix A.7)
+            acts = np.clip(rows[e, :, Do:Do + da], base.action_space.low, base.action_space.high)
+        out.append(types.TrajectoryWithRew(obs=obs, acts=acts, infos=None, terminal=True,
+                                           rews=rews[e].astype(np.float32)))
+    return out
 
 
 def rollout_stats(trajectories: Sequence[types.TrajectoryWithRew]) -> Mapping[str, float]:

@@ -533,6 +533,30 @@ int imb_rollout_explore(const imb_env_desc* env, const float* env_params, float*
                         const float* noise, int flags, const uint8_t* explore_policy, uint64_t explore_seed,
                         int64_t explore_step0, const int64_t* state, void* stream);
 
+/* ---- DAgger rollouts (algorithms/dagger.py) ---------------------------------------------------------------------------
+ * InteractiveTrajectoryCollector under generate_trajectories(expert, deterministic_policy=True) (algorithms/dagger.py:
+ * 232-287): the expert acts, and where robot_mask[t * n_envs + e] (uint8 [n_steps][n_envs]) is 1 env e executes the
+ * learner's action instead (policy.predict: sampled, clipped to the Box).  The mask does not depend on observations,
+ * so the host draws it beforehand.
+ * = imb_rollout with the expert as the policy (flags: IMB_RF_DETERMINISTIC for its mean / argmax) and reward_mode 0,
+ * without a ring, except: no value tower or bootstrap runs; each rollout row holds obs | label, the label being the
+ * expert's action clipped to the Box (Discrete: its index), the other columns of the row undefined; aux's V(last obs)
+ * and bootstrap entries are 0.  The learner (its own width, activation learner_act and feature RunningNorm) runs only
+ * at steps where a row of a tile has its mask bit set; its Box normals / Discrete uniforms come from Philox stream
+ * IMB_STREAM_DAGGER keyed by env->seed at counter (env id, global step + t, a / 4), or, with robot_noise != NULL, from
+ * robot_noise laid out as noise.  The env step, env-reward column of aux, terminal handling and flattened rows are
+ * imb_rollout's. */
+int imb_rollout_dagger(const imb_env_desc* env, const float* env_params, float* env_obs,
+                       const imb_policy_desc* expert, int32_t expert_act, const float* expert_params,
+                       const float* expert_norm, const imb_policy_desc* learner, int32_t learner_act,
+                       const float* learner_params, const float* learner_norm, int64_t n_envs, int64_t n_steps,
+                       float* rollout, float* flat_out, float* aux, const float* noise, const float* robot_noise,
+                       int flags, const uint8_t* robot_mask, const int64_t* state, void* stream);
+/* Rows per CTA (8, 32, 64 or 128) imb_rollout_dagger runs for these policies over n_envs envs on n_sms SMs (<= 0: the
+ * current device's), chosen as imb_rollout_plan chooses with both policy images resident; host only. */
+int imb_rollout_dagger_plan(const imb_policy_desc* expert, const imb_policy_desc* learner, int64_t n_envs,
+                            int32_t n_sms);
+
 /* ---- density-based reward (algorithms/density.py) ----------------------------------------------------------------------
  * DensityAlgorithm.__call__ (:295-360), which calls sklearn KernelDensity.score once per transition:
  *   r = log( (1/N_s) sum_i K_h(x - x_i) ),  x = (features - mean) / scale,
