@@ -108,6 +108,9 @@ KDE_GAUSSIAN, KDE_TOPHAT, KDE_EPANECHNIKOV, KDE_EXPONENTIAL, KDE_LINEAR, KDE_COS
 KDE_KERNELS = {"gaussian": KDE_GAUSSIAN, "tophat": KDE_TOPHAT, "epanechnikov": KDE_EPANECHNIKOV,
                "exponential": KDE_EXPONENTIAL, "linear": KDE_LINEAR, "cosine": KDE_COSINE}
 DENSITY_SEG_NONE, DENSITY_SEG_STEPS, DENSITY_SEG_ROLLOUT = 0, 1, 2
+# imb_mce_sweep: flags and the shape envelope
+MCE_BACKWARD, MCE_FORWARD = 1, 2
+MCE_MAX_STATES, MCE_MAX_ACTIONS, MCE_MAX_HORIZON = 4096, 32, 1000000
 
 _disc, _adam, _pol, _env, _hp, _pu, _members, _sync = map(C.POINTER, (
     DiscDesc, Adam, PolicyDesc, EnvDesc, PpoHparams, PrefUncDesc, RolloutMembers, SyncDesc))
@@ -170,6 +173,9 @@ SIGNATURES = {
     "imb_density_ws_floats": (_i64, [_i64], 0),
     "imb_density_score": (_i32, [_i32, _i32, _i32, _i32, _i32, _i32, _f32, _i32, _i64, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr,
                                  _ptr, _i32, _ptr, _i64, _i32, _ptr, _ptr, _i64, _i64, _i32, _ptr, _i64, _ptr, _ptr], None),
+    "imb_mce_plan": (_i64, [_i64, _i32, _i32, _i32, _i32, _ptr], 0),
+    "imb_mce_sweep": (_i32, [_i64, _i32, _i32, _i32, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr,
+                             _ptr, _ptr, _i64, _ptr], 1),
     "imb_sync_buffer_doubles": (_i64, [_sync], 0),
     "imb_sync_snapshot": (_i32, [_sync, _ptr, _ptr], None),
     "imb_sync_pack": (_i32, [_sync, _ptr, _ptr], 1),
@@ -532,6 +538,28 @@ def density_score(model, src, src_ld, n_query, out, out_stride, ws, seg_mode=DEN
                                    _p(steps, th.int64), _p(state, th.int64), n_envs, n_steps, horizon,
                                    _p(out, th.float32), out_stride, _p(ws, th.float32),
                                    _stream()), "imb_density_score", 1 if n_query > 0 else 0)
+
+
+def mce_plan(n_states: int, n_actions: int, horizon: int, flags: int, n_sms: int = 0):
+    """(workspace doubles, CTA count) of `mce_sweep` for this shape (host only; n_sms <= 0: the current device's SMs and
+    the kernel's occupancy, which is what `mce_sweep` launches).  NotImplementedError naming the limit when the shape is
+    outside the kernel's envelope."""
+    grid = C.c_int32(0)
+    rc = lib().imb_mce_plan(n_states, n_actions, horizon, flags, n_sms, C.addressof(grid))
+    if rc < 0:
+        raise NotImplementedError(f"imb_mce_plan: {lib().imb_last_error().decode()} (rc={rc})")
+    return rc, grid.value
+
+
+def mce_sweep(n_states, n_actions, horizon, flags, T, initial, reward, reward32, discounts, ws, V=None, Q=None, pi=None,
+              D=None, Dcum=None, demo_om=None, weights=None, linf=None):
+    """The MCE IRL time sweep (imb_mce_sweep): float64 CUDA tensors except reward32 / weights (float32); `discounts`
+    float64 [2] = (planning discount, occupancy discount); ws: float64 [mce_plan(...)[0]]."""
+    f64 = th.float64
+    _check(lib().imb_mce_sweep(n_states, n_actions, horizon, flags, _p(T, f64), _p(initial, f64), _p(reward, f64),
+                               _p(reward32, th.float32), _p(discounts, f64), _p(V, f64), _p(Q, f64), _p(pi, f64),
+                               _p(D, f64), _p(Dcum, f64), _p(demo_om, f64), _p(weights, th.float32), _p(linf, f64),
+                               _p(ws, f64), ws.numel(), _stream()), "imb_mce_sweep")
 
 
 def gae(rollout_tbl, rw, col_value, n_envs, n_steps, aux, gamma, gae_lambda, state, horizon):

@@ -610,6 +610,36 @@ int imb_density_score(int32_t d, int32_t col0, int32_t n0, int32_t col1, int32_t
                       const int64_t* row_map, int64_t n_query, int32_t seg_mode, const int64_t* steps, const int64_t* state, int64_t n_envs,
                       int64_t n_steps, int32_t horizon, float* out, int64_t out_stride, float* ws, void* stream);
 
+/* ---- tabular MCE IRL (algorithms/mce_irl.py) ----------------------------------------------------------------------------
+ * The time sweep of one finite-horizon MDP with S states, A actions and horizon H in ONE cooperative launch, float64
+ * throughout, as the reference's NumPy computes it:
+ *  IMB_MCE_BACKWARD  mce_partition_fh (:38-93): Q[H-1] = r, Q[t] = r + gamma_plan * (T @ V[t+1]) for t < H - 1,
+ *                    V[t] = scipy.special.logsumexp(Q[t], axis=1), pi = exp(Q - V).  reward: exactly one of `reward`
+ *                    (float64) and `reward32` (float32, widened: the reward net's output).
+ *  IMB_MCE_FORWARD   mce_occupancy_measures (:96-144): D[0] = initial, D[t+1] = sum_a (D[t] pi[t, :, a]) @ T[:, a, :],
+ *                    Dcum = rollout.discounted_sum(D, gamma_om) (polyval's Horner from t = H; a plain sum at 1).  With
+ *                    BACKWARD too, pi is the one the backward sweep computed; alone, it reads the caller's pi.
+ * transition: T as [S][A][S] (row (s, a) = the next-state distribution); discounts[2] = {gamma_plan, gamma_om} (device).
+ * Outputs, each optional unless stated: V [H][S], Q [H][S][A], pi [H][S][A] (an input without BACKWARD), D [H+1][S],
+ * Dcum [S] (required with FORWARD).  demo_om != NULL (FORWARD; MCEIRL._train_step): weights[s] = (float)(Dcum[s] -
+ * demo_om[s]) rounded to nearest, *linf = max_s |Dcum[s] - demo_om[s]| (NaN propagates).  Every sum has a fixed order
+ * and no floating-point atomics: two calls give the same bits.  ws: imb_mce_plan(...) doubles.
+ * imb_mce_plan is host only: the workspace in doubles (and, when grid_out != NULL, a HOST int32 pointer, the CTA count of
+ * the launch), or < 0 with imb_last_error() naming the limit when the shape is outside the envelope
+ * (1 <= S <= IMB_MCE_MAX_STATES, 1 <= A <= IMB_MCE_MAX_ACTIONS, 1 <= H <= IMB_MCE_MAX_HORIZON).  n_sms <= 0: the
+ * current device's SMs and the kernel's occupancy (what imb_mce_sweep launches); > 0: one CTA per SM, no GPU needed. */
+#define IMB_MCE_BACKWARD 1
+#define IMB_MCE_FORWARD 2
+#define IMB_MCE_MAX_STATES 4096
+#define IMB_MCE_MAX_ACTIONS 32
+#define IMB_MCE_MAX_HORIZON 1000000
+int64_t imb_mce_plan(int64_t n_states, int32_t n_actions, int32_t horizon, int32_t flags, int32_t n_sms,
+                     int32_t* grid_out);
+int imb_mce_sweep(int64_t n_states, int32_t n_actions, int32_t horizon, int32_t flags, const double* transition,
+                  const double* initial, const double* reward, const float* reward32, const double* discounts,
+                  double* V, double* Q, double* pi, double* D, double* Dcum, const double* demo_om, float* weights,
+                  double* linf, double* ws, int64_t ws_doubles, void* stream);
+
 /* ---- multi-GPU: replica state around the ONE all-reduce of a round ---------------------------
  * (SURVEY.md section 8e; the reference is single-process, so there is no reference interface to
  * cite: the merge restates RunningNorm's Chan update, util/networks.py:96-134, in its additive
