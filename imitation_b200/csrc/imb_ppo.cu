@@ -163,6 +163,20 @@ __device__ __forceinline__ void load8(float (&d)[8], const float* __restrict__ p
 __device__ __forceinline__ float sum8(const float (&d)[8]) {
   return ((d[0] + d[1]) + (d[2] + d[3])) + ((d[4] + d[5]) + (d[6] + d[7]));
 }
+// d[i] = p[i * stride], i < N: N independent loads into a register array (compile-time indices only)
+template <int N>
+__device__ __forceinline__ void load_strided(float (&d)[N], const float* __restrict__ p, const int stride) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) d[i] = p[i * stride];
+}
+// An empty asm that reads and writes every d[i]: the loads of d are issued before this point, and the compiler can neither
+// sink them next to their uses nor load again there (with shared-memory offsets that are compile-time constants it can
+// prove them independent of the stores in between, and did sink them without this)
+template <int N>
+__device__ __forceinline__ void pin_regs(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i]));
+}
 
 // ---- training statistics of PPO.train (imb_ppo_update_ex: stats_out, target_kl) -----------------------------------
 // Both kernels keep them in shared memory, out of the chain warps' registers.  Per step, the lanes that own a row's loss
@@ -770,6 +784,17 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
       const float* cW1 = Pm + (cnet ? PL.w1[1] : PL.w1[0]);
       const float* cW2 = Pm + (cnet ? PL.w2[1] : PL.w2[0]);
       const int c_b1 = cnet ? PL.b1[1] : PL.b1[0], c_b2 = cnet ? PL.b2[1] : PL.b2[0];
+      // WREG: the lane's W2 row (forward, lane = output unit) and W2 column (backward, lane = input unit) come from
+      // registers, each loaded as one block of 32 independent loads a phase before the loop that uses it (the row in
+      // layer 1, the column in layer 2; pin_regs holds each block there), so those two loops issue only their activation
+      // loads instead of a weight load beside every 16-byte activation load.  The FMAs and their order are unchanged;
+      // only where a weight is read from moves (nothing writes Pm between the step's top barrier and the end of the
+      // chain).  Only the shape-specialised Box instantiations: with runtime bounds the arrays would go to local memory,
+      // and the Discrete one spills with them.  W1 and the action head's weights stay in shared memory: with them in
+      // registers too the 17/6 instantiation spills.
+      constexpr bool WREG = SPEC && !DISC;
+      float w2r[WREG ? HP : 1], w2c[WREG ? HP : 1];
+      if constexpr (WREG) load_strided(w2r, cW2 + jc * ldh, 1);
       // policy warps: everything the loss needs that does not depend on the forward pass is fetched now, so its
       // latency (shared-memory loads, the exponential) hides behind the layers
       const bool gfast = cnet == 0 && !discrete && Da <= 8;  // one action per lane of the octet
@@ -797,19 +822,21 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
           a3 = fmaf(x.w, w, a3);
         }
       }
+      if constexpr (WREG) pin_regs(w2r);  // (loaded during layer 1)
       float b = Pm[c_b1 + jc];
       const float h10 = jl ? PPO_TANH(a0 + b) : 0.f, h11 = jl ? PPO_TANH(a1 + b) : 0.f;
       const float h12 = jl ? PPO_TANH(a2 + b) : 0.f, h13 = jl ? PPO_TANH(a3 + b) : 0.f;
       st4(cH1 + j * RL + r0, make_float4(h10, h11, h12, h13));
       __syncwarp();
       PPO_WCLK(3);
+      if constexpr (WREG) load_strided(w2c, cW2 + jc, ldh);
       // layer 2
       a0 = a1 = a2 = a3 = 0.f;
       {
         const float* wp = cW2 + jc * ldh;
 #pragma unroll U_H
         for (int i = 0; i < h; ++i) {
-          const float w = wp[i];
+          const float w = WREG ? w2r[i] : wp[i];
           const float4 x = ld4(cH1 + i * RL + r0);
           a0 = fmaf(x.x, w, a0);
           a1 = fmaf(x.y, w, a1);
@@ -817,6 +844,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
           a3 = fmaf(x.w, w, a3);
         }
       }
+      if constexpr (WREG) pin_regs(w2c);  // (loaded during layer 2)
       b = Pm[c_b2 + jc];
       const float lat0 = jl ? PPO_TANH(a0 + b) : 0.f, lat1 = jl ? PPO_TANH(a1 + b) : 0.f;
       const float lat2 = jl ? PPO_TANH(a2 + b) : 0.f, lat3 = jl ? PPO_TANH(a3 + b) : 0.f;
@@ -1004,7 +1032,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
         const float* wp = cW2 + jc;
 #pragma unroll U_H
         for (int jj = 0; jj < h; ++jj) {
-          const float w = wp[jj * ldh];
+          const float w = WREG ? w2c[jj] : wp[jj * ldh];
           const float4 d = ld4(cDZ2 + jj * RL + r0);
           a0 = fmaf(d.x, w, a0);
           a1 = fmaf(d.y, w, a1);
