@@ -19,6 +19,7 @@ IMB_F_ZERO_GRAD = 1
 IMB_F_TRAIN_NORM = 2
 IMB_F_NO_TENSOR = 4   # force the fp32-FFMA discriminator kernel (A/B measurements)
 IMB_RF_DETERMINISTIC = 1  # imb_rollout flags
+ENV_SYNTH, ENV_CARTPOLE, ENV_PENDULUM = 0, 1, 2  # EnvDesc.kind: the env the rollout kernels step
 ACT_TANH, ACT_RELU = 0, 1  # pol_act: the policy towers' activation (imb_rollout, imb_ppo_update, imb_policy_logp, ...)
 
 # device-resident counter block (include/imb.h enum)
@@ -63,7 +64,7 @@ class PolicyDesc(C.Structure):
 
 class EnvDesc(C.Structure):
     _fields_ = [("d_obs", _i32), ("d_act", _i32), ("discrete", _i32), ("horizon", _i32), ("seed", _u64),
-                ("env_id_offset", _i64)]
+                ("env_id_offset", _i32), ("kind", _i32)]
 
 
 class PpoHparams(C.Structure):

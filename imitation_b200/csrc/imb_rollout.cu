@@ -16,6 +16,27 @@ static int check_shapes(const imb_policy_desc* pol, const imb_disc_desc* disc) {
   return 0;
 }
 
+// the env kind against the shapes it steps (include/imb.h IMB_ENV_*)
+static int check_env(const imb_env_desc* env) {
+  IMB_REQUIRE(env != nullptr, "no env descriptor");
+  switch (env->kind) {
+    case IMB_ENV_SYNTH:
+      return 0;
+    case IMB_ENV_CARTPOLE:
+      IMB_REQUIRE(env->d_obs == 4 && env->d_act == 2 && env->discrete == 1,
+                  "seals/CartPole-v0 (kind %d) takes d_obs 4, d_act 2, discrete 1; got %d, %d, %d", env->kind,
+                  env->d_obs, env->d_act, env->discrete);
+      return 0;
+    case IMB_ENV_PENDULUM:
+      IMB_REQUIRE(env->d_obs == 3 && env->d_act == 1 && env->discrete == 0,
+                  "Pendulum-v1 (kind %d) takes d_obs 3, d_act 1, discrete 0; got %d, %d, %d", env->kind, env->d_obs,
+                  env->d_act, env->discrete);
+      return 0;
+    default:
+      IMB_FAIL(-1, "unknown env kind %d (IMB_ENV_SYNTH, IMB_ENV_CARTPOLE or IMB_ENV_PENDULUM)", env->kind);
+  }
+}
+
 extern "C" int imb_rollout_plan(const imb_policy_desc* pol, const imb_disc_desc* disc, int32_t n_members,
                                 int64_t n_envs, int32_t n_sms) {
   IMB_REQUIRE(pol && n_envs >= 1, "rollout plan needs a policy and n_envs >= 1");
@@ -45,6 +66,7 @@ static int rollout_common(const imb_env_desc* env, const float* env_params, floa
                           float* ring, int64_t ring_capacity, float* flat_out, float* aux, const float* noise, int flags,
                           const int64_t* state, const RolloutExplore* Xp, const RolloutDagger* Dg, void* stream) {
   IMB_REQUIRE(n_envs >= 1 && n_steps >= 1, "rollout needs n_envs, n_steps >= 1");
+  if (int rc = check_env(env)) return rc;
   IMB_REQUIRE(env->d_obs == pol->d_obs && env->d_act == pol->d_act && env->discrete == pol->discrete,
               "env / policy space mismatch");
   IMB_REQUIRE(pol_act == IMB_ACT_TANH || pol_act == IMB_ACT_RELU,
@@ -209,8 +231,9 @@ extern "C" int imb_gae(float* rollout, int32_t rw, int32_t col_value, int64_t n_
 
 extern "C" int imb_env_reset(float* env_obs, int64_t n_envs, const imb_env_desc* env, const int64_t* state,
                              void* stream) {
-  k_env_reset<<<(int)((n_envs + 127) / 128), 128, 0, (cudaStream_t)stream>>>(env_obs, n_envs, env->d_obs, env->seed,
-                                                                            env->env_id_offset, state);
+  if (int rc = check_env(env)) return rc;
+  k_env_reset<<<(int)((n_envs + 127) / 128), 128, 0, (cudaStream_t)stream>>>(env_obs, n_envs, env->d_obs, env->kind,
+                                                                            env->seed, env->env_id_offset, state);
   IMB_CHECK_LAUNCH("k_env_reset");
   return 0;
 }

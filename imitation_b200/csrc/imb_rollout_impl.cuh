@@ -6,8 +6,9 @@
 // dynamics all resident in shared memory for the whole rollout:
 //   policy forward + sampling      SB3 OnPolicyAlgorithm.collect_rollouts (restated; see
 //                                  oracle/ppo_port.py -- parity unpinned by the reference)
-//   env step + auto-reset          synthetic MuJoCo-shaped env (SURVEY.md section 8d); VecEnv
-//                                  contract of data/rollout.py:161-186
+//   env step + auto-reset          synthetic MuJoCo-shaped env (SURVEY.md section 8d), or seals/CartPole-v0 /
+//                                  Pendulum-v1 stepped thread per env in float64 (DESIGN.md section 7e);
+//                                  VecEnv contract of data/rollout.py:161-186
 //   reward relabel                 rewards/reward_wrapper.py:92-133 -> RewardNet.predict_processed
 //                                  (reward_nets.py:120-204), GAIL transform gail.py:83
 //   trajectory bookkeeping         data/wrappers.py:69-148 + data/rollout.py:563-621: the flattened
@@ -82,17 +83,93 @@ struct RolloutDagger {
 
 enum { RM_PLAIN = 0, RM_EXPLORE = 1, RM_DAGGER = 2 };
 
+// ---- classic-control envs (imb_env_desc.kind; DESIGN.md section 7e) ---------------------------------------------------
+// The observation is the env's whole state, so the SoA [d_obs][E] obs buffer is the only state array.  One thread steps
+// one env: it reads the float32 observation obs[k * stride], computes in float64 as gymnasium does and writes the next
+// observation nobs[k * stride] in float32; returns the env reward.
+
+// the Box bound of the env's actions: Pendulum-v1's torque is in [-2, 2], the synthetic env's Box is [-1, 1] (and the
+// Discrete envs have no Box)
+__device__ __forceinline__ float env_act_bound(int kind) { return kind == IMB_ENV_PENDULUM ? 2.0f : 1.0f; }
+
+// seals/CartPole-v0 (gymnasium CartPole, Euler integrator; seals' FixedHorizonCartPole reward, never terminates).
+// ctl: the one-hot control, action 1 pushes the cart in +x.
+__device__ __forceinline__ float cartpole_step(const float* __restrict__ obs, const float* __restrict__ ctl,
+                                               float* __restrict__ nobs, int stride) {
+  constexpr double g = 9.8, masspole = 0.1, total_mass = 1.0 + 0.1, length = 0.5, polemass_length = 0.1 * 0.5;
+  constexpr double force_mag = 10.0, tau = 0.02, x_threshold = 2.4, theta_threshold = 12.0 * 2.0 * M_PI / 360.0;
+  const double x = obs[0], x_dot = obs[stride], theta = obs[2 * stride], theta_dot = obs[3 * stride];
+  const double force = ctl[stride] > 0.5f ? force_mag : -force_mag;
+  double sintheta, costheta;
+  sincos(theta, &sintheta, &costheta);
+  const double temp = (force + polemass_length * (theta_dot * theta_dot) * sintheta) / total_mass;
+  const double thetaacc =
+      (g * sintheta - costheta * temp) / (length * (4.0 / 3.0 - masspole * (costheta * costheta) / total_mass));
+  const double xacc = temp - polemass_length * thetaacc * costheta / total_mass;
+  const double nx = x + tau * x_dot, nx_dot = x_dot + tau * xacc;
+  const double ntheta = theta + tau * theta_dot, ntheta_dot = theta_dot + tau * thetaacc;
+  nobs[0] = (float)nx;
+  nobs[stride] = (float)nx_dot;
+  nobs[2 * stride] = (float)ntheta;
+  nobs[3 * stride] = (float)ntheta_dot;
+  const bool inside = fabs(nx) <= x_threshold && fabs(ntheta) <= theta_threshold;
+  return inside ? 1.0f : 0.0f;
+}
+
+// Pendulum-v1 (g = 10, m = l = 1, dt = 0.05, |thdot| <= 8, |u| <= 2; reward on the pre-step state).  The angle comes
+// back as atan2(sin, cos) in [-pi, pi]: the dynamics see only sin(theta) and theta mod 2 pi, and angle_normalize of an
+// angle in [-pi, pi] squares to its own square.  ctl: the control, already clipped to [-2, 2].
+__device__ __forceinline__ float pendulum_step(const float* __restrict__ obs, const float* __restrict__ ctl,
+                                               float* __restrict__ nobs, int stride) {
+  constexpr double g = 10.0, dt = 0.05, max_speed = 8.0, max_torque = 2.0;
+  const double th = atan2((double)obs[stride], (double)obs[0]), thdot = obs[2 * stride];
+  const double u = fmin(fmax((double)ctl[0], -max_torque), max_torque);
+  const double costs = th * th + 0.1 * (thdot * thdot) + 0.001 * (u * u);
+  const double newthdot = fmin(fmax(thdot + (3.0 * g / 2.0 * sin(th) + 3.0 * u) * dt, -max_speed), max_speed);
+  const double newth = th + newthdot * dt;
+  double s, c;
+  sincos(newth, &s, &c);
+  nobs[0] = (float)c;
+  nobs[stride] = (float)s;
+  nobs[2 * stride] = (float)newthdot;
+  return (float)(-costs);
+}
+
+// The reset observation of a classic env from the four uniforms of Philox stream IMB_STREAM_ENV_RESET keyed by `seed`
+// at counter (env id, episode): CartPole x, x_dot, theta, theta_dot ~ U(-0.05, 0.05); Pendulum theta ~ U(-pi, pi),
+// theta_dot ~ U(-1, 1), observed as (cos theta, sin theta, theta_dot).  (The same distributions as gymnasium's resets,
+// not its PCG64 bits.)
+__device__ __forceinline__ void classic_reset(int kind, uint64_t seed, uint32_t egid, uint32_t episode,
+                                              float* __restrict__ obs, int64_t stride) {
+  uint32_t k0, k1;
+  philox_key(seed, IMB_STREAM_ENV_RESET, k0, k1);
+  const Philox4 r = philox4x32(egid, episode, 0u, 0u, k0, k1);
+  const uint32_t w[4] = {r.x, r.y, r.z, r.w};
+  if (kind == IMB_ENV_CARTPOLE) {
+    for (int k = 0; k < 4; ++k) obs[k * stride] = (float)(-0.05 + 0.1 * (double)u01(w[k]));
+  } else {
+    const double th = -M_PI + 2.0 * M_PI * (double)u01(w[0]), thdot = -1.0 + 2.0 * (double)u01(w[1]);
+    double s, c;
+    sincos(th, &s, &c);
+    obs[0] = (float)c;
+    obs[stride] = (float)s;
+    obs[2 * stride] = (float)thdot;
+  }
+}
+
 // The action head of one policy for this thread's tile row (thread per env), on the pi latent H2: Box -> mean + std * z,
 // z = 0 (deterministic), the pinned noise[nidx * Da + a] or a normal of Philox stream `stream` at counter (egid, ctr,
 // a / 4); Discrete -> inverse-CDF sampling with the uniform noise[nidx] or one of that stream (argmax when
-// deterministic).  CTRL[a * RRS] receives the control the env sees (the clipped action / the one-hot; Discrete uses it
-// for the logits first); rec (nullable) the recorded action: Box unclipped unless clip_rec, Discrete the index.
+// deterministic).  CTRL[a * RRS] receives the control the env sees (the action clipped to the Box [-ahi, ahi] / the
+// one-hot; Discrete uses it for the logits first); rec (nullable) the recorded action: Box unclipped unless clip_rec,
+// Discrete the index.
 // Returns log pi(action).
 __device__ __forceinline__ float action_head(const float* __restrict__ psm, const PolImg& S, int HP, int h, int Da,
                                              bool discrete, const float* __restrict__ H2, int RRS, int rt,
                                              float* __restrict__ CTRL, float* __restrict__ rec, bool clip_rec,
                                              bool deterministic, const float* __restrict__ noise, int64_t nidx,
-                                             bool live, uint64_t seed, uint32_t stream, uint32_t egid, uint32_t ctr) {
+                                             bool live, uint64_t seed, uint32_t stream, uint32_t egid, uint32_t ctr,
+                                             float ahi) {
   float logp = 0.f;
   if (!discrete) {
     float z4[4] = {0.f, 0.f, 0.f, 0.f};
@@ -113,7 +190,7 @@ __device__ __forceinline__ float action_head(const float* __restrict__ psm, cons
       const float act = fmaf(sd, z, m);
       const float diff = act - m;
       logp += -(diff * diff) / (2.0f * sd * sd) - ls - 0.9189385332046727f;
-      const float ctl = fminf(fmaxf(act, -1.0f), 1.0f);
+      const float ctl = fminf(fmaxf(act, -ahi), ahi);
       if (rec) rec[a] = clip_rec ? ctl : act;  // SB3 stores the UNCLIPPED action; predict() returns the clipped one
       CTRL[a * RRS] = ctl;                     // env and wrappers see the clipped one
     }
@@ -204,9 +281,11 @@ __global__ void __launch_bounds__(RT, 1) k_rollout(const RolloutArgs A, const Di
   const PolImg LS(Do, Da, DAG ? Dg.HP : HP);
   float* lsm = smem + (DAG ? Dg.img_off : A.pol_off);
   if (DAG) load_policy_img(lsm, LS, Dg.pol, Dg.HP, Dg.params, Dg.norm);
-  for (int i = tid; i < (KU + 2) * IP; i += RT) esm[i] = 0.f;
-  __syncthreads();
-  {
+  const int kind = A.env.kind;  // block-uniform: the env step branches on it
+  const float ahi = env_act_bound(kind);
+  if (kind == IMB_ENV_SYNTH) {  // the classic-control envs have no matrices (and no env_params)
+    for (int i = tid; i < (KU + 2) * IP; i += RT) esm[i] = 0.f;
+    __syncthreads();
     const float* eA = env_params;
     const float* eB = eA + Do * Do;
     const float* eC = eB + Do * Da;
@@ -322,7 +401,7 @@ __global__ void __launch_bounds__(RT, 1) k_rollout(const RolloutArgs A, const Di
       philox_key(Xp.seed, IMB_STREAM_EXPLORE, k0, k1);
       const uint32_t ctr = (uint32_t)(Xp.step0 + t);
       if (!A.pol.discrete) {
-        constexpr float lo = -1.0f, hi = 1.0f;  // the synthetic env's Box
+        const float lo = -ahi, hi = ahi;  // the env's Box
         Philox4 r = {0u, 0u, 0u, 0u};
         for (int a = 0; a < Da; ++a) {
           if (!noise && (a & 3) == 0) r = philox4x32(egid, ctr, (uint32_t)(a >> 2), 0u, k0, k1);
@@ -341,7 +420,7 @@ __global__ void __launch_bounds__(RT, 1) k_rollout(const RolloutArgs A, const Di
     } else {
       logp = action_head(psm, S, HP, h, Da, A.pol.discrete, H2, RRS, rt, OBSU + Do * RRS + tid, live ? row + Do : nullptr,
                          DAG, A.deterministic, noise, t * E + e, live, A.env.seed, IMB_STREAM_ACT_NOISE, egid,
-                         (uint32_t)(gstep0 + t));
+                         (uint32_t)(gstep0 + t), ahi);
     }
     if (DAG) {
       // ---- the learner acts where the mask says so; its tower runs only when some row of the tile needs it --------
@@ -355,7 +434,7 @@ __global__ void __launch_bounds__(RT, 1) k_rollout(const RolloutArgs A, const Di
         __syncthreads();
         if (robot)
           action_head(lsm, LS, LHP, lh, Da, Dg.pol.discrete, H2, RRS, rt, OBSU + Do * RRS + tid, nullptr, false, false,
-                      Dg.noise, t * E + e, live, A.env.seed, IMB_STREAM_DAGGER, egid, (uint32_t)(gstep0 + t));
+                      Dg.noise, t * E + e, live, A.env.seed, IMB_STREAM_DAGGER, egid, (uint32_t)(gstep0 + t), ahi);
       }
     }
     if (live) {
@@ -367,18 +446,25 @@ __global__ void __launch_bounds__(RT, 1) k_rollout(const RolloutArgs A, const Di
     }
     __syncthreads();
 
-    // ---- environment step: NOBS = tanh([obs | u] . [A | B]^T + c) --------------------------------------------------
-    tile_layer<ACT_TANH, RPL>(OBSU, KU, esm, IP, ecv, NOBS, IP);
-    __syncthreads();
+    // ---- environment step -------------------------------------------------------------------------------------------
     float rew_env = 0.f;
-    for (int i = 0; i < Do; ++i) rew_env = fmaf(ewv[i], NOBS[i * RRS + rt], rew_env);
-    if (!A.env.discrete) {
-      float pen = 0.f;
-      for (int a = 0; a < Da; ++a) {
-        const float uu = OBSU[(Do + a) * RRS + rt];
-        pen = fmaf(uu, uu, pen);
+    if (kind == IMB_ENV_SYNTH) {  // NOBS = tanh([obs | u] . [A | B]^T + c)
+      tile_layer<ACT_TANH, RPL>(OBSU, KU, esm, IP, ecv, NOBS, IP);
+      __syncthreads();
+      for (int i = 0; i < Do; ++i) rew_env = fmaf(ewv[i], NOBS[i * RRS + rt], rew_env);
+      if (!A.env.discrete) {
+        float pen = 0.f;
+        for (int a = 0; a < Da; ++a) {
+          const float uu = OBSU[(Do + a) * RRS + rt];
+          pen = fmaf(uu, uu, pen);
+        }
+        rew_env -= 0.1f * pen;
       }
-      rew_env -= 0.1f * pen;
+    } else {  // classic control: thread per env, float64
+      if (rowthread)
+        rew_env = kind == IMB_ENV_CARTPOLE ? cartpole_step(OBSU + tid, OBSU + Do * RRS + tid, NOBS + tid, RRS)
+                                           : pendulum_step(OBSU + tid, OBSU + Do * RRS + tid, NOBS + tid, RRS);
+      __syncthreads();
     }
     done = ((t0 + t + 1) % H) == 0;
     const float donef = done ? 1.f : 0.f;
@@ -460,7 +546,9 @@ __global__ void __launch_bounds__(RT, 1) k_rollout(const RolloutArgs A, const Di
     // ---- advance: on done the next observation is the reset observation ------------------------------------------
     if (done) {
       ++episode;
-      if (rowthread)
+      if (rowthread && kind != IMB_ENV_SYNTH)
+        classic_reset(kind, A.env.seed, egid, (uint32_t)episode, OBSU + tid, RRS);
+      else if (rowthread)
         for (int k = 0; k < Do; ++k)
           OBSU[k * RRS + tid] = 0.1f * philox_normal(A.env.seed, IMB_STREAM_ENV_RESET, egid, (uint32_t)episode, k);
     } else if (rowthread) {
@@ -532,11 +620,15 @@ __global__ void __launch_bounds__(128) k_gae(float* __restrict__ rollout, int rw
   }
 }
 
-__global__ void k_env_reset(float* __restrict__ env_obs, int64_t E, int d_obs, uint64_t seed, int64_t id_off,
+__global__ void k_env_reset(float* __restrict__ env_obs, int64_t E, int d_obs, int kind, uint64_t seed, int64_t id_off,
                             const int64_t* __restrict__ state) {
   const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= E) return;
   const uint32_t ep = (uint32_t)state[IMB_ST_EPISODE];
+  if (kind != IMB_ENV_SYNTH) {
+    classic_reset(kind, seed, (uint32_t)(id_off + e), ep, env_obs + e, E);
+    return;
+  }
   for (int k = 0; k < d_obs; ++k)
     env_obs[(int64_t)k * E + e] = 0.1f * philox_normal(seed, IMB_STREAM_ENV_RESET, (uint32_t)(id_off + e), ep, k);
 }

@@ -17,14 +17,22 @@ class DeviceVecEnv:
 
     def __init__(self, d_obs: int, d_act: int, num_envs: int, *, discrete: bool = False, horizon: int = 1000,
                  seed: int = 0, env_id_offset: int = 0, device="cuda"):
+        self._init_env(_lib.ENV_SYNTH, d_obs, d_act, num_envs, discrete, horizon, seed, env_id_offset, device,
+                       spaces.Box(-np.inf, np.inf, (d_obs,), np.float32),
+                       spaces.Discrete(d_act) if discrete else spaces.Box(-1.0, 1.0, (d_act,), np.float32))
+        self.params = th.as_tensor(_desc.synth_env_params(d_obs, d_act, seed)).to(self.device)
+
+    def _init_env(self, kind: int, d_obs: int, d_act: int, num_envs: int, discrete: bool, horizon: int, seed: int,
+                  env_id_offset: int, device, observation_space, action_space) -> None:
+        """Everything but the env's parameters (`self.params`, the synthetic env's matrices; None for the
+        classic-control kinds, whose dynamics are fixed)."""
         self.num_envs = int(num_envs)
+        self.kind = kind
         self.d_obs, self.d_act, self.discrete, self.horizon, self.seed = d_obs, d_act, discrete, horizon, seed
-        self.observation_space = spaces.Box(-np.inf, np.inf, (d_obs,), np.float32)
-        self.action_space = spaces.Discrete(d_act) if discrete else spaces.Box(-1.0, 1.0, (d_act,), np.float32)
+        self.observation_space, self.action_space = observation_space, action_space
         self.device = th.device(device)
         self.desc = _lib.EnvDesc(d_obs=d_obs, d_act=d_act, discrete=int(discrete), horizon=horizon, seed=seed,
-                                 env_id_offset=env_id_offset)
-        self.params = th.as_tensor(_desc.synth_env_params(d_obs, d_act, seed)).to(self.device)
+                                 env_id_offset=env_id_offset, kind=kind)
         self.obs = th.zeros(d_obs, self.num_envs, device=self.device)  # SoA
         self.state = th.zeros(_lib.ST_WORDS, dtype=th.int64, device=self.device)
         self._reset_done = False

@@ -255,12 +255,20 @@ typedef struct imb_policy_desc {
   int32_t n_params;
 } imb_policy_desc;
 
-/* Synthetic MuJoCo-shaped environment (defined by this repo, SURVEY section 8d):
- * obs' = tanh(A obs + Bm u + c), reward = w.obs' - 0.1|u|^2, fixed horizon, auto-reset. */
+/* The environment the rollout kernels step, by kind; every kind is fixed-horizon with auto-reset:
+ *   IMB_ENV_SYNTH     the synthetic MuJoCo-shaped env (defined by this repo, SURVEY section 8d):
+ *                     obs' = tanh(A obs + Bm u + c), reward = w.obs' - 0.1|u|^2, parameters in env_params
+ *   IMB_ENV_CARTPOLE  seals/CartPole-v0: d_obs 4, Discrete(2), never terminates (DESIGN section 7e)
+ *   IMB_ENV_PENDULUM  Pendulum-v1: d_obs 3, Box(-2, 2, (1,)), never terminates (DESIGN section 7e)
+ * The classic-control kinds read no env_params; their observation is the whole env state. */
+#define IMB_ENV_SYNTH 0
+#define IMB_ENV_CARTPOLE 1
+#define IMB_ENV_PENDULUM 2
 typedef struct imb_env_desc {
   int32_t d_obs, d_act, discrete, horizon;
   uint64_t seed;
-  int64_t env_id_offset;    /* global id of this rank's env 0 (multi-GPU sharding) */
+  int32_t env_id_offset;    /* global id of this rank's env 0 (multi-GPU sharding) */
+  int32_t kind;             /* IMB_ENV_* */
 } imb_env_desc;
 
 typedef struct imb_ppo_hparams {
@@ -306,7 +314,9 @@ int imb_gae(float* rollout, int32_t rw, int32_t col_value, int64_t n_envs, int64
 /* advance EP_STEP/EPISODE/GLOBAL_STEP (+ ring header when ring_capacity > 0) after a rollout */
 int imb_rollout_advance(int64_t* state, int64_t n_envs, int64_t n_steps, int32_t horizon,
                         int64_t ring_capacity, void* stream);
-/* VecEnv.reset(): env_obs[d_obs][E] = 0.1 * N(0,1) from Philox(seed, env id, episode). */
+/* VecEnv.reset() from Philox stream IMB_STREAM_ENV_RESET keyed by seed at counter (env id, episode): env_obs[d_obs][E] =
+ * 0.1 * N(0,1) for the synthetic env, the kind's uniform reset draw for the classic-control ones (DESIGN section 7e).
+ * <0 when env's kind and shapes do not match. */
 int imb_env_reset(float* env_obs, int64_t n_envs, const imb_env_desc* env, const int64_t* state,
                   void* stream);
 
