@@ -33,6 +33,14 @@ STAT_KEYS = ("disc_loss", "disc_acc", "disc_acc_expert", "disc_acc_gen", "disc_e
              "disc_proportion_expert_true", "disc_proportion_expert_pred", "n_expert", "n_generated")
 
 
+def policy_norm_slots(demo_batch_size: int, demo_minibatch_size: int) -> int:
+    """Slots of the list that holds the policy feature-norm moments of GAIL's discriminator minibatches until they are
+    folded (`_policy_norm_side_effect`): 256, or one discriminator update's minibatches if that is more.  The list is
+    folded before an update that would overflow it, so one update must always fit; a full list would overwrite its
+    last slot and lose those moments."""
+    return max(256, demo_batch_size // demo_minibatch_size)
+
+
 def compute_train_stats(disc_logits_expert_is_high: th.Tensor, labels_expert_is_one: th.Tensor,
                         disc_loss: th.Tensor) -> Mapping[str, float]:
     """Torch restatement of common.py:27-92 for the generic (non-fused optimiser) path; the fused
@@ -220,7 +228,7 @@ class AdversarialTrainer(base.DemonstrationAlgorithm):
         # batch moments are computed beside the discriminator update and folded into the policy's statistics, in
         # order, once the PPO update (which updates the same statistics) has finished.
         self.reproduce_evaluate_actions_side_effect = True
-        self._pn_cap = 256
+        self._pn_cap = policy_norm_slots(self.demo_batch_size, self.demo_minibatch_size)
         self._pn_defer = None    # [4 + cap * (2 d_obs + 1)] slot list of deferred batch moments
         self._pn_pending = 0     # host mirror of the number of slots in use
         self._ev_fold = None

@@ -131,7 +131,7 @@ __global__ void __launch_bounds__(256, 6) k_norm_stats(NormJobs J, const float* 
     float* slot = nullptr;
     if (defer) {
       int s = (int)defer[0];
-      if (s >= defer_cap) s = defer_cap - 1;  // (host folds long before this; never overrun)
+      if (s >= defer_cap) s = defer_cap - 1;  // a full list: the last slot is overwritten (the host folds before this)
       slot = defer + 4 + (int64_t)s * (2 * Lj.din + 1);
     }
     const int32_t old_count = defer ? 0 : *Lj.cnt;
@@ -157,7 +157,7 @@ __global__ void __launch_bounds__(256, 6) k_norm_stats(NormJobs J, const float* 
     if (threadIdx.x == 0) {
       if (slot) {
         slot[2 * Lj.din] = (float)n;
-        defer[0] += 1.0f;
+        if (defer[0] < (float)defer_cap) defer[0] += 1.0f;  // saturates at defer_cap: a fold never reads past the list
       } else {
         *Lj.cnt = old_count + (int32_t)n;
       }
@@ -733,7 +733,9 @@ __global__ void __launch_bounds__(256) k_pref_loss(const float* __restrict__ rew
     const float lp = fmaxf(logf(p), -100.0f), l1p = fmaxf(log1pf(-p), -100.0f);
     const float loss = -(y * lp + (1.0f - y) * l1p);
     const float dl_dp = (p - y) / fmaxf(p * (1.0f - p), 1e-12f) * inv_P;
-    const float dp_dd = -(1.0f - noise_prob) * m * m * ed;  // = -(1 - noise) m (1 - m), without the cancellation in 1 - m
+    // = -(1 - noise) m (1 - m), without the cancellation in 1 - m; m (m e^d), not m m e^d: for |s| > 43.7 m m is
+    // subnormal and keeps only a few bits, while m e^d = 1 - m is never small
+    const float dp_dd = -(1.0f - noise_prob) * (m * (m * ed));
     const float g = clipped ? 0.f : grad_scale * dl_dp * dp_dd;  // d loss / d (returns difference)
     if (grad_rews) {
       float* g1 = grad_rews + (int64_t)pr * L;

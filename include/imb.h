@@ -124,7 +124,10 @@ int imb_disc_norm_update(const imb_disc_desc* d, const float* batch, int64_t ld,
  * PPO.train).  defer == NULL: fold into (norm_state = [mean | var], norm_count) immediately.  defer != NULL: append the
  * batch moments to the slot list `defer` ([0] = number of slots in use, [4 + k * (2 din + 1) ...] = mean | var | n) so that
  * the update can be computed on a stream that runs beside the PPO update and applied afterwards, in order, by
- * imb_norm_fold.  `d` / `ws`: any discriminator descriptor + its workspace (chunk partials live there). */
+ * imb_norm_fold.  The counter saturates at `defer_cap`: once the list is full, every further call overwrites the last
+ * slot and leaves [0] == defer_cap, so those batches' moments are lost but a fold never reads past the list.  A caller
+ * sizes the list for the most calls it makes between two folds.  `d` / `ws`: any discriminator descriptor + its
+ * workspace (chunk partials live there). */
 int imb_norm_batch_stats(const imb_disc_desc* d, const float* batch, int64_t ld, int64_t n, int row0, int din,
                                  float* norm_state, int32_t* norm_count, float* defer, int defer_cap, float* ws,
                                  void* stream);

@@ -61,7 +61,8 @@ def pref_loss_closed_form(rews: np.ndarray, prefs: np.ndarray, noise_prob=0.0, d
     computes for probability_port + binary_cross_entropy (:487-530, :1043-1090):
       d = clip(sum_t g^t (r2 - r1)),  m = 1 / (1 + e^d),  p = noise / 2 + (1 - noise) m
       d loss / d p = (p - y) / max(p (1 - p), 1e-12) / P           (torch's BCE backward, incl. its clamp)
-      d p / d d    = -(1 - noise) m^2 e^d                          (= -(1 - noise) m (1 - m) without the cancellation in 1 - m)
+      d p / d d    = -(1 - noise) m (m e^d)                        (= -(1 - noise) m (1 - m) without the cancellation in 1 - m,
+                                                                    and without the subnormal m^2 of |d| > 43.7)
       d d / d r2_t = g^t = -d d / d r1_t, and 0 where the return difference was clipped."""
     f = np.float32
     r = np.asarray(rews, dtype=f)
@@ -79,6 +80,6 @@ def pref_loss_closed_form(rews: np.ndarray, prefs: np.ndarray, noise_prob=0.0, d
     loss = float(np.mean(-(y * lp + (f(1) - y) * l1p)))
     acc = float(np.mean((p > 0.5) == (y > 0.5)))
     g = np.where(clipped, f(0), f(grad_scale) * (p - y) / np.maximum(p * (f(1) - p), f(1e-12)) / f(P)
-                 * (-(f(1) - f(noise_prob)) * m * m * ed)).astype(f)
+                 * (-(f(1) - f(noise_prob)) * (m * (m * ed)))).astype(f)
     grad = np.stack([-(g[:, None] * w[None, :]), g[:, None] * w[None, :]]).astype(f)
     return p, loss, acc, grad
