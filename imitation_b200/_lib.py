@@ -156,6 +156,12 @@ SIGNATURES = {
     "imb_bc_train": (_i32, [_pol, _i32, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _i64, _i32, _i32, _i64, _i64, _i32, _f32, _f32,
                             _f32, _f32, _i32, _ptr, _ptr, _ptr, _i32, _ptr, _ptr], 1),
     "imb_bc_plan": (_i32, [_pol, _i32, _i32], 0),
+    "imb_dqn_ring_store": (_i32, [_ptr, _i32, _ptr, _i64, _i64, _i64, _i32, _ptr, _ptr, _ptr], 1),
+    "imb_dqn_target": (_i32, [_pol, _i32, _ptr, _ptr, _i64, _ptr, _ptr, _i64, _ptr, _i64, _i64, _i64, _f32, _f32, _f32,
+                              _ptr, _i64, _ptr, _ptr], None),
+    "imb_dqn_step": (_i32, [_pol, _i32, _ptr, _ptr, _ptr, _ptr, _i32, _i64, _f32, _f32, _f32, _ptr, _i64, _ptr, _ptr],
+                     None),
+    "imb_dqn_plan": (_i32, [_pol, _i32, _i32], 0),
     "imb_policy_logp": (_i32, [_pol, _i32, _ptr, _ptr, _ptr, _i64, _i64, _i32, _ptr], 1),
     "imb_disc_reduce_adam": (_i32, [_disc, _adam, _ptr, _ptr, _ptr, _f32, _ptr, _ptr, _ptr, _ptr], 1),
     "imb_pref_loss": (_i32, [_ptr, _i64, _i32, _ptr, _f32, _f32, _f32, _f32, _ptr, _ptr, _ptr, _i32, _ptr], 1),
@@ -642,4 +648,42 @@ def bc_plan(pol: PolicyDesc, minibatch_size: int, act: int = ACT_TANH) -> int:
     rc = lib().imb_bc_plan(pol, act, minibatch_size)
     if rc < 0:
         raise ImbError(f"imb_bc_plan: {lib().imb_last_error().decode()} (rc={rc})")
+    return rc
+
+
+def dqn_ring_store(flat, tw, ring, positions, n_envs, n_steps, horizon, env_state, ring_state):
+    """Store a rollout's flat rows into the feature-major learner ring at SB3's (position, env) columns, position read
+    from and advanced in ring_state (imb_dqn_ring_store)."""
+    _check(lib().imb_dqn_ring_store(_p(flat, th.float32), tw, _p(ring, th.float32), positions, n_envs, n_steps, horizon,
+                                    _p(env_state, th.int64), _p(ring_state, th.int64), _stream()), "imb_dqn_ring_store")
+
+
+def dqn_target(pol, target_params, ring, ring_ld, ring_idx, expert, expert_ld, expert_idx, n_learner, n_expert, n_steps,
+               gamma, reward_learner, reward_expert, rows, step_base=0, state=None, act=ACT_RELU):
+    """TD rows obs | action index | y of n_steps minibatches (imb_dqn_target): learner rows from columns ring_idx of the
+    feature-major ring [tw][ring_ld], expert rows from columns expert_idx of the feature-major expert table, from TD
+    step state[ST_PPO_STEP] - step_base of the index lists on (state None: from step 0)."""
+    _check(lib().imb_dqn_target(pol, act, _p(target_params, th.float32), _p(ring, th.float32), ring_ld, _p(ring_idx, th.int64),
+                                _p(expert, th.float32), expert_ld, _p(expert_idx, th.int64), n_learner, n_expert, n_steps,
+                                gamma, reward_learner, reward_expert, _p(rows, th.float32), step_base,
+                                _p(state, th.int64), _stream()), "imb_dqn_target",
+           1 if n_steps * (n_learner + n_expert) > 0 else 0)
+
+
+def dqn_step(pol, q_params, exp_avg, exp_avg_sq, rows, batch_size, n_steps, lr, adam_eps, max_grad_norm, loss_log, state,
+             loss_base=0, act=ACT_RELU):
+    """n_steps DQN TD steps on the rows dqn_target wrote, in one launch (imb_dqn_step); loss_log float32 [rows][4] or
+    None, row k - 1 - loss_base for the step that brings state[ST_PPO_STEP] to k."""
+    _check(lib().imb_dqn_step(pol, act, _p(q_params, th.float32), _p(exp_avg, th.float32), _p(exp_avg_sq, th.float32),
+                              _p(rows, th.float32), batch_size, n_steps, lr, adam_eps, max_grad_norm,
+                              _p(loss_log, th.float32), loss_base, _p(state, th.int64), _stream()), "imb_dqn_step",
+           1 if n_steps > 0 else 0)
+
+
+def dqn_plan(pol: PolicyDesc, batch_size: int, act: int = ACT_RELU) -> int:
+    """PPO_PLAN_GEN1 / PPO_PLAN_GEN2: the kernel `dqn_step` runs for the Q-net `pol` at batch_size (host only);
+    ImbError naming the limit when the shape does not fit."""
+    rc = lib().imb_dqn_plan(pol, act, batch_size)
+    if rc < 0:
+        raise ImbError(f"imb_dqn_plan: {lib().imb_last_error().decode()} (rc={rc})")
     return rc

@@ -28,7 +28,7 @@ import torch as th
 from .. import _lib
 from ..data import rollout, serialize, types
 from ..util import logger as imit_logger
-from . import base, bc
+from . import base, bc, dqn
 
 
 class BetaSchedule(abc.ABC):
@@ -184,6 +184,8 @@ class InteractiveTrajectoryCollector:
         pin the expert's and the learner's sampling of every batch ([H][E][d_act] normals or [H][E] uniforms)."""
         env, learner = self.base, self.policy
         exp = rollout._policy_of(expert)
+        if isinstance(exp, dqn.DQNPolicy):  # SB3's QNetwork._predict takes the argmax whatever `deterministic` says
+            deterministic_policy = True
         ep, en, _ = exp.flat_vectors()
         lp, ln, _ = learner.flat_vectors()
         E, H, Do = env.num_envs, env.horizon, env.d_obs

@@ -1277,9 +1277,38 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update(const PpoArgs A, float* __
 }
 
 // ---- log pi(a|s) for the AIRL discriminator batch --------------------------------------------------------------
+// The pi tower of the policy's PolImg (staged in shared memory) on the inputs x[0, Do): lat = its last hidden layer.
+// ACT: the towers' activation (ACT_TANH: tanhf, ACT_RELU: fmaxf(z, 0)).
+template <int HP, int ACT>
+__device__ __forceinline__ void policy_tower(const float* __restrict__ smem, const PolImg& S, int Do,
+                                             const float* __restrict__ x, float (&lat)[HP]) {
+  const float* w1t = smem + S.w1p;
+  const float* w2t = smem + S.w2p;
+  float h1[HP];
+#pragma unroll
+  for (int j = 0; j < HP; ++j) h1[j] = smem[S.b1p + j];
+  for (int k = 0; k < Do; ++k) {
+    const float xv = x[k];
+#pragma unroll
+    for (int j = 0; j < HP; ++j) h1[j] = fmaf(w1t[k * HP + j], xv, h1[j]);
+  }
+#pragma unroll
+  for (int j = 0; j < HP; ++j) {
+    h1[j] = ACT == ACT_TANH ? tanhf(h1[j]) : fmaxf(h1[j], 0.f);
+    lat[j] = smem[S.b2p + j];
+  }
+#pragma unroll
+  for (int i = 0; i < HP; ++i) {
+    const float hv = h1[i];
+#pragma unroll
+    for (int j = 0; j < HP; ++j) lat[j] = fmaf(w2t[i * HP + j], hv, lat[j]);
+  }
+#pragma unroll
+  for (int j = 0; j < HP; ++j) lat[j] = ACT == ACT_TANH ? tanhf(lat[j]) : fmaxf(lat[j], 0.f);
+}
+
 // thread per batch column; obs rows [0,Do), act rows [Do, Do+Da_onehot) of the feature-major batch.  The pi tower, the
-// action head and log_std come from the policy's PolImg; then xn_ld >= Do inputs per thread.  ACT: the towers'
-// activation (ACT_TANH: tanhf, ACT_RELU: fmaxf(z, 0)).
+// action head and log_std come from the policy's PolImg; then xn_ld >= Do inputs per thread.
 template <int HP, int ACT>
 __global__ void __launch_bounds__(128) k_policy_logp(const imb_policy_desc pd, const float* __restrict__ params,
                                                     const float* __restrict__ norm, float* __restrict__ batch,
@@ -1290,8 +1319,6 @@ __global__ void __launch_bounds__(128) k_policy_logp(const imb_policy_desc pd, c
   const int tid = threadIdx.x;
   load_policy_img(smem, S, pd, HP, params, norm);
   __syncthreads();
-  const float* w1t = smem + S.w1p;
-  const float* w2t = smem + S.w2p;
   const float* wa = smem + S.wa;
   float* x = smem + xn_off + tid * xn_ld;
   for (int64_t col = (int64_t)blockIdx.x * blockDim.x + tid; col < n; col += (int64_t)gridDim.x * blockDim.x) {
@@ -1300,27 +1327,8 @@ __global__ void __launch_bounds__(128) k_policy_logp(const imb_policy_desc pd, c
       if (pd.has_norm) v = (v - norm[k]) / sqrtf(norm[Do + k] + pd.norm_eps);
       x[k] = v;
     }
-    float h1[HP], lat[HP];
-#pragma unroll
-    for (int j = 0; j < HP; ++j) h1[j] = smem[S.b1p + j];
-    for (int k = 0; k < Do; ++k) {
-      const float xv = x[k];
-#pragma unroll
-      for (int j = 0; j < HP; ++j) h1[j] = fmaf(w1t[k * HP + j], xv, h1[j]);
-    }
-#pragma unroll
-    for (int j = 0; j < HP; ++j) {
-      h1[j] = ACT == ACT_TANH ? tanhf(h1[j]) : fmaxf(h1[j], 0.f);
-      lat[j] = smem[S.b2p + j];
-    }
-#pragma unroll
-    for (int i = 0; i < HP; ++i) {
-      const float hv = h1[i];
-#pragma unroll
-      for (int j = 0; j < HP; ++j) lat[j] = fmaf(w2t[i * HP + j], hv, lat[j]);
-    }
-#pragma unroll
-    for (int j = 0; j < HP; ++j) lat[j] = ACT == ACT_TANH ? tanhf(lat[j]) : fmaxf(lat[j], 0.f);
+    float lat[HP];
+    policy_tower<HP, ACT>(smem, S, Do, x, lat);
     float logp = 0.f;
     if (!pd.discrete) {
       for (int a = 0; a < Da; ++a) {
@@ -1347,6 +1355,57 @@ __global__ void __launch_bounds__(128) k_policy_logp(const imb_policy_desc pd, c
       logp = chosen - (mx + logf(se));
     }
     batch[(int64_t)row_logp * ld + col] = logp;
+  }
+}
+
+// ---- DQN TD targets (imb_dqn_target) ----------------------------------------------------------------------------
+// The max-over-head output mode of the policy forward above, on the target Q-net: thread per TD row r = gs * B + i of
+// n_steps minibatches of B = n_l + n_e rows (learner rows first).  Row i < n_l reads column ring_idx[gs * n_l + i] of
+// the feature-major learner ring, the others column exp_idx[gs * n_e + i - n_l] of the expert table (both [tw][ld]
+// transition tables, Discrete actions one-hot).  y = r + ((1 - done) * gamma) * max_a Q_target(s')[a], each operation
+// rounded as torch rounds DQN.train's expression; the row written is obs | action index | y (rollout-row format).
+template <int HP, int ACT>
+__global__ void __launch_bounds__(128) k_dqn_target(const imb_policy_desc pd, const float* __restrict__ params,
+                                                   const float* __restrict__ ring, int64_t ring_ld,
+                                                   const int64_t* __restrict__ ring_idx, const float* __restrict__ expert,
+                                                   int64_t exp_ld, const int64_t* __restrict__ exp_idx, int64_t n_l,
+                                                   int64_t n_e, int64_t n, float gamma, float rew_l, float rew_e,
+                                                   float* __restrict__ out, int rw, int xn_off, int xn_ld,
+                                                   int64_t step_base, const int64_t* __restrict__ state) {
+  extern __shared__ __align__(128) float smem[];
+  const int Do = pd.d_obs, Da = pd.d_act, h = pd.hidden;
+  const PolImg S(Do, Da, HP);
+  const int tid = threadIdx.x;
+  load_policy_img(smem, S, pd, HP, params, nullptr);
+  __syncthreads();
+  const float* wa = smem + S.wa;
+  float* x = smem + xn_off + tid * xn_ld;
+  const int64_t B = n_l + n_e;
+  const int64_t s0 = state ? state[IMB_ST_PPO_STEP] - step_base : 0;  // TD steps of the sample lists already taken
+  for (int64_t r = (int64_t)blockIdx.x * blockDim.x + tid; r < n; r += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t gs = r / B + s0, i = r - (r / B) * B;
+    const bool learner = i < n_l;
+    const float* src = learner ? ring : expert;
+    const int64_t ld = learner ? ring_ld : exp_ld;
+    const int64_t col = learner ? ring_idx[gs * n_l + i] : exp_idx[gs * n_e + (i - n_l)];
+    for (int k = 0; k < Do; ++k) x[k] = src[(int64_t)(Do + Da + k) * ld + col];
+    float lat[HP];
+    policy_tower<HP, ACT>(smem, S, Do, x, lat);
+    float mx = -INFINITY;
+    int act = 0;
+    for (int a = 0; a < Da; ++a) {
+      float m = smem[S.ba + a];
+#pragma unroll
+      for (int j = 0; j < HP; ++j) m = (j < h) ? fmaf(wa[a * HP + j], lat[j], m) : m;
+      mx = fmaxf(mx, m);
+      if (src[(int64_t)(Do + a) * ld + col] > 0.5f) act = a;
+    }
+    const float done = src[(int64_t)(2 * Do + Da) * ld + col];
+    const float y = __fadd_rn(learner ? rew_l : rew_e, __fmul_rn(__fmul_rn(1.0f - done, gamma), mx));
+    float* o = out + r * rw;
+    for (int k = 0; k < Do; ++k) o[k] = src[(int64_t)k * ld + col];
+    o[Do] = (float)act;
+    o[Do + 1] = y;
   }
 }
 
@@ -1612,6 +1671,105 @@ extern "C" int imb_bc_train(const imb_policy_desc* pol, int32_t pol_act, float* 
   const int u = plan == IMB_PPO_PLAN_GEN1 ? 0 : 1;
   return launch_cluster(kernels[u][pol_act], names[u][pol_act], bytes, &attr_bytes[u][pol_act], (cudaStream_t)stream, A,
                         pol_params, pol_norm, pol_norm_count, exp_avg, exp_avg_sq, table, perm, nullptr, state, B);
+}
+
+extern "C" int imb_dqn_plan(const imb_policy_desc* pol, int32_t pol_act, int32_t batch_size) {
+  IMB_REQUIRE(pol->discrete, "the DQN step runs Discrete action spaces only");
+  IMB_REQUIRE(!pol->has_norm, "the DQN step runs Q-nets without a feature RunningNorm");
+  PpoArgs A = {};
+  A.pol = *pol;
+  A.hp.batch_size = batch_size;
+  size_t bytes;
+  const int rc = ppo_plan_shape(A, pol_act, "DQN");
+  return rc != 0 ? rc : gen_plan(A, &bytes, "DQN");
+}
+
+extern "C" int imb_dqn_step(const imb_policy_desc* pol, int32_t pol_act, float* q_params, float* exp_avg,
+                            float* exp_avg_sq, const float* rows, int32_t batch_size, int64_t n_steps, float lr,
+                            float adam_eps, float max_grad_norm, float* loss_log, int64_t loss_base, int64_t* state,
+                            void* stream) {
+  IMB_REQUIRE(n_steps >= 0 && n_steps * (int64_t)batch_size < (1ll << 31), "bad n_steps");
+  if (n_steps == 0) return 0;
+  PpoArgs A = {};
+  A.pol = *pol;
+  A.hp.batch_size = batch_size;
+  A.hp.n_epochs = 1;
+  A.hp.lr = lr;
+  A.hp.adam_eps = adam_eps;
+  A.hp.max_grad_norm = max_grad_norm;
+  A.n_rows = n_steps * batch_size;
+  const int plan = imb_dqn_plan(pol, pol_act, batch_size);
+  if (plan < 0) return plan;
+  size_t bytes;
+  ppo_plan_shape(A, pol_act, "DQN");
+  gen_plan(A, &bytes, "DQN");
+  static size_t attr_bytes[2][2] = {};
+  constexpr decltype(&k_ppo_update_gen<1, ACT_TANH, LOSS_DQN>) kernels[2][2] = {
+      {k_ppo_update_gen<1, ACT_TANH, LOSS_DQN>, k_ppo_update_gen<1, ACT_RELU, LOSS_DQN>},
+      {k_ppo_update_gen<2, ACT_TANH, LOSS_DQN>, k_ppo_update_gen<2, ACT_RELU, LOSS_DQN>}};
+  constexpr const char* names[2][2] = {{"k_ppo_update_gen<1, dqn>", "k_ppo_update_gen<1, relu, dqn>"},
+                                       {"k_ppo_update_gen<2, dqn>", "k_ppo_update_gen<2, relu, dqn>"}};
+  const int u = plan == IMB_PPO_PLAN_GEN1 ? 0 : 1;
+  BcArgs B = {};
+  B.j0 = loss_base;
+  return launch_cluster(kernels[u][pol_act], names[u][pol_act], bytes, &attr_bytes[u][pol_act], (cudaStream_t)stream, A,
+                        q_params, nullptr, nullptr, exp_avg, exp_avg_sq, rows, nullptr, loss_log, state, B);
+}
+
+template <int HP, int ACT>
+static int launch_dqn_target(const imb_policy_desc* pol, const float* params, const float* ring, int64_t ring_ld,
+                             const int64_t* ring_idx, const float* expert, int64_t exp_ld, const int64_t* exp_idx,
+                             int64_t n_l, int64_t n_e, int64_t n, float gamma, float rew_l, float rew_e, float* out,
+                             int rw, int64_t step_base, const int64_t* state, cudaStream_t st) {
+  auto al = [](int x) { return (x + 31) / 32 * 32; };
+  const int xn_off = al(PolImg(pol->d_obs, pol->d_act, HP).total), xn_ld = pol->d_obs | 1;
+  const size_t bytes = (size_t)(xn_off + al(128 * xn_ld)) * 4;
+  IMB_REQUIRE(bytes <= IMB_SMEM_MAX, "policy too large");
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(k_dqn_target<HP, ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, IMB_SMEM_MAX);
+    if (e != cudaSuccess) IMB_FAIL(-2, "cudaFuncSetAttribute(k_dqn_target): %s", cudaGetErrorString(e));
+    attr_set = true;
+  }
+  int64_t blocks = (n + 127) / 128;
+  const int64_t cap = (int64_t)imb_num_sms() * 2;
+  if (blocks > cap) blocks = cap;
+  k_dqn_target<HP, ACT><<<(int)blocks, 128, bytes, st>>>(*pol, params, ring, ring_ld, ring_idx, expert, exp_ld, exp_idx,
+                                                        n_l, n_e, n, gamma, rew_l, rew_e, out, rw, xn_off, xn_ld,
+                                                        step_base, state);
+  IMB_CHECK_LAUNCH("k_dqn_target");
+  return 0;
+}
+
+extern "C" int imb_dqn_target(const imb_policy_desc* pol, int32_t pol_act, const float* target_params,
+                              const float* ring, int64_t ring_ld, const int64_t* ring_idx, const float* expert,
+                              int64_t expert_ld, const int64_t* expert_idx, int64_t n_learner, int64_t n_expert,
+                              int64_t n_steps, float gamma, float reward_learner, float reward_expert, float* rows,
+                              int64_t step_base, const int64_t* state, void* stream) {
+  IMB_REQUIRE(pol_act == IMB_ACT_TANH || pol_act == IMB_ACT_RELU,
+              "pol_act must be IMB_ACT_TANH (0) or IMB_ACT_RELU (1), got %d", pol_act);
+  IMB_REQUIRE(pol->discrete && !pol->has_norm, "the DQN target runs Discrete Q-nets without a feature RunningNorm");
+  IMB_REQUIRE(pol->hidden >= 1 && pol->hidden <= 64, "policy tower width must be <= 64");
+  IMB_REQUIRE(n_learner >= 0 && n_expert >= 0 && n_steps >= 0, "bad row counts");
+  IMB_REQUIRE(n_learner == 0 || (ring != nullptr && ring_idx != nullptr), "learner rows need the ring and its indices");
+  IMB_REQUIRE(n_expert == 0 || (expert != nullptr && expert_idx != nullptr), "expert rows need the table and its indices");
+  const int64_t n = n_steps * (n_learner + n_expert);
+  if (n <= 0) return 0;
+  const int rw = imb_rollout_row_width(pol);
+  const cudaStream_t st = (cudaStream_t)stream;
+  if (pol_act == IMB_ACT_TANH)
+    return pol->hidden <= 32
+               ? launch_dqn_target<32, ACT_TANH>(pol, target_params, ring, ring_ld, ring_idx, expert, expert_ld,
+                                                 expert_idx, n_learner, n_expert, n, gamma, reward_learner,
+                                                 reward_expert, rows, rw, step_base, state, st)
+               : launch_dqn_target<64, ACT_TANH>(pol, target_params, ring, ring_ld, ring_idx, expert, expert_ld,
+                                                 expert_idx, n_learner, n_expert, n, gamma, reward_learner,
+                                                 reward_expert, rows, rw, step_base, state, st);
+  return pol->hidden <= 32
+             ? launch_dqn_target<32, ACT_RELU>(pol, target_params, ring, ring_ld, ring_idx, expert, expert_ld, expert_idx,
+                                               n_learner, n_expert, n, gamma, reward_learner, reward_expert, rows, rw, step_base, state, st)
+             : launch_dqn_target<64, ACT_RELU>(pol, target_params, ring, ring_ld, ring_idx, expert, expert_ld, expert_idx,
+                                               n_learner, n_expert, n, gamma, reward_learner, reward_expert, rows, rw, step_base, state, st);
 }
 
 template <int HP, int ACT>

@@ -27,7 +27,15 @@
 //     batch is carried between launches in BcArgs::carry); the optimiser step adds l2_weight * w to every gradient, then
 //     runs Adam without clip_grad_norm_ (no squared-norm exchange); the last, incomplete batch of a train() also steps;
 //   * the BCTrainingMetrics of every logged batch's last minibatch written to BcArgs::metrics.
-constexpr int LOSS_PPO = 0, LOSS_BC = 1;
+// A DQN step (LOSS_DQN: SB3 2.2 DQN.train, restated by oracle/sqil_port.py) is this kernel's step with
+//   * minibatch gs made of table rows [gs * mb, (gs + 1) * mb) (no permutation), each row obs | act (index) | y, y the TD
+//     target r + (1 - done) gamma max_a Q_target(s') that imb_dqn_target wrote before the launch;
+//   * the Q values = the pi tower + action head's outputs, dL/dQ_a = clamp(Q_a - y, -1, 1) / mb on the taken action and
+//     0 elsewhere (F.smooth_l1_loss, beta 1, mean); no value tower, entropy or ratio;
+//   * clip_grad_norm_ and Adam as PPO's, with the Adam bias corrections from the step count (as BC's), so that steps
+//     split over launches compute the same bits; loss_log[(k - 1 - B.j0) * 4] = the loss (the mean smooth L1) of the
+//     step that makes the Adam step count k: the row is read from the device, so that a captured launch replays exactly.
+constexpr int LOSS_PPO = 0, LOSS_BC = 1, LOSS_DQN = 2;
 struct BcArgs {
   int64_t j0, n_mb;    // minibatches [j0, j0 + n_mb) of the train() call's sequence (numbered from 0 in every train())
   int k;               // minibatches per optimiser batch: batch_size / minibatch_size
@@ -119,7 +127,8 @@ __device__ __forceinline__ float ppo_act_grad(float g, float a) {
   return ACT == ACT_TANH ? g * (1.0f - a * a) : (a > 0.f ? g : 0.f);
 }
 
-// PACT: the towers' activation (ACT names the shared-memory action tile below); LK: the loss, LOSS_PPO or LOSS_BC.  Under LOSS_BC
+// PACT: the towers' activation (ACT names the shared-memory action tile below); LK: the loss, LOSS_PPO, LOSS_BC or
+// LOSS_DQN (`rollout` = the TD rows, perm_in unused, A.n_rows = steps x mb).  Under LOSS_BC
 // `rollout` is the demonstration table, perm_in holds the permutations of the epochs from (j0 / (N / mb)) on, [epoch][N],
 // A.hp.ent_coef is ent_weight, and loss_log is unused.
 template <int U, int PACT, int LK = LOSS_PPO>
@@ -131,6 +140,8 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
                                                           float* __restrict__ loss_log, int64_t* __restrict__ state,
                                                           const BcArgs B) {
   constexpr bool BC = LK == LOSS_BC;
+  constexpr bool DQN = LK == LOSS_DQN;
+  constexpr bool NOV = BC || DQN;  // no value tower
   constexpr int HP = 32 * U;
   namespace cg = cooperative_groups;
   cg::cluster_group cluster = cg::this_cluster();
@@ -238,18 +249,22 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
     // ---- 0. the step's rollout rows, a clean gradient vector, Adam bias corrections ------------------------------
     for (int r = tid; r < (flush_only ? 0 : nb); r += PT) {
       int64_t idx;
-      if (perm_in) {
-        idx = perm_in[(int64_t)ep_now * N + start + r];
+      if constexpr (DQN) {
+        idx = start + r;
       } else {
-        const FeistelKey fk = feistel_key(A.seed, IMB_STREAM_PPO_PERM, (uint64_t)(perm_draw0 + ep_now), (uint64_t)N);
-        idx = (int64_t)feistel_perm(fk, (uint64_t)(start + r), (uint64_t)N);
+        if (perm_in) {
+          idx = perm_in[(int64_t)ep_now * N + start + r];
+        } else {
+          const FeistelKey fk = feistel_key(A.seed, IMB_STREAM_PPO_PERM, (uint64_t)(perm_draw0 + ep_now), (uint64_t)N);
+          idx = (int64_t)feistel_perm(fk, (uint64_t)(start + r), (uint64_t)N);
+        }
       }
       IDX[r] = (int)idx;
     }
     for (int i = tid; i < CL * S; i += PT) GP[i] = 0.f;
     if (rec && tid < RS_N * RG) RSL[tid] = 0.f;
     if (tid == PT - 1) {
-      if (BC) {  // from the step count alone, so that a train() split over launches computes the same bits
+      if (NOV) {  // from the step count alone, so that a train() split over launches computes the same bits
         b1pow = pow(0.9, (double)adam_step);
         b2pow = pow(0.999, (double)adam_step);
       } else {
@@ -314,7 +329,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
     const int npass = flush_only ? 0 : (nb + CL * RG - 1) / (CL * RG);
     for (int pass = 0; pass < npass; ++pass) {
       const int base = pass * (CL * RG) + crank * RG;  // first minibatch row of this CTA in this pass
-      const int rws = BC ? col_logp : rw;  // BC reads the obs | act columns only
+      const int rws = BC ? col_logp : DQN ? col_logp + 1 : rw;  // BC reads obs | act, DQN obs | act | y
       for (int e = tid; e < RG * rws; e += PT) {
         const int i = e / rws, c = e - i * rws, r = base + i;
         const bool rl = r < nb;
@@ -332,7 +347,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
         }
       }
       __syncthreads();
-      if (!BC || warp < 4) {  // (BC has no value tower)
+      if (!NOV || warp < 4) {  // (BC and DQN have no value tower)
         // warp = (tower, 4 own rows), lane = hidden unit(s) lane + 32 u; only __syncwarp() between the layers
         const int cnet = warp >> 2, r0 = 4 * (warp & 3);
         const int rr = lane >> 3, la = lane & 7;  // per-row parts: lane octet rr handles row r0 + rr
@@ -473,6 +488,21 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
             }
           }
           __syncwarp();
+          if constexpr (DQN) {
+            // smooth L1 (beta 1) between Q(s)[a] and y = LPO: its gradient clamp(d, -1, 1) / mb on the taken action
+            const int act = (int)ACT[lrow];
+            const float y = LPO[lrow];
+            for (int a = la; a < Da; a += 8) {
+              float g = 0.f;
+              if (live && a == act) {
+                const float d = MEAN[a * RG + lrow] - y, ad = fabsf(d);
+                l_pg += ad < 1.0f ? 0.5f * d * d : ad - 0.5f;
+                g = fminf(fmaxf(d, -1.0f), 1.0f) * inv_nb;
+              }
+              DM[a * RG + lrow] = g;
+              DLS[a * RG + lrow] = 0.f;
+            }
+          } else {
           const float adv = ADV[lrow], logp_old = LPO[lrow];
           float logp = 0.f, ent = 0.f;
           int act = 0;
@@ -552,6 +582,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
               DLS[a * RG + lrow] = 0.f;
             }
           }
+          }
           __syncwarp();
 #pragma unroll 2
           for (int a = 0; a < Da; ++a) {
@@ -611,7 +642,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
         const int o_w1 = net ? PL.w1[1] : PL.w1[0], o_b1 = net ? PL.b1[1] : PL.b1[0];
         const int o_w2 = net ? PL.w2[1] : PL.w2[0], o_b2 = net ? PL.b2[1] : PL.b2[0];
         float dz[16];
-        if (gj < h && (!BC || net == 0)) {
+        if (gj < h && (!NOV || net == 0)) {
           load16(dz, DZ2 + gj * RG);
           for (int i = wq; i < h; i += NWQ) GP[o_w2 + gj * ldh + i] += dot16r(dz, H1 + i * RG);
           if (wq == 0) GP[o_b2 + gj] += sum16(dz);
@@ -673,10 +704,11 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
         el += LOSS[c * 3 + 2];
       }
       pg *= inv_nb, vl *= inv_nb, el *= inv_nb;
-      loss_log[gs * 4 + 0] = pg;
-      loss_log[gs * 4 + 1] = vl;
-      loss_log[gs * 4 + 2] = el;
-      loss_log[gs * 4 + 3] = pg + A.hp.ent_coef * el + A.hp.vf_coef * vl;
+      const int64_t lrow = DQN ? adam_step - 1 - B.j0 : gs;
+      loss_log[lrow * 4 + 0] = pg;
+      loss_log[lrow * 4 + 1] = vl;
+      loss_log[lrow * 4 + 2] = el;
+      loss_log[lrow * 4 + 3] = pg + A.hp.ent_coef * el + A.hp.vf_coef * vl;
     }
     if constexpr (BC) {
       if (crank == 0 && tid == 0 && bc_log) {  // BCTrainingMetrics (bc.py:134-146)

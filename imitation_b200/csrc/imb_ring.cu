@@ -172,7 +172,43 @@ __global__ void k_sample_advance2(int64_t n, int64_t e_n, int64_t* e_state, int6
   expert_advance(e_state, n, e_n);
 }
 
+// ---- DQN learner ring (imb_dqn_ring_store) ---------------------------------------------------------------------
+// one block: copy the T x E flat rows of a rollout into the feature-major ring [tw][P * E] at SB3's column
+// ((pos + t) mod P) * E + e, pos = ring_state[RING_IDX], then advance pos by T and RING_N (= positions filled) as
+// SB3's ReplayBuffer.add does T times.  flat row of (e, t): flat_index(e, t, E, T, t0, H), t0 = env_state[EP_STEP]
+// (the rollout's first episode step: the call goes before imb_rollout_advance).
+__global__ void __launch_bounds__(256) k_dqn_ring_store(const float* __restrict__ flat, int tw, float* __restrict__ ring,
+                                                       int64_t P, int64_t E, int64_t T, int H,
+                                                       const int64_t* __restrict__ env_state,
+                                                       int64_t* __restrict__ ring_state) {
+  const int64_t pos = ring_state[IMB_ST_RING_IDX], t0 = env_state[IMB_ST_EP_STEP], C = P * E;
+  // with T > P a later step overwrites an earlier one at its position, as SB3's sequential adds do: only the last
+  // min(T, P) steps are written
+  const int64_t tskip = T > P ? T - P : 0, n = (T - tskip) * E * tw;
+  for (int64_t i = threadIdx.x; i < n; i += blockDim.x) {
+    const int64_t c = i % tw, te = i / tw, t = tskip + te / E, e = te % E;
+    const int64_t f = flat_index(e, t, E, T, t0, H);
+    ring[c * C + ((pos + t) % P) * E + e] = flat[f * tw + c];
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    ring_state[IMB_ST_RING_IDX] = (pos + T) % P;
+    const int64_t filled = ring_state[IMB_ST_RING_N] + T;
+    ring_state[IMB_ST_RING_N] = filled < P ? filled : P;
+  }
+}
+
 }  // namespace
+
+extern "C" int imb_dqn_ring_store(const float* flat, int32_t tw, float* ring, int64_t positions, int64_t n_envs,
+                                  int64_t n_steps, int32_t horizon, const int64_t* env_state, int64_t* ring_state,
+                                  void* stream) {
+  IMB_REQUIRE(positions >= 1 && n_envs >= 1 && n_steps >= 1 && horizon >= 1 && tw >= 1, "bad ring store shape");
+  k_dqn_ring_store<<<1, 256, 0, (cudaStream_t)stream>>>(flat, tw, ring, positions, n_envs, n_steps, horizon, env_state,
+                                                        ring_state);
+  IMB_CHECK_LAUNCH("k_dqn_ring_store");
+  return 0;
+}
 
 extern "C" int imb_table_store(float* table, int64_t capacity, int32_t d_obs, int32_t d_act, const float* obs,
                                const float* acts_f, const int64_t* acts_i, const float* next_obs,

@@ -60,7 +60,9 @@ struct RolloutMembers {
 // Exploration rollout (imb_rollout_explore, policies/exploration_wrapper.py): policy[t] = 1 makes step t a random-policy
 // step for every env (action_space.sample(): uniform on the Box [-1, 1], or a uniform action index), drawn from Philox
 // stream IMB_STREAM_EXPLORE keyed by `seed` at counter (env id, step0 + t, a / 4); with pinned noise the uniform is read
-// from the slot the policy step would read.
+// from the slot the policy step would read.  step0 < 0 reads both from the device, so that a captured launch replays
+// exactly: the counter is state[IMB_ST_GLOBAL_STEP] + t and the step's entry is policy[state[IMB_ST_GLOBAL_STEP] + t - g0]
+// with g0 = -1 - step0 (the global step the vector starts at).
 struct RolloutExplore {
   const uint8_t* policy;  // [T]: 0 = the wrapped policy, 1 = random
   uint64_t seed;
@@ -336,6 +338,9 @@ __global__ void __launch_bounds__(RT, 1) k_rollout(const RolloutArgs A, const Di
   const int64_t t0 = state[IMB_ST_EP_STEP];
   int64_t episode = state[IMB_ST_EPISODE];
   const int64_t gstep0 = state[IMB_ST_GLOBAL_STEP];
+  // exploration: the random-action counter of step 0 and the policy vector's entry of step 0 (RolloutExplore)
+  const int64_t xstep0 = MODE == RM_EXPLORE ? (Xp.step0 < 0 ? gstep0 : Xp.step0) : 0;
+  const int64_t xoff = MODE == RM_EXPLORE && Xp.step0 < 0 ? gstep0 - (-1 - Xp.step0) : 0;
   const uint32_t egid = (uint32_t)(A.env.env_id_offset + e);
   const int rw = A.rw;
   const int tw = 2 * Do + Da + 1;
@@ -380,7 +385,7 @@ __global__ void __launch_bounds__(RT, 1) k_rollout(const RolloutArgs A, const Di
   bool done = false;
   for (int64_t t = 0; t < T; ++t) {
     float* row = rollout + (e * T + t) * rw;
-    const bool rnd = MODE == RM_EXPLORE && Xp.policy[t] != 0;  // block-uniform: one entry per step
+    const bool rnd = MODE == RM_EXPLORE && Xp.policy[xoff + t] != 0;  // block-uniform: one entry per step
     // ---- policy: value tower, then pi tower (H2 ends up holding the pi latent) ------------------------------
     float value = 0.f;
     if (!rnd) {
@@ -399,7 +404,7 @@ __global__ void __launch_bounds__(RT, 1) k_rollout(const RolloutArgs A, const Di
       // random policy: action_space.sample() (exploration_wrapper.py:58-66)
       uint32_t k0, k1;
       philox_key(Xp.seed, IMB_STREAM_EXPLORE, k0, k1);
-      const uint32_t ctr = (uint32_t)(Xp.step0 + t);
+      const uint32_t ctr = (uint32_t)(xstep0 + t);
       if (!A.pol.discrete) {
         const float lo = -ahi, hi = ahi;  // the env's Box
         Philox4 r = {0u, 0u, 0u, 0u};

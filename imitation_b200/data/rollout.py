@@ -49,12 +49,15 @@ def make_sample_until(min_timesteps: Optional[int] = None, min_episodes: Optiona
 
 
 def _policy_of(policy):
+    """The device policy `policy` is or holds: an ActorCriticPolicy, or a DQN's Q-net policy (which acts greedily)."""
+    from ..algorithms import dqn
     from ..policies import base as policies
 
-    if isinstance(policy, policies.ActorCriticPolicy):
+    kinds = (policies.ActorCriticPolicy, dqn.DQNPolicy)
+    if isinstance(policy, kinds):
         return policy
     inner = getattr(policy, "policy", None)
-    if isinstance(inner, policies.ActorCriticPolicy):
+    if isinstance(inner, kinds):
         return inner
     raise TypeError("Policy must be an imitation_b200 ActorCriticPolicy or an algorithm holding one "
                     f"(host callables have no GPU path), got {type(policy)} instead")
@@ -64,7 +67,7 @@ def generate_trajectories(policy, venv, sample_until: GenTrajTerminationFn, rng:
                           deterministic_policy: bool = False) -> Sequence[types.TrajectoryWithRew]:
     """Roll `policy` in the device VecEnv until `sample_until` holds (unbiased, see module doc).  With a DAgger
     `InteractiveTrajectoryCollector` as `venv`, `policy` is the expert it collects demonstrations from."""
-    from ..algorithms import dagger
+    from ..algorithms import dagger, dqn
     from ..envs import synth
 
     if isinstance(venv, dagger.InteractiveTrajectoryCollector):
@@ -75,6 +78,8 @@ def generate_trajectories(policy, venv, sample_until: GenTrajTerminationFn, rng:
             raise TypeError("generate_trajectories on the GPU path needs a DeviceVecEnv")
         base = base.venv
     pol = _policy_of(policy)
+    if isinstance(pol, dqn.DQNPolicy):  # SB3's QNetwork._predict takes the argmax whatever `deterministic` says
+        deterministic_policy = True
     pp, pn, _ = pol.flat_vectors()
     E, H, Do = base.num_envs, base.horizon, base.d_obs
     rw = _lib.rollout_row_width(pol.desc)

@@ -416,6 +416,48 @@ int imb_bc_train(const imb_policy_desc* pol, int32_t pol_act, float* pol_params,
  * needed.  <0 (imb_last_error() names the shared-memory need and limit) when the shape does not fit. */
 int imb_bc_plan(const imb_policy_desc* pol, int32_t pol_act, int32_t minibatch_size);
 
+/* ---- DQN (SQIL's learner; SB3 2.2 DQN.train, restated by oracle/sqil_port.py) ------------------------------------------
+ * The Q-net is a policy image: the pi tower and the action head are SB3's QNetwork (Flatten -> Linear -> act -> Linear ->
+ * act -> Linear(h, n_actions)), the logits its Q values.  The value tower and value head are parameters no module owns,
+ * left at zero: their gradient is 0, so clip_grad_norm_ and Adam leave them at zero.  Discrete actions, no feature
+ * RunningNorm.
+ *
+ * imb_dqn_ring_store: the T steps of E envs an imb_rollout_explore just wrote as flat rows (flat_out, [E*T][tw]) into the
+ * learner ring in SB3's ReplayBuffer order: the ring is a feature-major transition table [tw][positions * n_envs]
+ * (tw = 2 d_obs + n_actions + 1, one-hot actions), step t of env e goes to column ((pos + t) mod positions) * n_envs + e
+ * with pos = ring_state[IMB_ST_RING_IDX]; then pos advances by n_steps (mod positions) and ring_state[IMB_ST_RING_N]
+ * (positions filled) by n_steps, capped at positions.  The flat row of (e, t) is the rollout's transition order from
+ * episode step env_state[IMB_ST_EP_STEP], so the call goes between the rollout and imb_rollout_advance.  One launch.
+ *
+ * imb_dqn_target: the TD rows of n_steps minibatches of B = n_learner + n_expert rows, in one launch of the policy
+ * forward's max-over-head mode on the TARGET Q-net.  Row r = s * B + i belongs to TD step k = s0 + s of the index lists,
+ * s0 = state[IMB_ST_PPO_STEP] - step_base (state NULL: s0 = 0): i < n_learner reads column ring_idx[k * n_learner + i]
+ * of the learner ring, else column expert_idx[k * n_expert + i - n_learner] of the expert table (both feature-major
+ * transition tables [tw][ld], one-hot actions).  rows[r] (imb_rollout_row_width floats) = obs | action index | y with
+ * y = reward + ((1 - done) * gamma) * max_a Q_target(next_obs)[a], reward = reward_learner or reward_expert, each operation
+ * rounded separately as torch rounds DQN.train's float32 expression.
+ * imb_dqn_step: n_steps TD steps on those rows as ONE launch of k_ppo_update_gen with the DQN loss (the PPO update's
+ * persistent cluster kernel): step s takes rows [s * B, (s + 1) * B), loss = F.smooth_l1_loss(Q(obs)[a], y) (beta 1,
+ * mean), backward (dL/dQ_a = clamp(Q_a - y, -1, 1) / B on the taken action), clip_grad_norm_(max_grad_norm), torch Adam
+ * (betas 0.9 / 0.999, lr, adam_eps; bias corrections from state[IMB_ST_PPO_STEP], which advances per step).
+ * loss_log (optional): element [(k - 1 - loss_base) * 4] = the loss of the step that brings state[IMB_ST_PPO_STEP] to k.
+ * state[IMB_ST_PPO_EPOCH] advances by one per call.
+ * Every per-call offset is read from the counter blocks, so a learn() iteration (rollout, ring store, advance, target
+ * pass, TD steps) can be captured in a CUDA graph and replayed.
+ * imb_dqn_plan: the kernel imb_dqn_step runs for `pol` at batch_size (IMB_PPO_PLAN_GEN1 or GEN2); host only; <0 naming
+ * the limit when the Q-net or batch does not fit. */
+int imb_dqn_ring_store(const float* flat, int32_t tw, float* ring, int64_t positions, int64_t n_envs, int64_t n_steps,
+                       int32_t horizon, const int64_t* env_state, int64_t* ring_state, void* stream);
+int imb_dqn_target(const imb_policy_desc* pol, int32_t pol_act, const float* target_params, const float* ring,
+                   int64_t ring_ld, const int64_t* ring_idx, const float* expert, int64_t expert_ld,
+                   const int64_t* expert_idx, int64_t n_learner, int64_t n_expert, int64_t n_steps, float gamma,
+                   float reward_learner, float reward_expert, float* rows, int64_t step_base, const int64_t* state,
+                   void* stream);
+int imb_dqn_step(const imb_policy_desc* pol, int32_t pol_act, float* q_params, float* exp_avg, float* exp_avg_sq,
+                 const float* rows, int32_t batch_size, int64_t n_steps, float lr, float adam_eps, float max_grad_norm,
+                 float* loss_log, int64_t loss_base, int64_t* state, void* stream);
+int imb_dqn_plan(const imb_policy_desc* pol, int32_t pol_act, int32_t batch_size);
+
 /* log pi(a|s) of the generator policy for the disc batch (common.py:476-519 ->
  * ActorCriticPolicy.evaluate_actions), written into the batch's last feature row. */
 int imb_policy_logp(const imb_policy_desc* pol, int32_t pol_act, const float* pol_params, const float* pol_norm,
@@ -536,6 +578,9 @@ int imb_ensemble_relabel(const imb_pref_unc_desc* d, float alpha, float* rollout
  * and value are 0, and the action is low + u (high - low) on the Box [-1, 1] or min(floor(u n), n - 1) for Discrete(n),
  * with u a uniform of Philox stream IMB_STREAM_EXPLORE keyed by explore_seed at counter (env id, explore_step0 + t,
  * a / 4) -- or, with noise != NULL, the value in the slot the policy step would read ([T][E][d_act] or [T][E]).
+ * explore_step0 < 0 reads the per-call scalars from the device, so that a captured launch replays exactly: the counter
+ * of step t is state[IMB_ST_GLOBAL_STEP] + t, and its entry is explore_policy[state[IMB_ST_GLOBAL_STEP] + t - g0] with
+ * g0 = -1 - explore_step0 (the global step the vector starts at).
  * Policy steps follow flags (IMB_RF_DETERMINISTIC: ExplorationWrapper(deterministic_policy=True)).  The env step, reward
  * relabel, env-reward column, terminal handling and flattened rows are imb_rollout's. */
 int imb_rollout_explore(const imb_env_desc* env, const float* env_params, float* env_obs,
