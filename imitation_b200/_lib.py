@@ -162,6 +162,13 @@ SIGNATURES = {
     "imb_dqn_step": (_i32, [_pol, _i32, _ptr, _ptr, _ptr, _ptr, _i32, _i64, _f32, _f32, _f32, _ptr, _i64, _ptr, _ptr],
                      None),
     "imb_dqn_plan": (_i32, [_pol, _i32, _i32], 0),
+    "imb_sac_plan": (_i32, [_i32, _i32, _i32, _i32], 0),
+    "imb_sac_ws_floats": (_i64, [_i32, _i32, _i32, _i32], 0),
+    "imb_sac_collect": (_i32, [_env, _ptr, _ptr, _i32, _ptr, _i64, _i64, _ptr, _ptr, _ptr, _i64, _i32, _u64, _ptr, _ptr],
+                        1),
+    "imb_sac_step": (_i32, [_i32, _i32, _i32, _i32, _f32, _f32, _f32, _f32, _i32, _f32, _f32, _f32, _f32, _i32, _u64, _ptr,
+                            _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _i64, _ptr, _ptr, _i64, _ptr, _i64, _i64, _ptr,
+                            _ptr, _ptr, _ptr], None),
     "imb_policy_logp": (_i32, [_pol, _i32, _ptr, _ptr, _ptr, _i64, _i64, _i32, _ptr], 1),
     "imb_disc_reduce_adam": (_i32, [_disc, _adam, _ptr, _ptr, _ptr, _f32, _ptr, _ptr, _ptr, _ptr], 1),
     "imb_pref_loss": (_i32, [_ptr, _i64, _i32, _ptr, _f32, _f32, _f32, _f32, _ptr, _ptr, _ptr, _i32, _ptr], 1),
@@ -687,3 +694,45 @@ def dqn_plan(pol: PolicyDesc, batch_size: int, act: int = ACT_RELU) -> int:
     if rc < 0:
         raise ImbError(f"imb_dqn_plan: {lib().imb_last_error().decode()} (rc={rc})")
     return rc
+
+
+SAC_STEP_LAUNCHES = 4  # kernels per SAC gradient step (imb_sac_step)
+SAC_DETERMINISTIC, SAC_PREDICT = 1, 2  # imb_sac_collect flags
+
+
+def sac_plan(d_obs: int, d_act: int, hidden: int, batch_size: int) -> None:
+    """Host only: ImbError naming the limit when the SAC kernels cannot run the shape (imb_sac_plan)."""
+    rc = lib().imb_sac_plan(d_obs, d_act, hidden, batch_size)
+    if rc < 0:
+        raise ImbError(f"imb_sac_plan: {lib().imb_last_error().decode()} (rc={rc})")
+
+
+def sac_ws_floats(d_obs: int, d_act: int, hidden: int, batch_size: int) -> int:
+    return lib().imb_sac_ws_floats(d_obs, d_act, hidden, batch_size)
+
+
+def sac_collect(env, env_params, env_obs, hidden, actor, n_envs, n_steps, flat_out, aux, random_steps, g0, flags,
+                seed, state):
+    """n_steps steps of n_envs Box envs with the SAC actor in one launch (imb_sac_collect): flat rows obs | buffer action |
+    next obs | done into flat_out, env rewards into aux; step t random when random_steps[global step + t - g0]; flags
+    SAC_DETERMINISTIC | SAC_PREDICT (evaluation: the env gets predict()'s action, which the rows record)."""
+    _check(lib().imb_sac_collect(env, _p(env_params), _p(env_obs, th.float32), hidden, _p(actor, th.float32), n_envs,
+                                 n_steps, _p(flat_out, th.float32), _p(aux, th.float32), _p(random_steps, th.uint8), g0,
+                                 int(flags), seed & 0xFFFFFFFFFFFFFFFF, _p(state, th.int64), _stream()),
+           "imb_sac_collect")
+
+
+def sac_step(hp: dict, actor, actor_m, actor_v, critic, critic_m, critic_v, critic_target, ent, ring, ring_ld, ring_idx,
+             expert, expert_ld, expert_idx, n_steps, step_base, loss_log, ws, state):
+    """n_steps SAC gradient steps (imb_sac_step).  hp: d_obs, d_act, hidden, batch_size, gamma, tau, lr, adam_eps,
+    auto_ent, ent_coef, target_entropy, reward_learner, reward_expert, target_update_interval, seed."""
+    _check(lib().imb_sac_step(hp["d_obs"], hp["d_act"], hp["hidden"], hp["batch_size"], hp["gamma"], hp["tau"], hp["lr"],
+                              hp["adam_eps"], int(hp["auto_ent"]), hp["ent_coef"], hp["target_entropy"],
+                              hp["reward_learner"], hp["reward_expert"], hp["target_update_interval"],
+                              hp["seed"] & 0xFFFFFFFFFFFFFFFF, _p(actor, th.float32), _p(actor_m, th.float32),
+                              _p(actor_v, th.float32), _p(critic, th.float32), _p(critic_m, th.float32),
+                              _p(critic_v, th.float32), _p(critic_target, th.float32), _p(ent, th.float32),
+                              _p(ring, th.float32), ring_ld, _p(ring_idx, th.int64), _p(expert, th.float32), expert_ld,
+                              _p(expert_idx, th.int64), n_steps, step_base, _p(loss_log, th.float32),
+                              _p(ws, th.float32), _p(state, th.int64), _stream()), "imb_sac_step",
+           SAC_STEP_LAUNCHES * max(int(n_steps), 0))

@@ -182,10 +182,12 @@ class LearnSchedule(NamedTuple):
 def learn_schedule(total_timesteps: int, n_envs: int, train_freq: int, gradient_steps: int, learning_starts: int,
                    batch_size: int, buffer_positions: int, pos: int, full: bool, n_expert: int,
                    target_update_interval: int, n_calls: int, exploration_rate: float, rate_fn,
-                   num_timesteps: int = 0) -> LearnSchedule:
+                   num_timesteps: int = 0, exploration_draws: bool = True) -> LearnSchedule:
     """The host pass of one learn(): every global-numpy draw in SB3's order (np.random.rand per step after
     learning_starts; per TD step the learner's randint(0, upper) and randint(0, n_envs), then the expert's randint(0,
-    n_expert)), the target-update calls, the exploration rates and the ring positions."""
+    n_expert)), the target-update calls, the exploration rates and the ring positions.  exploration_draws False (SAC,
+    which acts without epsilon-greedy draws): a step is random exactly before learning_starts, and the only draws are
+    the replay indices."""
     E, T, P = n_envs, train_freq, buffer_positions
     n_l, n_e = batch_size // 2, batch_size - batch_size // 2
     every = max(target_update_interval // E, 1)
@@ -196,6 +198,8 @@ def learn_schedule(total_timesteps: int, n_envs: int, train_freq: int, gradient_
         for _ in range(T):
             if num_timesteps < learning_starts:
                 explore.append(1)
+            elif not exploration_draws:
+                explore.append(0)
             else:
                 explore.append(1 if np.random.rand() < exploration_rate else 0)
             num_timesteps += E

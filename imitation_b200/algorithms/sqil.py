@@ -3,8 +3,13 @@
 `SQIL` trains a DQN (`algorithms.dqn.DeviceDQN`) whose replay buffer, `SQILReplayBuffer`, gives every learner
 transition reward 0 and draws half of each minibatch from the demonstrations, which have reward 1.  Both buffers live
 on the device: the learner ring as a feature-major transition table [tw][buffer_size] in SB3's (position, env) order,
-the demonstrations as a feature-major table uploaded once.  Only Discrete action spaces are supported: the reference's
-continuous-action SQIL trains SAC / TD3 / DDPG, which have no device port.
+the demonstrations as a feature-major table uploaded once.  With Discrete actions the learner is the device DQN and
+the action columns are one-hot; with Box actions it is the device SAC (`algorithms.sac.SAC`) and the action columns
+are the float actions.  TD3 and DDPG have no device port.
+
+As in the reference, the expert rows hold the demonstrations' actions as recorded (env scale, e.g. [-2, 2] on
+Pendulum-v1), while the learner rows hold SAC's buffer actions, scaled to [-1, 1]: `set_demonstrations` adds the
+demonstrations unscaled.
 """
 from typing import Any, Dict, List, NamedTuple, Optional, Tuple
 
@@ -15,7 +20,7 @@ from .. import _lib, spaces
 from ..data import rollout, types
 from ..util import logger as imit_logger
 from . import base as algo_base
-from . import dqn
+from . import dqn, sac
 
 
 def split_in_half(x: int) -> Tuple[int, int]:
@@ -36,11 +41,12 @@ class ExpertBuffer:
     """The demonstrations as SB3's ReplayBuffer(n_envs=1) holds them: observations / actions / next_observations
     [n][1][...], dones and rewards [n][1] (NumPy, host)."""
 
-    def __init__(self, obs, acts, next_obs, dones):
+    def __init__(self, obs, acts, next_obs, dones, discrete: bool = True):
         n = len(obs)
         self.buffer_size = n
         self.observations = np.asarray(obs, np.float32).reshape(n, 1, -1)
-        self.actions = np.asarray(acts).astype(np.int64).reshape(n, 1, 1)
+        self.actions = (np.asarray(acts).astype(np.int64).reshape(n, 1, 1) if discrete
+                        else np.asarray(acts, np.float32).reshape(n, 1, -1))
         self.next_observations = np.asarray(next_obs, np.float32).reshape(n, 1, -1)
         self.dones = np.asarray(dones, np.float32).reshape(n, 1)
         self.rewards = np.ones((n, 1), np.float32)
@@ -73,13 +79,17 @@ class SQILReplayBuffer:
                  n_envs: int = 1, optimize_memory_usage: bool = False):
         if optimize_memory_usage:
             raise NotImplementedError("optimize_memory_usage=True: the device ring stores next_obs beside obs")
-        if not spaces.is_discrete(action_space):
-            raise NotImplementedError(f"action space {action_space!r}: the device SQIL runs Discrete action spaces")
+        if not (spaces.is_discrete(action_space) or spaces.is_box(action_space)):
+            raise NotImplementedError(f"action space {action_space!r}: the device SQIL runs Discrete and Box action "
+                                      "spaces")
         self.observation_space, self.action_space = observation_space, action_space
         self.device = th.device("cuda" if device == "auto" else device)
         self.n_envs = int(n_envs)
         self.buffer_size = max(int(buffer_size) // self.n_envs, 1)
-        self.d_obs, self.n_actions = spaces.flat_dim(observation_space), int(action_space.n)
+        self.discrete = spaces.is_discrete(action_space)
+        # action columns: one-hot over n_actions (Discrete) or the d_act floats (Box)
+        self.d_obs = spaces.flat_dim(observation_space)
+        self.n_actions = int(action_space.n) if self.discrete else spaces.flat_dim(action_space)
         self.tw = 2 * self.d_obs + self.n_actions + 1
         self.capacity = self.buffer_size * self.n_envs
         self.ring = th.zeros(self.tw, self.capacity, device=self.device)
@@ -95,12 +105,15 @@ class SQILReplayBuffer:
         """Set the expert demonstrations to be injected when sampling; uploads them once as a feature-major table."""
         d = _transitions(demonstrations)
         n = len(d)
-        self.expert_buffer = ExpertBuffer(d.obs, d.acts, d.next_obs, d.dones)
+        self.expert_buffer = ExpertBuffer(d.obs, d.acts, d.next_obs, d.dones, self.discrete)
         table = np.zeros((self.tw, n), np.float32)
         Do, A = self.d_obs, self.n_actions
         table[:Do] = np.asarray(d.obs, np.float32).reshape(n, Do).T
-        acts = np.asarray(d.acts).astype(np.int64).reshape(n)
-        table[Do + acts, np.arange(n)] = 1.0
+        if self.discrete:
+            acts = np.asarray(d.acts).astype(np.int64).reshape(n)
+            table[Do + acts, np.arange(n)] = 1.0
+        else:  # the recorded actions, unscaled (the reference adds the demonstrations as they are)
+            table[Do:Do + A] = np.asarray(d.acts, np.float32).reshape(n, A).T
         table[Do + A:2 * Do + A] = np.asarray(d.next_obs, np.float32).reshape(n, Do).T
         table[2 * Do + A] = np.asarray(d.dones, np.float32).reshape(n)
         self.expert_table = th.as_tensor(table).to(self.device)
@@ -113,6 +126,8 @@ class SQILReplayBuffer:
 
     @property
     def actions(self) -> np.ndarray:
+        if not self.discrete:
+            return self._field(self.d_obs, self.n_actions)
         return self._field(self.d_obs, self.n_actions).argmax(-1)[..., None].astype(np.int64)
 
     @property
@@ -144,7 +159,10 @@ class SQILReplayBuffer:
         E, Do, A = self.n_envs, self.d_obs, self.n_actions
         col = np.zeros((self.tw, E), np.float32)
         col[:Do] = np.asarray(obs, np.float32).reshape(E, Do).T
-        col[Do + np.asarray(action).astype(np.int64).reshape(E), np.arange(E)] = 1.0
+        if self.discrete:
+            col[Do + np.asarray(action).astype(np.int64).reshape(E), np.arange(E)] = 1.0
+        else:
+            col[Do:Do + A] = np.asarray(action, np.float32).reshape(E, A).T
         col[Do + A:2 * Do + A] = np.asarray(next_obs, np.float32).reshape(E, Do).T
         col[2 * Do + A] = np.asarray(done, np.float32).reshape(E)
         self.ring[:, self.pos * E:(self.pos + 1) * E] = th.as_tensor(col).to(self.device)
@@ -156,7 +174,8 @@ class SQILReplayBuffer:
         Do, A = self.d_obs, self.n_actions
         x = table[:, th.as_tensor(cols, device=self.device)].t()
         n = len(cols)
-        return ReplayBufferSamples(x[:, :Do], x[:, Do:Do + A].argmax(1, keepdim=True), x[:, Do + A:2 * Do + A],
+        acts = x[:, Do:Do + A].argmax(1, keepdim=True) if self.discrete else x[:, Do:Do + A]
+        return ReplayBufferSamples(x[:, :Do], acts, x[:, Do + A:2 * Do + A],
                                    x[:, 2 * Do + A:], th.full((n, 1), reward, device=self.device))
 
     def sample(self, batch_size: int, env=None) -> ReplayBufferSamples:
@@ -174,8 +193,8 @@ class SQILReplayBuffer:
 
 
 class SQIL(algo_base.DemonstrationAlgorithm):
-    """Soft Q Imitation Learning (SQIL): a DQN trained on a buffer that mixes reward-0 learner transitions with
-    reward-1 demonstrations."""
+    """Soft Q Imitation Learning (SQIL): a DQN (Discrete actions) or a SAC (Box actions) trained on a buffer that mixes
+    reward-0 learner transitions with reward-1 demonstrations."""
 
     def __init__(self, *, venv, demonstrations, policy, custom_logger: Optional[imit_logger.HierarchicalLogger] = None,
                  rl_algo_class=dqn.DQN, rl_kwargs: Optional[Dict[str, Any]] = None):
@@ -185,9 +204,9 @@ class SQIL(algo_base.DemonstrationAlgorithm):
             raise ValueError("SQIL uses a custom replay buffer: 'replay_buffer_class' not allowed.")
         if "replay_buffer_kwargs" in rl_kwargs:
             raise ValueError("SQIL uses a custom replay buffer: 'replay_buffer_kwargs' not allowed.")
-        if rl_algo_class is not dqn.DeviceDQN:
+        if rl_algo_class not in (dqn.DeviceDQN, sac.SAC):
             raise NotImplementedError(f"rl_algo_class {getattr(rl_algo_class, '__name__', rl_algo_class)!r}: the "
-                                      "device SQIL trains DQN (SAC / TD3 / DDPG have no device port)")
+                                      "device SQIL trains DQN and SAC (TD3 / DDPG have no device port)")
         self.rl_algo = rl_algo_class(policy=policy, env=venv, replay_buffer_class=SQILReplayBuffer,
                                      replay_buffer_kwargs={"demonstrations": demonstrations}, **rl_kwargs)
         super().__init__(demonstrations=demonstrations, custom_logger=custom_logger)
@@ -200,5 +219,5 @@ class SQIL(algo_base.DemonstrationAlgorithm):
         self.rl_algo.learn(total_timesteps=total_timesteps, tb_log_name=tb_log_name, **kwargs)
 
     @property
-    def policy(self) -> dqn.DQNPolicy:
+    def policy(self):
         return self.rl_algo.policy

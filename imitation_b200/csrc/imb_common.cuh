@@ -121,6 +121,9 @@ __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, u
 #define IMB_STREAM_PPO_PERM 0x5005u
 #define IMB_STREAM_EXPLORE 0x7007u  // random-policy actions of the exploration rollout (0x6006: oracle expert policy)
 #define IMB_STREAM_DAGGER 0x8008u   // the learner's sampled actions in the DAgger rollout
+#define IMB_STREAM_SAC_ACT 0x9009u     // SAC collection: the actor's noise (imb_sac_collect)
+#define IMB_STREAM_SAC_RANDOM 0xA00Au  // SAC collection: the warm-up steps' action_space.sample()
+#define IMB_STREAM_SAC_STEP 0xB00Bu    // SAC gradient step: the actor's noise on s and s' (imb_sac_step)
 
 struct Philox4 {
   uint32_t x, y, z, w;

@@ -49,11 +49,12 @@ def make_sample_until(min_timesteps: Optional[int] = None, min_episodes: Optiona
 
 
 def _policy_of(policy):
-    """The device policy `policy` is or holds: an ActorCriticPolicy, or a DQN's Q-net policy (which acts greedily)."""
-    from ..algorithms import dqn
+    """The device policy `policy` is or holds: an ActorCriticPolicy, a DQN's Q-net policy (which acts greedily), or a
+    SAC's policy."""
+    from ..algorithms import dqn, sac
     from ..policies import base as policies
 
-    kinds = (policies.ActorCriticPolicy, dqn.DQNPolicy)
+    kinds = (policies.ActorCriticPolicy, dqn.DQNPolicy, sac.SACPolicy)
     if isinstance(policy, kinds):
         return policy
     inner = getattr(policy, "policy", None)
@@ -67,7 +68,7 @@ def generate_trajectories(policy, venv, sample_until: GenTrajTerminationFn, rng:
                           deterministic_policy: bool = False) -> Sequence[types.TrajectoryWithRew]:
     """Roll `policy` in the device VecEnv until `sample_until` holds (unbiased, see module doc).  With a DAgger
     `InteractiveTrajectoryCollector` as `venv`, `policy` is the expert it collects demonstrations from."""
-    from ..algorithms import dagger, dqn
+    from ..algorithms import dagger, dqn, sac
     from ..envs import synth
 
     if isinstance(venv, dagger.InteractiveTrajectoryCollector):
@@ -78,6 +79,8 @@ def generate_trajectories(policy, venv, sample_until: GenTrajTerminationFn, rng:
             raise TypeError("generate_trajectories on the GPU path needs a DeviceVecEnv")
         base = base.venv
     pol = _policy_of(policy)
+    if isinstance(pol, sac.SACPolicy):
+        return _sac_trajectories(pol, base, sample_until, rng, deterministic_policy)
     if isinstance(pol, dqn.DQNPolicy):  # SB3's QNetwork._predict takes the argmax whatever `deterministic` says
         deterministic_policy = True
     pp, pn, _ = pol.flat_vectors()
@@ -98,6 +101,35 @@ def generate_trajectories(policy, venv, sample_until: GenTrajTerminationFn, rng:
         _lib.rollout_advance(base.state, E, H, H, 0)
         base.host_ep_step = 0
         trajectories += batch_trajectories(base, tbl, flat, aux)
+        if sample_until(trajectories):
+            break
+    rng.shuffle(trajectories)
+    return trajectories
+
+
+def _sac_trajectories(pol, base, sample_until, rng, deterministic: bool) -> List[types.TrajectoryWithRew]:
+    """Whole episodes from reset of a SAC policy (imb_sac_collect in its predict mode, noise keyed by the env's seed):
+    as in the reference's evaluation, the env steps with `predict`'s action unscale(a), and that is the recorded
+    action."""
+    E, H, Do, Da = base.num_envs, base.horizon, base.d_obs, base.d_act
+    tw = 2 * Do + Da + 1
+    base.reset()
+    flat = th.zeros(E * H, tw, device=base.device)  # from t0 = 0: row e * H + t
+    aux = th.zeros(2 * E + 2 * E * H, device=base.device)
+    trajectories = []
+    while True:
+        flags = _lib.SAC_PREDICT | (_lib.SAC_DETERMINISTIC if deterministic else 0)
+        _lib.sac_collect(base.desc, base.params, base.obs, pol.hidden, pol.actor_flat(), E, H, flat, aux, None, 0,
+                         flags, base.seed, base.state)
+        _lib.rollout_advance(base.state, E, H, H, 0)
+        base.host_ep_step = 0
+        rows = flat.view(E, H, tw).cpu().numpy()
+        rews = aux[2 * E + E * H:].cpu().numpy().reshape(E, H)
+        for e in range(E):
+            obs = np.concatenate([rows[e, :, :Do], rows[e, -1:, Do + Da:2 * Do + Da]]).astype(np.float32)
+            acts = rows[e, :, Do:Do + Da].astype(np.float32)
+            trajectories.append(types.TrajectoryWithRew(obs=obs, acts=acts, infos=None, terminal=True,
+                                                        rews=rews[e].astype(np.float32)))
         if sample_until(trajectories):
             break
     rng.shuffle(trajectories)

@@ -458,6 +458,49 @@ int imb_dqn_step(const imb_policy_desc* pol, int32_t pol_act, float* q_params, f
                  float* loss_log, int64_t loss_base, int64_t* state, void* stream);
 int imb_dqn_plan(const imb_policy_desc* pol, int32_t pol_act, int32_t batch_size);
 
+/* ---- SAC (SQIL's continuous-action learner; SB3 2.2 SAC.train / collect_rollouts, restated by oracle/sac_port.py) -----
+ * Nets: ReLU MLPs [h, h], one flat fp32 vector each in nn.Linear order (weight [out][in], then bias):
+ *   actor          latent_pi.0 (Do -> h), latent_pi.2 (h -> h), mu (h -> Da), log_std (h -> Da)
+ *   critic/target  qf0.0 (Do + Da -> h), qf0.2 (h -> h), qf0.4 (h -> 1), then qf1 alike
+ * Envelope: 1 <= d_obs <= 64, 1 <= d_act <= 8, 1 <= hidden <= 256, 1 <= batch_size <= 256.
+ *
+ * imb_sac_collect: E envs (Box actions: Pendulum-v1 or the synthetic env) for T steps in one launch.  Step t of env e
+ * is a random step when random_steps[state[IMB_ST_GLOBAL_STEP] + t - g0] is 1 (random_steps NULL: none): u uniform
+ * from Philox stream IMB_STREAM_SAC_RANDOM keyed by seed at counter (env id, global step + t, a / 4), the sample
+ * lo + u (hi - lo); otherwise the actor's tanh(mean + std eps) (eps: normals of IMB_STREAM_SAC_ACT at counter (env id,
+ * global step + t, a / 4)), or tanh(mean) with flags & IMB_SAC_DETERMINISTIC.  The buffer action is scale(sample) or
+ * scale(unscale(tanh(..))), the env action unscale(buffer action), in SB3's float32 operation order; with flags &
+ * IMB_SAC_PREDICT (evaluation) the env action is predict()'s unscale(tanh(..)) and the row records it instead.  Flat row
+ * flat_index(e, t) of flat_out ([E*T][2 Do + Da + 1]) = obs | buffer action | next obs (terminal at the horizon) |
+ * done; the env reward goes to aux[2 E + E T + e T + t] (as imb_rollout_explore).  env_obs is read and written back;
+ * state is read only (imb_rollout_advance advances it).
+ *
+ * imb_sac_step: n_steps SAC gradient steps (ent_coef: the fixed coefficient when auto_ent is 0), four launches each (critic phase, critic reduce + Adam, actor phase, actor
+ * reduce + Adam + Polyak).  Step n = state[IMB_ST_PPO_STEP] (read on the device; advanced per step) takes minibatch
+ * k = n - step_base: rows b < B/2 from columns ring_idx[k * (B/2) + b] of the learner ring [tw][ring_ld], the others
+ * from columns expert_idx[k * (B - B/2) + b - B/2] of the expert table [tw][expert_ld] (feature-major, tw = 2 Do + Da +
+ * 1), rewards reward_learner / reward_expert.  The actor's noise on s / s' of row b: normals 0-7 / 8-15 of Philox stream
+ * IMB_STREAM_SAC_STEP keyed by seed at counter (b, n, chunk).  ent (auto_ent): [log_ent_coef, its Adam m, v].  Three
+ * torch Adams (betas 0.9 / 0.999, lr, adam_eps; bias corrections from n + 1); the critic targets get the Polyak update
+ * with tau at step s of the call when s % target_update_interval == 0.  loss_log (optional): row k = (critic_loss,
+ * actor_loss, ent_coef_loss, ent_coef).  ws: imb_sac_ws_floats floats.  Every per-step offset is read on the device, so
+ * the launches replay from a CUDA graph.
+ * imb_sac_plan: 0, or <0 naming the limit the shape exceeds (host only). */
+#define IMB_SAC_DETERMINISTIC 1
+#define IMB_SAC_PREDICT 2
+int imb_sac_plan(int32_t d_obs, int32_t d_act, int32_t hidden, int32_t batch_size);
+int64_t imb_sac_ws_floats(int32_t d_obs, int32_t d_act, int32_t hidden, int32_t batch_size);
+int imb_sac_collect(const imb_env_desc* env, const float* env_params, float* env_obs, int32_t hidden, const float* actor,
+                    int64_t n_envs, int64_t n_steps, float* flat_out, float* aux, const uint8_t* random_steps,
+                    int64_t g0, int32_t flags, uint64_t seed, const int64_t* state, void* stream);
+int imb_sac_step(int32_t d_obs, int32_t d_act, int32_t hidden, int32_t batch_size, float gamma, float tau, float lr,
+                 float adam_eps, int32_t auto_ent, float ent_coef, float target_entropy, float reward_learner,
+                 float reward_expert, int32_t target_update_interval, uint64_t seed, float* actor, float* actor_m,
+                 float* actor_v, float* critic, float* critic_m, float* critic_v, float* critic_target, float* ent,
+                 const float* ring, int64_t ring_ld,
+                 const int64_t* ring_idx, const float* expert, int64_t expert_ld, const int64_t* expert_idx,
+                 int64_t n_steps, int64_t step_base, float* loss_log, float* ws, int64_t* state, void* stream);
+
 /* log pi(a|s) of the generator policy for the disc batch (common.py:476-519 ->
  * ActorCriticPolicy.evaluate_actions), written into the batch's last feature row. */
 int imb_policy_logp(const imb_policy_desc* pol, int32_t pol_act, const float* pol_params, const float* pol_norm,
