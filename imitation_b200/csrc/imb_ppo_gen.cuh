@@ -34,7 +34,8 @@
 //     0 elsewhere (F.smooth_l1_loss, beta 1, mean); no value tower, entropy or ratio;
 //   * clip_grad_norm_ and Adam as PPO's, with the Adam bias corrections from the step count (as BC's), so that steps
 //     split over launches compute the same bits; loss_log[(k - 1 - B.j0) * 4] = the loss (the mean smooth L1) of the
-//     step that makes the Adam step count k: the row is read from the device, so that a captured launch replays exactly.
+//     step that makes the Adam step count k: the row is read from the device, so that a captured launch replays exactly;
+//   * of the state words only ST_PPO_STEP advances (no epoch count), so a split leaves the state a single launch leaves.
 constexpr int LOSS_PPO = 0, LOSS_BC = 1, LOSS_DQN = 2;
 struct BcArgs {
   int64_t j0, n_mb;    // minibatches [j0, j0 + n_mb) of the train() call's sequence (numbered from 0 in every train())
@@ -837,7 +838,7 @@ __global__ void __launch_bounds__(PT, 1) k_ppo_update_gen(const PpoArgs A, float
       state[IMB_ST_PPO_STEP] = kstop ? adam_step - 1 : adam_step;  // (the stopping step took no Adam step)
       if constexpr (BC) {  // the epochs the launch completed
         state[IMB_ST_PPO_EPOCH] = perm_draw0 + (B.j0 + B.n_mb) / steps_per_epoch - B.j0 / steps_per_epoch;
-      } else {
+      } else if constexpr (!DQN) {  // (DQN steps draw no permutations: a launch is not an epoch)
         state[IMB_ST_PPO_EPOCH] = perm_draw0 + (kstop ? ep_now + 1 : A.hp.n_epochs);
       }
     }

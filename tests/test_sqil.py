@@ -95,7 +95,23 @@ SCHEDULES = [  # n_envs, learning_starts, train_freq, gradient_steps, total, buf
 
 @pytest.mark.parametrize("E, ls, tf, gs, total, bs, tui", SCHEDULES)
 def test_learn_schedule_matches_sb3_loop(E, ls, tf, gs, total, bs, tui):
-    n_exp, B = 57, 33
+    _check_learn_schedule(E, ls, tf, gs, total, bs, tui, 33)
+
+
+@pytest.mark.parametrize("E, ls, tf, gs, total, bs, tui", SCHEDULES[2:4])
+def test_learn_schedule_without_learner_rows_matches_sb3_loop(E, ls, tf, gs, total, bs, tui):
+    """batch_size 1: no learner rows.  SB3 still calls randint(0, upper, size=0) and randint(0, n_envs, size=(0,)),
+    which return empty arrays and consume no draws; the schedule must make the same draws."""
+    np.random.seed(2)
+    empty = np.random.randint(0, 5, size=0), np.random.randint(0, high=4, size=(0,))
+    after = np.random.rand()
+    np.random.seed(2)
+    assert all(e.shape == (0,) for e in empty) and np.random.rand() == after
+    _check_learn_schedule(E, ls, tf, gs, total, bs, tui, 1)
+
+
+def _check_learn_schedule(E, ls, tf, gs, total, bs, tui, B):
+    n_exp = 57
     port = sqil_port.LearnLoopPort(n_envs=E, d_obs=1, n_expert=n_exp, buffer_size=bs, learning_starts=ls,
                                    batch_size=B, train_freq=tf, gradient_steps=gs, target_update_interval=tui,
                                    exploration_fraction=0.3)
@@ -119,6 +135,7 @@ def test_learn_schedule_matches_sb3_loop(E, ls, tf, gs, total, bs, tui):
     np.testing.assert_array_equal(calls[calls % every == 0], port.target_update_calls)
     n_td = len(port.samples)
     assert s1.learner_idx.shape[0] + s2.learner_idx.shape[0] == n_td > 0
+    assert s1.learner_idx.shape[1] == B // 2 and s1.expert_idx.shape[1] == B - B // 2
     lidx = np.concatenate([s1.learner_idx, s2.learner_idx])
     eidx = np.concatenate([s1.expert_idx, s2.expert_idx])
     for k, (bi, ei, xi) in enumerate(port.samples):

@@ -7,7 +7,9 @@ import numpy as np
 import pytest
 import torch as th
 from scipy import stats
+from torch import nn
 
+from imitation_b200 import _lib
 from oracle import classic_env as ce
 from oracle import exploration_port, sqil_port
 
@@ -116,6 +118,29 @@ def test_learner_ring_after_learn_follows_cartpole_the_random_stream_and_the_arg
     T, steps, P = 3, 1200, 256
     algo = _sqil(n_envs, learning_starts=300 * n_envs, buffer_size=P * n_envs, train_freq=T, learning_rate=0.0,
                  exploration_fraction=0.01, exploration_final_eps=0.5, seed=3)
+    _check_learner_ring(algo, n_envs, steps, P, lambda o, a: ce.cartpole_step(o, a)[0], 2e-6)
+
+
+@pytest.mark.parametrize("n_envs", [1, 4])
+def test_learner_ring_after_learn_follows_the_synthetic_env_the_random_stream_and_the_argmax(n_envs):
+    """The CartPole test above on envs.synth.DeviceVecEnv(17, 9, discrete=True) with a tanh [20, 20] Q-net: 399 steps
+    per env, horizon 100, a ring of 128 positions.  The transitions must follow oracle.synth_env's dynamics of the
+    one-hot control, and every stored action column be one-hot."""
+    from imitation_b200.envs import synth
+    from oracle import synth_env
+
+    T, steps, P, H = 3, 399, 128, 100
+    venv = synth.DeviceVecEnv(17, 9, n_envs, discrete=True, horizon=H, seed=5)
+    spec = synth_env.SynthEnvSpec(17, 9, discrete=True, horizon=H, seed=5)
+    algo = _sqil_synth(venv, learning_starts=150 * n_envs, buffer_size=P * n_envs, train_freq=T, learning_rate=0.0,
+                       exploration_fraction=0.01, exploration_final_eps=0.5, seed=3,
+                       policy_kwargs=dict(net_arch=[20, 20], activation_fn=nn.Tanh))
+    _check_learner_ring(algo, n_envs, steps, P, lambda o, a: spec.dynamics(o, a)[0], 2e-5)
+    cols = algo.rl_algo.replay_buffer._field(17, 9)
+    assert set(np.unique(cols)) == {0.0, 1.0} and (cols.sum(-1) == 1).all(), "action columns not one-hot"
+
+
+def _check_learner_ring(algo, n_envs, steps, P, step_fn, atol):
     dq = algo.rl_algo
     np.random.seed(7)
     algo.train(total_timesteps=steps * n_envs)
@@ -123,14 +148,17 @@ def test_learner_ring_after_learn_follows_cartpole_the_random_stream_and_the_arg
     buf = dq.replay_buffer
     assert buf.full and buf.pos == steps % P
     assert int(buf.ring_state[0]) == buf.pos
+    Do, A = dq.env.d_obs, dq.env.d_act
     obs, acts, nobs, dones = buf.observations, buf.actions[..., 0], buf.next_observations, buf.dones
-    nxt, _ = ce.cartpole_step(obs.reshape(-1, 4), acts.reshape(-1))
-    np.testing.assert_allclose(nxt, nobs.reshape(-1, 4), rtol=0, atol=2e-6)
+    nxt = step_fn(obs.reshape(-1, Do), acts.reshape(-1))
+    np.testing.assert_allclose(nxt, nobs.reshape(-1, Do), rtol=0, atol=atol)
     explore = dq.last_schedule.explore
-    u = exploration_port.random_uniforms(dq._explore_seed(), np.arange(n_envs), 0, steps, 2, True)
-    want_rand = np.minimum(np.floor(u * np.float32(2)).astype(np.int64), 1)
-    q = sqil_port.q_forward(_params64(dq.policy.q_flat(), dq.policy), obs.reshape(-1, 4).astype(np.float64))[2]
-    q = q.reshape(P, n_envs, 2)
+    u = exploration_port.random_uniforms(dq._explore_seed(), np.arange(n_envs), 0, steps, A, True)
+    want_rand = np.minimum(np.floor(u * np.float32(A)).astype(np.int64), A - 1)
+    relu = dq.policy.act == _lib.ACT_RELU
+    q = sqil_port.q_forward(_params64(dq.policy.q_flat(), dq.policy), obs.reshape(-1, Do).astype(np.float64), relu)[2]
+    q = q.reshape(P, n_envs, A)
+    top2 = np.sort(q, -1)[..., -2:]
     H = dq.env.horizon
     n_rand = n_greedy = n_done = 0
     for g in range(steps - P, steps):  # the steps the ring still holds
@@ -139,7 +167,7 @@ def test_learner_ring_after_learn_follows_cartpole_the_random_stream_and_the_arg
             np.testing.assert_array_equal(acts[p], want_rand[g])
             n_rand += 1
         else:
-            clear = np.abs(q[p, :, 0] - q[p, :, 1]) > 1e-4  # (a near tie may round either way in float32)
+            clear = top2[p, :, 1] - top2[p, :, 0] > 1e-4  # (a near tie may round either way in float32)
             np.testing.assert_array_equal(acts[p][clear], q[p].argmax(1)[clear])
             n_greedy += int(clear.sum())
         done = (g + 1) % H == 0
@@ -159,17 +187,60 @@ def test_sqil_train_matches_the_sb3_loop_replayed_in_float64(n_envs):
     with the target copied at the loop's target-update calls."""
     kw = dict(learning_starts=60, learning_rate=1e-3, batch_size=33, target_update_interval=24, buffer_size=10_000,
               seed=11, exploration_fraction=0.5)
-    total = 240 * n_envs
-    algo = _sqil(n_envs, **kw)
+    _check_train_against_the_sb3_loop(_sqil(n_envs, **kw), kw, [240 * n_envs])
+
+
+@pytest.mark.parametrize("batch_size", [33, 1])
+@pytest.mark.parametrize("n_envs", [1, 4])
+def test_two_sqil_trains_on_a_synthetic_env_match_the_sb3_loop_replayed_in_float64(n_envs, batch_size):
+    """The test above off CartPole: envs.synth.DeviceVecEnv(17, 9, discrete=True), a tanh [20, 20] Q-net, and two
+    consecutive train() calls.  The second starts at a TD step count above 0, so the Adam step count carries over, its
+    loss rows are offset and k_dqn_target reads its index lists at s0 = state - step_base > 0.  batch_size 1 has no
+    learner rows: every TD step is one expert row."""
+    from imitation_b200.envs import synth
+
+    kw = dict(learning_starts=60, learning_rate=1e-3, batch_size=batch_size, target_update_interval=24,
+              buffer_size=10_000, seed=11, exploration_fraction=0.5,
+              policy_kwargs=dict(net_arch=[20, 20], activation_fn=nn.Tanh))
+    algo = _sqil_synth(synth.DeviceVecEnv(17, 9, n_envs, discrete=True, horizon=70, seed=5), **kw)
+    _check_train_against_the_sb3_loop(algo, kw, [240 * n_envs, 150 * n_envs])
+
+
+def _sqil_synth(venv, **rl_kwargs):
+    """SQIL on a synthetic Discrete env with 300 expert transitions drawn from the env's own dynamics."""
+    from imitation_b200.algorithms import sqil
+    from imitation_b200.data import types
+    from oracle import synth_env
+
+    spec = synth_env.SynthEnvSpec(venv.d_obs, venv.d_act, discrete=True, horizon=venv.horizon, seed=venv.seed)
+    r = np.random.default_rng(0)
+    obs = r.standard_normal((300, venv.d_obs)).astype(np.float32) * 0.5
+    acts = r.integers(0, venv.d_act, 300)
+    demos = types.Transitions(obs=obs, acts=acts, infos=np.array([{}] * 300), next_obs=spec.dynamics(obs, acts)[0],
+                              dones=r.random(300) < 0.1)
+    return sqil.SQIL(venv=venv, demonstrations=demos, policy="MlpPolicy", rl_kwargs=rl_kwargs)
+
+
+def _check_train_against_the_sb3_loop(algo, kw, totals):
+    """Run algo.train(total) for each total, then walk SB3's loop over the same totals from the same NumPy seed,
+    replaying every TD step in float64 on the rows of the device's buffers, with the target copied at the loop's
+    target-update calls; the Q-net, its target and every learn()'s losses must agree."""
     dq = algo.rl_algo
+    E, Do, A = dq.n_envs, dq.env.d_obs, dq.env.d_act
+    relu = dq.policy.act == _lib.ACT_RELU
     p64 = _params64(dq.policy.q_flat(), dq.policy)
     np.random.seed(123)
-    algo.train(total_timesteps=total)
+    dev_losses, explore = [], []
+    for total in totals:
+        algo.train(total_timesteps=total)
+        dev_losses.append(dq._last_losses.cpu().numpy())
+        explore.append(dq.last_schedule.explore)
     buf = dq.replay_buffer
     ring = buf.ring.double().cpu().numpy()
     expert = buf.expert_table.double().cpu().numpy()
-    port = sqil_port.LearnLoopPort(n_envs=n_envs, d_obs=4, n_expert=buf.n_expert, buffer_size=kw["buffer_size"],
-                                   learning_starts=kw["learning_starts"], batch_size=33,
+    B = kw["batch_size"]
+    port = sqil_port.LearnLoopPort(n_envs=E, d_obs=Do, n_expert=buf.n_expert, buffer_size=kw["buffer_size"],
+                                   learning_starts=kw["learning_starts"], batch_size=B,
                                    target_update_interval=kw["target_update_interval"],
                                    exploration_fraction=kw["exploration_fraction"])
     pt64 = {k: x.copy() for k, x in p64.items()}
@@ -179,31 +250,36 @@ def test_sqil_train_matches_the_sb3_loop_replayed_in_float64(n_envs):
 
     def train_fn(sample):
         bi, ei, xi = sample
-        src = np.concatenate([ring[:, bi * n_envs + ei], expert[:, xi]], 1)
-        y = sqil_port.td_targets(pt64, src[6:10].T, src[10], np.r_[np.zeros(len(bi)), np.ones(len(xi))], 0.99)
+        src = np.concatenate([ring[:, bi * E + ei], expert[:, xi]], 1)
+        y = sqil_port.td_targets(pt64, src[Do + A:2 * Do + A].T, src[2 * Do + A],
+                                 np.r_[np.zeros(len(bi)), np.ones(len(xi))], 0.99, relu)
         step[0] += 1
-        losses.append(sqil_port.td_step(p64, m64, v64, step[0], src[:4].T, src[4:6].argmax(0), y, 1e-3, 10.0))
+        losses[-1].append(sqil_port.td_step(p64, m64, v64, step[0], src[:Do].T, src[Do:Do + A].argmax(0), y,
+                                            kw["learning_rate"], 10.0, relu=relu))
 
     def target_fn():
         for k in p64:
             pt64[k] = p64[k].copy()
 
     np.random.seed(123)
-    port.learn(total, train_fn=train_fn, target_fn=target_fn)
-    assert dq._n_updates == port._n_updates == len(losses) > 0
+    for total in totals:
+        losses.append([])
+        port.learn(total, train_fn=train_fn, target_fn=target_fn)
+    n = step[0]
+    assert dq._n_updates == port._n_updates == n > 0 and all(losses)
     assert dq._n_calls == port._n_calls
     assert dq.exploration_rate == port.exploration_rate
-    np.testing.assert_array_equal(dq.last_schedule.explore, port.random_steps)
+    np.testing.assert_array_equal(np.concatenate(explore), port.random_steps)
     got = _params64(dq.policy.q_flat(), dq.policy)
     for k in sqil_port.KEYS:
-        np.testing.assert_allclose(got[k], p64[k], rtol=0, atol=1e-3 * 1e-3 * len(losses) + 1e-6)
+        np.testing.assert_allclose(got[k], p64[k], rtol=0, atol=1e-3 * kw["learning_rate"] * n + 1e-6)
     got_t = _params64(dq.policy.target_flat(), dq.policy)
     for k in sqil_port.KEYS:
-        np.testing.assert_allclose(got_t[k], pt64[k], rtol=0, atol=1e-3 * 1e-3 * len(losses) + 1e-6)
-    dev_losses = dq._last_losses.cpu().numpy()
-    np.testing.assert_allclose(dev_losses, losses, rtol=1e-3, atol=1e-5)
-    assert dq._last_logged["train/n_updates"] == len(losses)
-    assert abs(dq._last_logged["train/loss"] - losses[-1]) <= 1e-3 * max(1.0, abs(losses[-1]))
+        np.testing.assert_allclose(got_t[k], pt64[k], rtol=0, atol=1e-3 * kw["learning_rate"] * n + 1e-6)
+    for d, l in zip(dev_losses, losses):
+        np.testing.assert_allclose(d, l, rtol=1e-3, atol=1e-5)
+    assert dq._last_logged["train/n_updates"] == n
+    assert abs(dq._last_logged["train/loss"] - losses[-1][-1]) <= 1e-3 * max(1.0, abs(losses[-1][-1]))
     assert dq._last_logged["rollout/exploration_rate"] == port.exploration_rate
 
 
